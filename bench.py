@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — GP fit + batched query throughput on B200 (BASELINE.json's metric).
+"""bench.py — GP fit + batched query throughput on H100 (BASELINE.json's metric).
 
 One "step" = one pass of the hot path over one batch of synthetic input:
     fit  : K-build (N x N) -> blocked Cholesky -> alpha            (model/gp.hpp:550-571)
     query: M UCB candidates: K*, L^-1 K*, mu, sigma^2, UCB, argmax (gp.hpp:159-167, acqui/ucb.hpp:83-90)
 at N = 16384, D = 6, SquaredExpARD, fp64, M = 10000 (SURVEY.md §8d (i)).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...] [--dump-outputs DIR]
 
 `value`   : steps/s with inputs already resident in HBM (device-pointer ABI), CUDA events on the library's stream.
 `e2e`     : the same step through the public host API (limbo_b200.model.GP.compute + acqui.UCB.argmax_batch /
@@ -21,8 +21,14 @@ N > 1     : STRONG scaling of the same global job.  The fit is DISTRIBUTED (limb
 `config4` / `config5`: sub-records for the two multi-GPU splits BASELINE.json names (1M EI candidates in tf32 sharded over
             the ranks; N = 65536 panel-broadcast Cholesky), measured in the same run at the same N.
 `cpu_baseline` / `--impl reference`: the reference's own gp.hpp / ucb.hpp loops (oracle/_ref/libref_gp.so, compiled from
-            /root/reference against the Eigen stand-in) when that library is present, else the oracle port; on the host
+            the reference's sources against the Eigen stand-in) when that library is present, else the oracle port; on the host
             cores, on a bounded sample extrapolated to the full size (stated in `sample`).
+--dump-outputs DIR: after the timed steps, what the last timed step handed back is written as DIR/<name>.npy (float64):
+            best_value and best_index (the global argmax of the acquisition over all candidates, as every rank receives it) and
+            alpha (N x 1, the fitted model).  Headline workloads of the GPU arm only.
+            Inputs are seeded, so two builds run with the same arguments can be compared output for output.
+The library must have been built (__graft_entry__.build()): bench.py compiles nothing and writes nothing into the tree, so that it
+can run from a read-only checkout, and it refuses a library whose build stamp does not match the current sources.
 """
 from __future__ import annotations
 
@@ -63,7 +69,7 @@ def workload_config(n_gpus: int) -> dict:
         "parallelism": (f"fit distributed over {n_gpus} GPUs (1-D block-cyclic 256-column panels, one NCCL broadcast per panel, factor assembled on "
                         f"every rank), {M_CAND} candidates sharded x{n_gpus} (<= {per} each), one all_gather of 16-byte records for the argmax"
                         if n_gpus > 1 else "single GPU"),
-        "l2": "inputs larger than L2 (factor 2.1 GB, K* / V 1.3 GB vs 126 MB L2); no explicit flush",
+        "l2": "inputs larger than L2 (factor 2.1 GB, K* / V 1.3 GB vs 50 MB L2); no explicit flush",
         "hyperparams": "reference defaults: log ell_d = 0, log sigma_f = 0, noise 0.01, UCB alpha 0.5, mean::Data",
         "seeds": {"data": 1234, "candidates": 1235},
     }
@@ -257,7 +263,7 @@ def pick_cpu_sample(budget_s: float, threads: int):
 
 
 def sample_text(kind: str, s: dict, n_s: int, m_s: int, threads: int) -> str:
-    what = ("the reference's own gp.hpp / acqui/ucb.hpp loops (oracle/_ref/libref_gp.so: /root/reference headers over an Eigen stand-in with "
+    what = ("the reference's own gp.hpp / acqui/ucb.hpp loops (oracle/_ref/libref_gp.so: the reference's headers over an Eigen stand-in with "
             "Eigen's blocked-LLT structure)" if kind == "reference" else "oracle port of the reference path")
     return (f"{what}: fit at N={n_s} on 1 thread like Eigen::LLT ({s['t_fit']:.2f} s) + {m_s} one-at-a-time UCB queries over {threads} threads "
             f"({s['t_query']:.2f} s); extrapolated to N={N_TRAIN}, M={M_CAND}: {s['fit_model']} -> {s['sec_fit']:.0f} s, queries by M*N^2 -> "
@@ -320,14 +326,10 @@ def syrk_flops_per_fit(n: int) -> float:
 
 
 def fp64_tensor_peak() -> tuple[float, str]:
-    p = os.path.join(ROOT, "profiles", "fp64_peaks.json")
-    if os.path.exists(p):
-        try:
-            j = json.load(open(p))
-            return float(j["dmma_tflops"]), f"builder-measured DMMA peak ({j.get('source', 'tools/microbench.cu')}); MEASURED_PEAKS.json has no fp64 figure"
-        except Exception:
-            pass
-    return 40.0, "nominal B200 fp64 tensor peak (40 TFLOP/s); MEASURED_PEAKS.json has no fp64 figure"
+    mp = measured_peaks()
+    if "fp64_tflops" in mp:
+        return float(mp["fp64_tflops"]), "measured (MEASURED_PEAKS.json fp64_tflops)"
+    return 67.0, "H100 SXM data sheet fp64 tensor peak (67 TFLOP/s at 700 W; not a measured figure)"
 
 
 def measured_peaks() -> dict:
@@ -338,24 +340,11 @@ def measured_peaks() -> dict:
         return {}
 
 
-def ncu_traffic(kernel: str):
-    """DRAM bytes of one captured launch (ncu --set full), from the committed profile summaries (latest round first)."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        try:
-            j = json.load(open(os.path.join(ROOT, "profiles", name)))[kernel]
-            j = dict(j)
-            j["source"] = "profiles/" + name
-            return j["dram_bytes"], j
-        except Exception:
-            continue
-    return None, None
-
-
 def hbm_peak() -> tuple[float, str]:
     mp = measured_peaks()
     if "hbm_gbs" in mp:
         return float(mp["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (3.35 TB/s; not a measured figure)"
 
 
 def prof_api(lib):
@@ -515,7 +504,7 @@ def run_config4(args, torch, dist, dev, rank, world, lib, precision: str = "tf32
     score_ms = stage.get("kstar", 0.0) + stage.get("qstep", 0.0) + stage.get("qreduce", 0.0)
     mp = measured_peaks()
     # the GEMM is timed alone (CUDA events around its launches): burst figure; tf32 runs at half the 16-bit rate
-    bf16 = float(mp.get("bf16_tflops", 1676.8))
+    bf16 = float(mp.get("bf16_tflops", 989.0))
     tens_peak = bf16 / 2 if precision == "tf32" else bf16
     flops = float(m_loc) * n * n * (3.0 if precision == "fp16x3" else 1.0)  # split operands: three products per MAC
     gemm_ms = stage.get("qstep", 0.0)
@@ -534,11 +523,12 @@ def run_config4(args, torch, dist, dev, rank, world, lib, precision: str = "tf32
                     (f"fp64 fit ({fit_ms:.0f} ms) + inversion/cast ({inv_ms:.0f} ms) are replicated on every rank (Amdahl); only the "
                      f"{score_ms:.0f} ms of scoring shard")),
         "best": {"value": best[0], "index": best[1]},
-        "roofline": {"kernel": ("pair_split_gemm_norm_kernel" if precision == "fp16x3" else "pair_gemm_norm_kernel") + " (tcgen05 cta_group::2, sigma^2 GEMM)", "bound": "tensor",
+        "roofline": {"kernel": "gemm_norm_kernel (wgmma, sigma^2 GEMM)", "bound": "tensor",
                      "achieved": flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else None, "peak": tens_peak, "unit": "TFLOP/s",
                      "frac": (flops / (gemm_ms * 1e-3) / 1e12 / tens_peak) if gemm_ms > 0 else None,
                      "algorithmic_flops_per_step": flops,
-                     "peak_source": ("MEASURED_PEAKS.json bf16_tflops (cuBLAS bf16 burst; fp16 MMAs run at the same rate)"
+                     "peak_source": (("MEASURED_PEAKS.json bf16_tflops" if "bf16_tflops" in mp else "H100 SXM data sheet dense bf16 (989 TFLOP/s; not measured)")
+                                     + " (fp16 MMAs run at the bf16 rate)"
                                      + (" / 2 (tf32 runs at half the 16-bit rate)" if precision == "tf32" else ""))},
     }
     del gp
@@ -602,6 +592,26 @@ def run_config5(args, torch, dist, dev, rank, world, n: int = 65536) -> dict | N
     return out
 
 
+def load_built_lib():
+    """The library as __graft_entry__.build() left it; a missing or stale build is an error, not something to rebuild here."""
+    from limbo_b200 import _lib
+    from limbo_b200 import build as lbuild
+    if not lbuild.up_to_date():
+        raise RuntimeError(f"{lbuild.LIB} is missing or older than limbo_b200/csrc: run __graft_entry__.build() first")
+    return _lib.load()
+
+
+def dump_outputs(out_dir: str, gp, n: int, best_value: float, best_index: int) -> None:
+    """What the last timed step handed back: the global acquisition argmax (value, candidate index) and the fitted alpha."""
+    os.makedirs(out_dir, exist_ok=True)
+    alpha = np.empty((n, 1), order="F")
+    from limbo_b200 import _lib
+    _lib.check(_lib.load().lb_get(gp._h, _lib.GET_ALPHA, alpha.ctypes.data), "lb_get(alpha)")
+    np.save(os.path.join(out_dir, "best_value.npy"), np.array([best_value], dtype=np.float64))
+    np.save(os.path.join(out_dir, "best_index.npy"), np.array([best_index], dtype=np.float64))
+    np.save(os.path.join(out_dir, "alpha.npy"), np.ascontiguousarray(alpha[:, 0]))
+
+
 def run_ours(args) -> None:
     import torch
     import torch.distributed as dist
@@ -615,15 +625,10 @@ def run_ours(args) -> None:
     dev = torch.device("cuda", local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    import __graft_entry__ as ge
-    if rank == 0:
-        ge.build()
-    if world > 1:
-        dist.barrier()
     from limbo_b200 import _lib, acqui, kernel, mean, model, synth
     from limbo_b200 import dist as lbdist
 
-    lib = _lib.load()
+    lib = load_built_lib()
     prof_api(lib)
 
     steps, warmup = args.steps, max(args.warmup, 3)
@@ -715,6 +720,13 @@ def run_ours(args) -> None:
     t_ms = e0.elapsed_time(e1)
     launches = gp.launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        if world > 1:  # the record every rank reduces from the last step's all_gather
+            arr = torch.stack(gather_buf).cpu().numpy()
+            best_dev = lbdist.reduce_records(arr[:, 0], arr[:, 1].astype(np.int64))
+        else:
+            best_dev = (float(dBest.item()), int(dIdx.item()) + lo)
+        dump_outputs(args.dump_outputs, gp, n, best_dev[0], best_dev[1])
     prof = prof_read(lib, h)
     lib.lb_profile_enable(h, 0)
     if fitter is not None:  # the trailing updates of the distributed fit run on the fitter's own handle
@@ -792,8 +804,7 @@ def run_ours(args) -> None:
             byts = 8.0 * n * n + 8.0 * n * d
             roof_km = {"kernel": "kbuild_kernel<MaternFiveHalves> (N x N kernel matrix; includes the tiny scale_x launch)", "bound": "hbm",
                        "achieved": byts / (km_ms * 1e-3) / 1e9, "peak": peak_h, "unit": "GB/s", "frac": byts / (km_ms * 1e-3) / 1e9 / peak_h,
-                       "avg_launch_ms": km_ms, "algorithmic_bytes_per_launch": byts, "peak_source": peak_h_src,
-                       "traffic": (ncu_traffic("kbuild_kernel_matern52")[0])}
+                       "avg_launch_ms": km_ms, "algorithmic_bytes_per_launch": byts, "peak_source": peak_h_src}
             del gm
         except Exception as e:
             roof_km = {"error": repr(e)}
@@ -810,16 +821,8 @@ def run_ours(args) -> None:
         table = roofline_table(prof, steps, t_ms, n, d, m_loc)
         roof = {}
         if table:
-            top = dict(table[0])
-            cls = top["class"]
-            kname = {"qstep": ("panel_update_kernel" if m_loc >= 256 else "query_slab_kernel"), "syrk": "syrk_kernel", "kbuild": "kbuild_kernel"}.get(cls)
-            tr, cap = ncu_traffic(kname) if kname else (None, None)
-            top["traffic"] = tr
-            top["traffic_capture"] = cap
-            roof = top
+            roof = dict(table[0])
         roof_k = next((dict(r) for r in table if r["class"] == "kbuild"), {})
-        if roof_k:
-            roof_k["traffic"] = ncu_traffic("kbuild_kernel")[0]
         fit_ms = sum(stage.get(k, 0.0) for k in ("kbuild", "syrk", "trsv"))
         q_ms = stage.get("qstep", 0.0)
         # CPU baseline on a bounded sample (rank 0, N=1 only)
@@ -902,13 +905,8 @@ def run_config4_workload(args) -> None:
     dev = torch.device("cuda", lr)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    import __graft_entry__ as ge
-    if rank == 0:
-        ge.build()
-    if world > 1:
-        dist.barrier()
     from limbo_b200 import _lib
-    lib = _lib.load()
+    lib = load_built_lib()
     prof_api(lib)
     stream = torch.cuda.Stream(dev)
     torch.cuda.set_stream(stream)
@@ -941,7 +939,13 @@ def main() -> None:
                     help="N > 1, config 4: every rank inverts the whole factor (round-1 scheme) instead of its column tiles + one all_gather")
     ap.add_argument("--workload", default="n16384_se_ard", choices=sorted(WORKLOADS) + ["config4"])
     ap.add_argument("--precision", default="tf32", choices=["tf32", "fp16"], help="--workload config4 only")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64; headline workload, rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.workload == "config4" or args.impl == "reference"):
+        ap.error("--dump-outputs covers the headline workloads of the GPU arm (--impl ours, not --workload config4)")
     if args.workload == "config4":
         if args.impl == "reference":
             print(json.dumps({"impl": "reference", "unavailable": "config 4 is a reduced-precision GPU workload; the reference arm is defined for the headline workload"}))

@@ -1,4 +1,4 @@
-/* include/limbo_b200.h — C ABI of the B200-native GP compute backend for Limbo.
+/* include/limbo_b200.h — C ABI of the H100-native (sm_90a) GP compute backend for Limbo.
  *
  * The reference (resibots/limbo @ 43c67a6) has no FFI for this path: the seam
  * is the C++ "Model concept" implemented by limbo::model::GP
@@ -62,9 +62,9 @@ typedef struct lb_gp lb_gp;
 
 /* precision modes */
 #define LB_PREC_FP64 0
-/* fit / likelihood in fp64; lb_query and lb_acq_argmax compute sigma^2 on the tf32 tensor cores (tcgen05, fp32
+/* fit / likelihood in fp64; lb_query and lb_acq_argmax compute sigma^2 on the tf32 tensor cores (wgmma, fp32
  * accumulation) from an fp64-inverted factor; mu stays fp64.  |d sigma^2| = a few 1e-3 k(v,v), growing with cond(K)
- * (measured maxima in tests/test_gpu_tf32.py) */
+ * (the bounds tests/test_gpu_tf32.py asserts) */
 #define LB_PREC_TF32 1
 /* same path with fp16 operands (same 11-bit significand as tf32, half the operand bytes, twice the tensor rate);
  * K* is scaled by 1/sigma_f^2 and L^-1 by a power of two so that both stay inside the fp16 range */

@@ -9,7 +9,7 @@
 // MultiGP<Params, limbo_b200::model::GP, ...>.  The kernel / mean / hp-opt policy
 // types stay the reference's own (kernel::SquaredExpARD<Params>, mean::Data<Params>,
 // gp::KernelLFOpt<Params> ...); only their public state (h_params(), noise()) is read
-// and handed to the B200 library through the C ABI (include/limbo_b200.h).
+// and handed to the CUDA library through the C ABI (include/limbo_b200.h).
 // Mean functions and aggregators remain host functors, exactly as in the reference.
 //
 // A kernel type without a trait specialisation below is a compile-time error: there

@@ -1,4 +1,4 @@
-"""limbo_b200 — B200-native (sm_100a) GP compute backend behind limbo::model::GP's interface.
+"""limbo_b200 — H100-native (sm_90a) GP compute backend behind limbo::model::GP's interface.
 
 Only what the hot path needs lives here: csrc/ (CUDA kernels + C ABI), the ctypes
 binding, and the host-side mirror of the reference's model / kernel / mean / acqui /

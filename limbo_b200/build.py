@@ -1,4 +1,4 @@
-"""Build the sm_100a CUDA library (limbo_b200/lib/liblimbo_b200.so) in-tree with nvcc.
+"""Build the sm_90a (H100) CUDA library (limbo_b200/lib/liblimbo_b200.so) in-tree with nvcc.
 
 The library is plain CUDA runtime + C ABI (include/limbo_b200.h); it does not
 link against torch.  nvcc cross-compiles without a GPU.
@@ -17,7 +17,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "liblimbo_b200.so")
 SOURCES = ["abi.cu", "pool.cu", "kbuild.cu", "potrf.cu", "trsv.cu", "query.cu", "lml.cu", "loo.cu", "tf32_query.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--extended-lambda", "-Xcompiler", "-fPIC", "-diag-suppress", "177",
 ]
 
@@ -42,12 +42,21 @@ def _stamp() -> str:
     return h.hexdigest()
 
 
+def up_to_date() -> bool:
+    """True when the library exists and was built from the current sources and flags (read-only check)."""
+    stamp_file = os.path.join(LIBDIR, "build.stamp")
+    if not (os.path.exists(LIB) and os.path.exists(stamp_file)):
+        return False
+    with open(stamp_file) as fh:
+        return fh.read() == _stamp()
+
+
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(LIBDIR, exist_ok=True)
     stamp_file = os.path.join(LIBDIR, "build.stamp")
-    stamp = _stamp()
-    if not force and os.path.exists(LIB) and os.path.exists(stamp_file) and open(stamp_file).read() == stamp:
+    if not force and up_to_date():
         return LIB
+    stamp = _stamp()
     nvcc = _nvcc()
     objdir = os.path.join(LIBDIR, "obj")
     os.makedirs(objdir, exist_ok=True)
@@ -64,7 +73,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 2)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

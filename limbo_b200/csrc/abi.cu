@@ -768,8 +768,11 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
 
 // Batches of at least this many candidates take the panel path (LB_QUERY_PANEL_MIN overrides).  The slab kernel keeps the
 // one-point / small-batch latency, but its time does not shrink with the batch: every CTA streams all of L through L2 whatever
-// its slab width (N = 16384: ~88 ms for ANY batch of <= 10^4 candidates; measured on 8 GPUs, 1250 candidates per rank), while
-// the panel path scales with the number of 128-candidate column tiles.
+// its slab width, while the panel path scales with the number of 128-candidate column tiles.  Measured on an H100 SXM at a 400 W
+// power limit, N = 16384, ms per batch of 32 / 64 / 128 / 256 / 512 candidates: slab path 86.1 for every size, panel path
+// 5.7 / 5.7 / 5.7 / 5.8 / 6.1: at this N the panel path wins from the smallest batch.  The default of 256 is not re-tuned:
+// batches at small N (the reference's own regime) have not been measured on H100, and below the threshold a batch is bit-identical
+// to one-point queries (query_point_kernel runs the slab body).
 static int64_t g_query_panel_min = -1;
 static int64_t query_panel_min()
 {
@@ -838,11 +841,11 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
             dQraw = w.dQraw;
         }
         if (h->precision == LB_PREC_TF32 || h->precision == LB_PREC_FP16 || h->precision == LB_PREC_FP16X3) {
-            // reduced-precision variance on tcgen05 (tf32_query.cu); mu is accumulated in fp64 from the fp64 kernel values
+            // reduced-precision variance on wgmma (tf32_query.cu); mu is accumulated in fp64 from the fp64 kernel values
             if ((rc = lb_tf32_prepare(h))) return rc;
-            // Candidate chunks of k x (SMs / 2 CTA pairs x 256 candidates): whole waves of the persistent tcgen05 GEMM (a 65536
-            // chunk = 3.46 waves cost 15 %); K*^T chunk <= 4 GiB.
-            int sms = 148;
+            // Candidate chunks of k x (SMs x 128 candidates): whole waves of the persistent wgmma GEMM (one 128-candidate tile
+            // per CTA per wave); K*^T chunk <= 4 GiB.
+            int sms = 132;
             LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
             const int64_t CH = 2 * LB_TILE, wave = (int64_t)(sms / 2) * CH;
             const int64_t cap = std::max<int64_t>(CH, ((int64_t)4 << 30) / (4 * h->Np) / CH * CH);
@@ -850,7 +853,7 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
             Mc = std::min((M + CH - 1) / CH * CH, Mc);
             if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * Mc))) return rc;
             if ((rc = ensure(h, &w.dKt, &w.kt_bytes, sizeof(float) * (size_t)Mc * h->Np))) return rc;
-            if ((rc = ensure(h, &w.dNorm2, &w.norm2_bytes, sizeof(float) * (size_t)Mc * 4))) return rc; // up to 4 cluster partials (split mode: Mc doubles)
+            if ((rc = ensure(h, &w.dNorm2, &w.norm2_bytes, sizeof(double) * (size_t)Mc))) return rc; // Mc floats (split mode: Mc doubles)
             if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * (size_t)(P + 1) * (h->Np / LB_TILE) * Mc))) return rc; // mean (+ bias) partials per training tile
             if ((rc = ensure(h, &w.dBias, &w.bias_bytes, sizeof(double) * Mc))) return rc;
             double* dBiasUse = (h->precision == LB_PREC_FP16X3) ? nullptr : w.dBias; // 22-bit operands: no rounding-bias term

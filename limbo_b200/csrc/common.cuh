@@ -1,4 +1,4 @@
-// limbo_b200/csrc/common.cuh — shared declarations for the sm_100a GP backend.
+// limbo_b200/csrc/common.cuh — shared declarations for the sm_90a GP backend.
 //
 // Data layout in HBM (see DESIGN.md §3):
 //   * every N-sized dimension is padded to Np = roundup(N, 128); the padded
@@ -199,7 +199,7 @@ __device__ __forceinline__ uint32_t lb_smem_u32(const void* p)
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// fp64 tensor-core MMA (DMMA).  tcgen05 has no f64 kind; on sm_100a the fp64
+// fp64 tensor-core MMA (DMMA).  wgmma has no f64 kind; on sm_90a the fp64
 // tensor path is warp-level mma.sync, which ptxas lowers to DMMA.8x8x4.
 //   A frag (16x8, row): a[i]: row = g + 8*(i&1), col = t + 4*(i>>1)
 //   B frag (8x8,  col): b[i]: k = t + 4*i, n = g
@@ -420,9 +420,6 @@ int lb_ensure_scratch(lb_gp* h, size_t bytes);
 int lb_tf32_prepare(lb_gp* h);
 int lb_launch_tf32_gemm_norm(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N, int64_t K,
     int tri, float* dNorm2, float* dDout, int* dErr, int grid, int f16);
-int lb_launch_tf32_gemm_norm_cluster(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N,
-    int64_t K, int tri, float* dNorm2, int* dErr, int sms, int cl, int f16);
-int lb_tf32_cluster_size();
 int lb_launch_kstar_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, const double* dQs, int64_t Mcp, float* dKt, double* dMuPart,
     double* dMu, double* dBias, long long* launches);
 int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mcp, const float* dKt, float* dNorm2, int* dErr,

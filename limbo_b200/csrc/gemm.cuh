@@ -3,15 +3,14 @@
 // A CTA accumulates a 128 x BN tile  acc (+/-)= A(128 x K) * B(K x BN)  with a 3-stage cp.async
 // pipeline.  Configurations (Cfg<BN, WN, BK>):
 //   * warps: 4 along M x WN along N  (THREADS = 128 * WN); warp tile 32 x (BN / WN);
-//     a single warp can only drive the DMMA pipe of its SM sub-partition at half rate
-//     (measured, profiles/r01_microbench.json), so an SM needs >= 2 warps per sub-partition that
-//     are actually issuing DMMA at any time:
+//     both configurations keep >= 2 DMMA-issuing warps per SM sub-partition, so that the dependent
+//     DMMAs of one warp do not leave the pipe idle:
 //       Cfg<128, 4, 32>: 512 threads, one CTA per SM, 4 warps per sub-partition;
 //       Cfg< 64, 2, 16>: 256 threads, TWO CTAs per SM (77 KB smem, <= 128 regs): while one CTA
 //                        is in its C-tile prologue / store epilogue the other one computes.
 //   * operands "outer-contiguous" (the m / n index is the unit-stride one, i.e. a column-major
 //     block) or "K-contiguous"; shared tiles are padded by 4 doubles so every 64-bit fragment
-//     load is bank-conflict free (DESIGN.md §4.1; ncu: 0 shared bank conflicts).
+//     load is bank-conflict free (DESIGN.md §4.1).
 //   * NEG_A: acc -= A*B, so a tile update C - A*B preloads C into the accumulators and those loads
 //     overlap the pipeline prologue instead of a dependent load-subtract-store epilogue.
 //
@@ -26,8 +25,8 @@ namespace lbg {
 constexpr int BM = 128;
 constexpr int STAGES = 3;
 
-// DF_ = number of n8-tiles per warp (0 or 1, the last ones) whose 32 x 8 strip is computed with plain DFMA instead of DMMA:
-// ncu shows the fp64 ALU pipe at 0 % while the DMMA (tensor) pipe is the bound of these kernels - they are separate pipes.
+// DF_ = number of n8-tiles per warp (0 or 1, the last ones) whose 32 x 8 strip is computed with plain DFMA instead of DMMA
+// (the LB_SYRK_DF=1 experiment: part of the tile on the fp64 ALU pipe beside DMMA; off by default).
 template <int BN_, int WN_, int BK_, int DF_ = 0>
 struct Cfg {
     static constexpr int BN = BN_, WN = WN_, BK = BK_, DF = DF_;

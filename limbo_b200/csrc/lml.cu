@@ -154,14 +154,13 @@ __device__ __forceinline__ void tile_from_index(int t, int& bi, int& bj)
 // grad partials: part[tile][q], q < nh.
 //   sum_{i>=j} w_ij * dK_ij/dtheta_q * (1/2 if i==j)        gp.hpp:299-308
 //   w = alpha alpha^T - K^-1                                  gp.hpp:293-296
-// One pass over the lower tiles of K^-1 (HBM floor 4 N^2 bytes).  Round 1 ran at 0.085 of that floor: libm exp, two global
-// loads of alpha per element and output, 64-bit index predicates on every element.  Now the kernel id and the edge handling
+// One pass over the lower tiles of K^-1 (HBM floor 4 N^2 bytes).  The kernel id and the edge handling
 // are template parameters (interior tiles carry no predicates), alpha_i / alpha_j are staged in shared memory, and the
 // exponentials use the branch-free lb_exp_nonpos (<= 3e-16 relative, inside the 1e-9 bar of the gradient).
 constexpr int GRAD_PMAX = 4; // outputs staged in shared memory (more: global loads)
 
 // columns per pass: 4 chunks of 8 (four passes over the 128 columns of a tile) keep the live accumulators small enough for three
-// CTAs per SM (the kernel is bound by latency / instruction issue, not by the fp64 pipe: 36 % active at two CTAs per SM)
+// CTAs per SM (the kernel is bound by latency / instruction issue rather than by the fp64 pipe)
 constexpr int GNC = 2, GNH = 16 / GNC, GHW = 8 * GNC;
 
 template <int KID, bool EDGE>

@@ -458,9 +458,8 @@ int lb_launch_potrf(lb_gp* h)
     // b(p) is split at a FIXED block column cstar into a left group (main stream) and a right group (second, normal-priority
     // stream): a tile never changes group, so each group's stream order carries its tile dependencies, and the tail of one
     // group's launch (partial last wave, plus SMs handed to the side-stream panel kernels) is filled by the other group's CTAs.
-    // In the panel query (query.cu) this is worth 6 % (85.5 -> 80.4 ms); here the side-stream panel kernels already fill the
-    // tails: measured 137.3 -> 136.8 ms per bench step, inside the noise, and the per-class launch timers would double count
-    // concurrent launches - so it is OFF unless LB_POTRF_SPLIT=1.
+    // Here the side-stream panel kernels already fill most of the tails, and the per-class launch timers would double count
+    // concurrent launches - so it is an experiment, OFF unless LB_POTRF_SPLIT=1.
     static int split_on = -1;
     if (split_on < 0) { const char* e = getenv("LB_POTRF_SPLIT"); split_on = (e && atoi(e) != 0) ? 1 : 0; }
     cudaStream_t second = main;

@@ -319,8 +319,8 @@ int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_
 //
 // One CTA per candidate slab of up to 72 candidates; the slab walks all T row
 // blocks of the factor by itself, so there is no inter-CTA dependency, no
-// per-step launch and no wave quantisation (slabs are sized so that all 148 SMs
-// get 8 or 9 n8-tiles).  For row block i:
+// per-step launch and little wave quantisation (slabs are sized from the SM count
+// so that every SM gets the same number of n8-tiles, give or take one).  For row block i:
 //   acc  = K*[i, slab]  (generated on chip from X_i and the slab's candidates;
 //                        mu += K*^T alpha on the way)
 //   acc -= L[i, 0:i] V[0:i, slab]      (DMMA, A = L via L2, B = the CTA's private V)
@@ -722,8 +722,7 @@ LbOncePerDevice g_attr_once2;
 //     solve_s  :  V_s   = inv(L_ss) T_s                      (same tiles, K = (i + 1) * 128: inv(L_ss) is lower triangular)
 // inv(L_ss) = the 16-tile diagonal blocks of L^-1 from the first levels of the recursive trtri (lml.cu, ~1 % of the flops of a
 // fit, cached until the next fit).  Each V block is read once per SUPER-block instead of once per 128-row block: the
-// fused slab kernel above streams its private V slab T/2 times (86 GB of DRAM traffic at N = 16384, M = 10^4, ncu round 1),
-// this path moves ~10 GB.  mu comes from K* before the solve; |V_c|^2 is reduced per tile in the solve epilogue (fixed
+// fused slab kernel above streams its private V slab T/2 times (T = N / 128 row blocks), this path once per super-block.  mu comes from K* before the solve; |V_c|^2 is reduced per tile in the solve epilogue (fixed
 // order: lanes -> warps -> tiles), so results are run-to-run deterministic and independent of the batch composition
 // (a candidate's value depends only on its own column).
 // ===========================================================================
@@ -861,39 +860,40 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
         mu_kernel<<<(unsigned)M, 256, 0, st>>>(dV, h->Np, h->dAlpha, h->P, dMu);
     }
     if (launches) *launches += 2;
-    // The chain update_s -> solve_s -> update_s+1 -> ... only couples tiles of the SAME candidate column tile: the column tiles
-    // are split into two groups that walk the chain on two streams, so the tail of one group's launch (a launch is 8.5 waves of
-    // 148 CTAs at M = 10^4: ncu showed the tensor pipe 93 % busy while active but 80 % of the elapsed time) is filled by the
-    // other group's CTAs instead of idle SMs.
+    // The chain update_s -> solve_s -> update_s+1 -> ... only couples tiles of the SAME candidate column tile, so the column tiles
+    // can walk it in groups on separate streams, the tail of one group's launch being filled by another group's CTAs.
     const int ctiles = (int)(Mp / LB_TILE);
     static int split_pct = -1, use_side = -1;
     if (split_pct < 0) {
         const char* e = getenv("LB_PANEL_SPLIT");   // percentage of the column tiles in the first group; 100 = one stream
-        split_pct = e ? atoi(e) : 70; // measured at N = 16384, M = 10^4: one stream 85.5 ms, 50 / 60 / 70 / 80 %: 81.3 / 80.6 / 80.5 / 80.4 ms
+        split_pct = e ? atoi(e) : 100; // see the group choice below
         if (split_pct < 1 || split_pct > 100) split_pct = 100;
         const char* e2 = getenv("LB_PANEL_SIDE");   // 1: second group on the high-priority side stream instead of a normal-priority one
         use_side = (e2 && atoi(e2) != 0) ? 1 : 0;
     }
-    // LB_PANEL_CFG=1: 128 x 128 tiles (CfgWide); default 128 x 64 tiles, two CTAs per SM.  Measured at N = 16384 (ms per batch,
-    // Wide / Dual): M = 1250: 13.6 / 13.1, 2500: 23.1 / 21.9, 5000: 42.6 / 39.8, 10^4: 80.4 / 78.3 (same bits: the tile shape does not
-    // change any element's accumulation order).
+    // LB_PANEL_CFG=1: 128 x 128 tiles (CfgWide); default 128 x 64 tiles, two CTAs per SM (same bits: the tile shape does not
+    // change any element's accumulation order).  H100 SXM, 400 W power limit, N = 16384, ms per batch (Dual / Wide): M = 1250:
+    // 16.6 / 19.0, 2500: 28.9 / 30.3, 10^4: 123.7 / 116.4 - inside the process-to-process spread for large batches, so the
+    // default stays the one that is better for small ones.
     static int cfg_mode = -1;
     if (cfg_mode < 0) { const char* e = getenv("LB_PANEL_CFG"); cfg_mode = e ? atoi(e) : 0; }
     const bool dual = cfg_mode != 1;
     const int wmul = dual ? 2 : 1; // 64-wide column tiles per 128 candidates
-    // Groups of column tiles, each walking the chain on its own stream.  Large batches: two groups (split_pct / rest).  Small batches
-    // (a launch of all column tiles is under ~4 rounds of the machine: M = 1250 is 320 CTAs for 296 slots, i.e. one full round and
-    // one nearly empty): up to four equal groups, so that a launch is a fraction of a round and the groups, drifting apart, keep the
-    // SMs full.  LB_PANEL_GROUPS=<1..4> forces the count.  Measured at N = 16384 (ms per batch, 1 / 2 / 3 / 4 groups): M = 640: 10.6 / 9.7 /
-    // 8.6 / 8.3, 1250: 14.8 / 13.3 / 12.9 / 12.5, 2500: 24.2 / 22.1 / 21.3 / 20.7, 5000: 42.6 / 40.0 / 39.8 / 39.8, 10^4: 83.6 / 78.3 / 78.4 / 78.3
-    // (profiles/r02_panel_groups.txt); results do not depend on the grouping (every tile's arithmetic is unchanged).
+    // Groups of column tiles, each walking the chain on its own stream.  A launch of all column tiles under one round of the machine
+    // (M = 640 at N = 16384: 160 CTAs for 264 slots): four equal groups, so that the groups, drifting apart, keep the SMs full.
+    // Otherwise one stream, unless LB_PANEL_SPLIT=<1..99> asks for two groups (that percentage / the rest).  LB_PANEL_GROUPS=<1..4>
+    // forces the count.  Measured on an H100 SXM at a 400 W power limit, N = 16384, ms per batch (process-to-process spread up to
+    // ~10 % at that limit): M = 10^4: one stream 121.9, 90 / 80 / 70 / 60 / 50 % splits 120.8 / 130.3 / 131.5 / 130.9 / 132.0;
+    // 1 / 2 / 3 / 4 groups: M = 640: 10.9 / 10.1 / 9.6 / 9.1, 1250: 16.3 / 15.2 / 15.5 / 16.0, 2500: 28.9 / 28.1 / 30.9 / 30.9.
+    // Results do not depend on the grouping (every tile's arithmetic is unchanged).
     static int force_groups = -1;
     if (force_groups < 0) { const char* e = getenv("LB_PANEL_GROUPS"); force_groups = e ? atoi(e) : 0; }
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const int slots = sms * (dual ? 2 : 1);
     int ngroups = 1;
-    if (split_pct < 100 && ctiles >= 4) ngroups = ((int64_t)ctiles * wmul * SB < (int64_t)4 * slots) ? 4 : 2;
+    if (ctiles >= 4 && (int64_t)ctiles * wmul * SB < (int64_t)slots) ngroups = 4;
+    else if (split_pct < 100 && ctiles >= 4) ngroups = 2;
     if (force_groups >= 1 && force_groups <= 4) ngroups = force_groups;
     if (ngroups > ctiles) ngroups = ctiles;
     cudaStream_t sts[4] = {st, st, st, st};

@@ -1,24 +1,20 @@
-// limbo_b200/csrc/tf32_query.cu — reduced-precision candidate scoring on the 5th-generation tensor cores
-// (BASELINE.json config 4: N = 16384, D = 12, 1M EI candidates; LB_PREC_TF32 / LB_PREC_FP16).
+// limbo_b200/csrc/tf32_query.cu — reduced-precision candidate scoring on the Hopper tensor cores (wgmma)
+// (BASELINE.json config 4: N = 16384, D = 12, 1M EI candidates; LB_PREC_TF32 / LB_PREC_FP16 / LB_PREC_FP16X3).
 //
 // The per-candidate variance needs |L^-1 k*|^2, i.e. V = L^-1 K* (M N^2 flops, gp.hpp:618-624 once per
-// candidate in the reference).  fp64 has no tcgen05 kind, so the fp64 path runs on DMMA (query.cu).  Here the
-// factor is inverted once in fp64 (lml.cu, recursive trtri), cast to a row-major tf32 (fp32 container) or fp16 copy, and
+// candidate in the reference).  The fp64 path runs on DMMA (query.cu).  Here the factor is inverted once in fp64 (lml.cu,
+// recursive trtri), cast to a row-major tf32 (fp32 container) or fp16 copy, and
 //     D[c, n] = sum_{k <= n} Kt[c, k] * Linv[n, k]          (Kt = K*^T, candidates x training points)
-// runs on tcgen05.mma with fp32 accumulators in TMEM; the epilogue never writes D: each of the 128 epilogue threads of a
-// CTA owns one candidate (one TMEM lane) and accumulates sum_n D[c, n]^2.
+// runs on wgmma with fp32 accumulators in registers; D is never written: every consumer thread squares the accumulator
+// fragment it holds and adds it to the partial norms of its two candidate rows.
 //
-// Kernels (all persistent, 192 threads: warp 0 = TMA producer, warp 1 = TMEM allocator + single-thread MMA issuer,
-// warps 2..5 = epilogue; 4-stage shared-memory ring of 128-byte SWIZZLE_128B rows; every mbarrier wait is bounded and
-// raises an error flag instead of hanging the GPU):
-//   pair_gemm_norm_kernel          DEFAULT.  Two CTAs = one MMA pair (tcgen05 ... cta_group::2, UMMA M = 256): each CTA
-//                                  owns 128 candidates and half of every B tile; each A slab feeds two n-tiles (all 512
-//                                  TMEM columns).  24 KB from L2 per 128x256x64-MAC unit instead of 40 KB.
-//   tf32_gemm_norm_cluster_kernel  fallback (LB_TF32_PAIR=0): clusters of 2 / 4 CTAs share the candidate tile by TMA
-//                                  multicast, split the n-tiles, double-buffered accumulators.
-//   tf32_gemm_norm_kernel          single CTA, 128 x 256 tiles (LB_TF32_CLUSTER=1; also the validation entry that can
-//                                  write D).
-// Around them: kstar_t32_kernel (K*^T chunk from fp64 kernel evaluations with the squared distances on the fp64 tensor pipe,
+// gemm_norm_kernel (persistent, 384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers,
+// each issuing m64 wgmmas for 64 of the tile's 128 candidates; a ring of 128-byte SWIZZLE_128B rows in shared memory;
+// every mbarrier wait is bounded and raises an error flag instead of hanging the GPU.
+//   F16 = false : tf32 operands, 128 x 256 tiles, 4 stages of 48 KB
+//   F16 = true  : fp16 operands, same tiles (64 k per stage instead of 32)
+//   SPLIT       : fp16 hi + 2^-11 lo operands (LB_PREC_FP16X3), 128 x 128 tiles, 3 stages of 64 KB, two accumulators
+// Around it: kstar_t32_kernel (K*^T chunk from fp64 kernel evaluations with the squared distances on the fp64 tensor pipe,
 // mean and rounding-bias partials fused), mu_reduce_kernel, sigma2_t32_kernel (clamp / noise of gp.hpp:623,166 and the
 // rounding-bias correction), linv_to_rowmajor_kernel (+ absmax / colnorm2 for the fp16 scale and the bias weights).
 #include "common.cuh"
@@ -30,18 +26,25 @@
 
 namespace tf32q {
 
-constexpr int BM = 128;       // candidates per tile (UMMA M)
-constexpr int BN = 256;       // outputs (rows of L^-1) per tile (UMMA N)
-// k elements per stage = 128 B = one swizzle atom row: 32 tf32 or 64 fp16; one stage is always 4 MMAs (K = 8 tf32 / 16 fp16)
+constexpr int BM = 128;       // candidates per tile (two consumer warpgroups x wgmma M = 64)
+constexpr int BN = 256;       // outputs (rows of L^-1) per tile (wgmma N); split mode: BN / 2
+// k elements per stage = 128 B = one swizzle atom row: 32 tf32 or 64 fp16; one stage is always 4 wgmmas (K = 8 tf32 / 16 fp16)
 template <bool F16> __host__ __device__ constexpr int bke() { return F16 ? 64 : 32; }
 constexpr int MMAS_PER_STAGE = 4;
-constexpr int STAGES = 4;
-constexpr int A_BYTES = BM * 128;  // 16 KB
-constexpr int B_BYTES = BN * 128;  // 32 KB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int THREADS = 192;
-constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int THREADS = 384;
 constexpr long long SPIN_LIMIT = 1LL << 24;
+
+// Shared-memory stage of one k-block: [A hi | B hi | A lo | B lo] (lo planes in split mode only).  The split mode halves the
+// tile width: two 64-register accumulators per thread instead of one of 128.
+template <bool SPLIT>
+struct Cfg {
+    static constexpr int BNT = SPLIT ? BN / 2 : BN;
+    static constexpr int A_BYTES = BM * 128;
+    static constexpr int B_BYTES = BNT * 128;
+    static constexpr int STAGE_BYTES = (SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);
+    static constexpr int STAGES = SPLIT ? 3 : 4;
+    static constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+};
 
 __device__ __forceinline__ void mbar_init(uint64_t* b, uint32_t n)
 {
@@ -68,8 +71,8 @@ __device__ __forceinline__ bool mbar_try(uint64_t* b, uint32_t parity)
     return ok != 0;
 }
 // bounded wait: returns false (and raises *err) instead of spinning forever
-// The error flag (global memory) is polled only every 1024 attempts: a volatile load per spin from six spinning warps
-// would saturate the SM's load/store path (and starve any kernel sharing the SM).
+// The error flag (global memory) is polled only every 1024 attempts: a volatile load per spin from every spinning thread
+// would saturate the SM's load/store path.
 __device__ __forceinline__ bool mbar_wait(uint64_t* b, uint32_t parity, int* err)
 {
     long long spins = 0;
@@ -81,25 +84,6 @@ __device__ __forceinline__ bool mbar_wait(uint64_t* b, uint32_t parity, int* err
     }
     return true;
 }
-// Long waits of a whole warp (epilogue waiting for ~100 us of MMAs): one lane polls with a back-off, the other 31 lanes
-// sleep at the warp barrier instead of issuing try_wait / branch instructions.
-__device__ __forceinline__ bool mbar_wait_warp(uint64_t* b, uint32_t parity, int* err)
-{
-    int ok = 1;
-    if ((threadIdx.x & 31) == 0) {
-        long long spins = 0;
-        while (!mbar_try(b, parity)) {
-            __nanosleep(128);
-            if ((++spins & 255) == 0 && (spins > (SPIN_LIMIT >> 4) || *(volatile int*)err)) {
-                atomicExch(err, 1);
-                ok = 0;
-                break;
-            }
-        }
-    }
-    ok = __shfl_sync(0xffffffffu, ok, 0);
-    return ok != 0;
-}
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar)
 {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
@@ -107,672 +91,199 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, i
                  "l"(map), "r"(c0), "r"(c1), "r"(lb_smem_u32(bar))
                  : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp):
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma (PTX ISA, "Matrix Descriptor Format"):
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major: 1) |
-//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B -> 64) | [46,48) version = 1 | [61,64) layout = 2 (SWIZZLE_128B)
+//   [32,46) stride byte offset >> 4 (8 rows x 128 B = 1024 B -> 64) | [62,64) layout = 1 (SWIZZLE_128B)
+// Every operand tile starts on a 1024-byte boundary, so the base-offset field stays 0.
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr)
 {
-    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 = 1 @4, a/b format TF32 = 2 @7/@10,
-// a/b K-major (0) @15/@16, N >> 3 @17, M >> 4 @24
-// a/b format: F16 = 0, TF32 = 2
-template <bool F16>
-__host__ __device__ constexpr uint32_t idesc()
+
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R])
 {
-    return (1u << 4) | ((F16 ? 0u : 2u) << 7) | ((F16 ? 0u : 2u) << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// m64 x N x k wgmmas, A and B from K-major shared memory, fp32 accumulators; accumulate == 0 overwrites d.
+// Accumulator fragment: d[i] is row (warp % 4) * 16 + lane / 4 + 8 * ((i >> 1) & 1), column (i >> 2) * 8 + 2 * (lane % 4) + (i & 1).
+__device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t a, uint64_t b, int accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t a, uint64_t b, int accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(a), "l"(b), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a, uint64_t b, int accumulate)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(accumulate));
 }
 
 template <bool F16>
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+__device__ __forceinline__ void wgmma_n256(float (&d)[128], uint64_t a, uint64_t b, int accumulate)
 {
-    if (F16)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc<true>()), "r"(accumulate)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc<false>()), "r"(accumulate)
-            : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(lb_smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
+    if (F16) wgmma_f16_n256(d, a, b, accumulate);
+    else wgmma_tf32_n256(d, a, b, accumulate);
 }
 
 // D[c, n] = sum_k A[c, k] B[n, k]; tri != 0: k only up to the end of the n-tile (B lower triangular).
-// norm2[c] += sum_n D[c, n]^2 ; Dout (optional, row-major M x N) receives D for validation.
-template <bool F16>
+// norm2[c] = sum_n D[c, n]^2 (float; double in split mode); Dout (optional, row-major M x N, not in split mode) receives D
+// for validation.  Split mode: D = A_hi B_hi + 2^-11 (A_hi B_lo + A_lo B_hi) from three fp16 wgmmas per k-step into two
+// accumulators (the 2^-22 A_lo B_lo term is dropped), combined and squared in fp64.
+template <bool F16, bool SPLIT>
 __global__ void __launch_bounds__(THREADS, 1)
-tf32_gemm_norm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, int64_t M, int64_t N,
-    int64_t K, int tri, float* __restrict__ norm2, float* __restrict__ Dout, int* __restrict__ err)
+gemm_norm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+    const __grid_constant__ CUtensorMap mapAlo, const __grid_constant__ CUtensorMap mapBlo, int64_t M, int64_t N, int64_t K, int tri,
+    void* __restrict__ norm2_, float* __restrict__ Dout, int* __restrict__ err)
 {
+    static_assert(F16 || !SPLIT, "split operands are fp16");
+    using C = Cfg<SPLIT>;
+    using NormT = typename std::conditional<SPLIT, double, float>::type;
+    constexpr int BNT = C::BNT, BKE = bke<F16>(), NACC = BNT / 2;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023); // SWIZZLE_128B needs 1024-byte alignment
-    uint64_t* full = (uint64_t*)(smem + (size_t)STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;   // [2]
-    uint64_t* tempty = tfull + 2;       // [2]
-    uint32_t* tmem_base_s = (uint32_t*)(tempty + 2);
+    uint64_t* full = (uint64_t*)(smem + (size_t)C::STAGES * C::STAGE_BYTES);
+    uint64_t* empty = full + C::STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m_tiles = (int)(M / BM), n_tiles = (int)(N / BN);
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int m_tiles = (int)(M / BM), n_tiles = (int)(N / BNT);
+    auto kblocks_of = [&](int nt) {
+        const int64_t kend = tri ? (int64_t)(nt + 1) * BNT : K;
+        return (int)((kend < K ? kend : K) / BKE);
+    };
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 4); }
+        for (int s = 0; s < C::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); } // empty: one arrival per consumer warpgroup
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) { // TMEM: 512 columns (2 accumulators of 256)
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(lb_smem_u32(tmem_base_s)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_s;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ===== TMA producer =====
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (threadIdx.x == 0) {
             int s = 0; uint32_t ph = 0; bool ok = true;
             for (int mt = blockIdx.x; mt < m_tiles && ok; mt += gridDim.x) {
                 for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                    const int64_t kend = tri ? (int64_t)(nt + 1) * BN : K;
-                    const int kblocks = (int)((kend < K ? kend : K) / bke<F16>());
+                    const int kblocks = kblocks_of(nt);
                     for (int kb = 0; kb < kblocks; ++kb) {
                         if (!mbar_wait(&empty[s], ph ^ 1, err)) { ok = false; break; }
-                        uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], STAGE_BYTES);
-                        tma_load_2d(sa, &mapA, kb * bke<F16>(), mt * BM, &full[s]);
-                        tma_load_2d(sa + A_BYTES, &mapB, kb * bke<F16>(), nt * BN, &full[s]);
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
+                        uint8_t* sa = smem + (size_t)s * C::STAGE_BYTES;
+                        mbar_expect_tx(&full[s], C::STAGE_BYTES);
+                        tma_load_2d(sa, &mapA, kb * BKE, mt * BM, &full[s]);
+                        tma_load_2d(sa + C::A_BYTES, &mapB, kb * BKE, nt * BNT, &full[s]);
+                        if (SPLIT) {
+                            tma_load_2d(sa + C::A_BYTES + C::B_BYTES, &mapAlo, kb * BKE, mt * BM, &full[s]);
+                            tma_load_2d(sa + 2 * C::A_BYTES + C::B_BYTES, &mapBlo, kb * BKE, nt * BNT, &full[s]);
+                        }
+                        if (++s == C::STAGES) { s = 0; ph ^= 1; }
                     }
-                }
-            }
-        }
-    }
-    else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            int buf = 0; uint32_t tph[2] = {0, 0};
-            for (int mt = blockIdx.x; mt < m_tiles && ok; mt += gridDim.x) {
-                for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                    const int64_t kend = tri ? (int64_t)(nt + 1) * BN : K;
-                    const int kblocks = (int)((kend < K ? kend : K) / bke<F16>());
-                    if (!mbar_wait(&tempty[buf], tph[buf] ^ 1, err)) { ok = false; break; } // epilogue drained this accumulator
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        if (!mbar_wait(&full[s], ph, err)) { ok = false; break; }
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sa = lb_smem_u32(smem + (size_t)s * STAGE_BYTES);
-                        const uint64_t adesc = make_desc(sa), bdesc = make_desc(sa + A_BYTES);
-#pragma unroll
-                        for (int k = 0; k < MMAS_PER_STAGE; ++k) // +32 B per MMA inside the 128 B swizzle row: +2 in the >>4 address field
-                            umma<F16>(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
-                        umma_commit(&empty[s]); // frees the smem slot when these MMAs have read it
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                    umma_commit(&tfull[buf]); // accumulator complete
-                    tph[buf] ^= 1;
-                    buf ^= 1;
                 }
             }
         }
     }
     else {
-        // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4 =====
-        const int q = warp & 3;
-        const int row = q * 32 + lane; // candidate inside the tile == TMEM lane
-        int buf = 0; uint32_t tph[2] = {0, 0}; bool ok = true;
-        for (int mt = blockIdx.x; mt < m_tiles && ok; mt += gridDim.x) {
-            float acc = 0.f;
-            for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                if (!mbar_wait_warp(&tfull[buf], tph[buf], err)) { ok = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(taddr + c, v);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        // ===== consumers: warpgroup c owns candidate rows [64 c, 64 c + 64) of the tile =====
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int c = wg - 1;
+        const int r0 = c * 64 + warp * 16 + (lane >> 2); // this thread's rows: r0 and r0 + 8
+        const bool signal = (warp == 0 && lane == 0);    // releases a stage for its warpgroup
+        float acc[NACC];
+        float acc1[SPLIT ? NACC : 1];
+        // A timed-out wait never leaves the loops: what follows it is warpgroup-collective (wgmma, wgmma.wait_group) and
+        // warp-collective (the quad shuffles), so every thread keeps walking the same trip counts, which depend only on the
+        // shapes and blockIdx.  It only marks its results invalid; once *err is raised every later wait gives up after one
+        // polling interval, and operands left stale in shared memory feed results that are never written.
+        int s = 0; uint32_t ph = 0; bool ok = true;
+        for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x) {
+            NormT n0 = 0, n1 = 0;
+            for (int nt = 0; nt < n_tiles; ++nt) {
+                const int kblocks = kblocks_of(nt);
+                int prev = -1;
+                for (int kb = 0; kb < kblocks; ++kb) {
+                    if (!mbar_wait(&full[s], ph, err)) ok = false;
+                    const uint32_t sa = lb_smem_u32(smem + (size_t)s * C::STAGE_BYTES);
+                    const uint64_t ad = make_desc(sa + c * 64 * 128), bd = make_desc(sa + C::A_BYTES);
+                    acc_fence(acc);
+                    if (SPLIT) acc_fence(acc1);
+                    wg_fence();
+                    if constexpr (SPLIT) {
+                        const uint64_t ald = make_desc(sa + C::A_BYTES + C::B_BYTES + c * 64 * 128),
+                                       bld = make_desc(sa + 2 * C::A_BYTES + C::B_BYTES);
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float d = __uint_as_float(v[j]);
-                        acc = fmaf(d, d, acc);
-                        if (Dout) Dout[((int64_t)mt * BM + row) * N + (int64_t)nt * BN + c + j] = d;
+                        for (int k = 0; k < MMAS_PER_STAGE; ++k) { // +32 B per wgmma inside the 128 B swizzle row: +2 in the >>4 address field
+                            wgmma_f16_n128(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kb | k) != 0);
+                            wgmma_f16_n128(acc1, ad + (uint64_t)(2 * k), bld + (uint64_t)(2 * k), (kb | k) != 0);
+                            wgmma_f16_n128(acc1, ald + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1);
+                        }
                     }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[buf]); // 4 arrivals (one per epilogue warp) release the accumulator
-                tph[buf] ^= 1;
-                buf ^= 1;
-            }
-            if (ok) norm2[(int64_t)mt * BM + row] = acc;
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Clustered variant: CL CTAs (CL = 2 or 4) share one candidate tile and split the n-tiles between them.  The A
-// tile (K*^T, private to a candidate tile, streamed from HBM once per n-tile) is loaded ONCE per cluster and
-// TMA-multicast into every CTA's shared memory, which divides the dominant HBM stream by CL; each CTA keeps its own
-// B tiles, TMEM accumulators, MMA issuer and epilogue.  Slot reuse is cluster-wide: every MMA commit multicasts its
-// "slot free" arrival to all CTAs of the cluster (empty barriers count CL arrivals).
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mcast(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar, uint16_t mask)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
-        ::"r"(lb_smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(lb_smem_u32(bar)), "h"(mask)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t mask)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     lb_smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
-}
-
-// norm2 is [CL][M]: each CTA of a cluster writes the partial sum over its own n-tiles (summed later, fixed order).
-template <int CL, bool F16>
-__global__ void __launch_bounds__(THREADS, 1)
-tf32_gemm_norm_cluster_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, int64_t M, int64_t N,
-    int64_t K, int tri, float* __restrict__ norm2, int* __restrict__ err)
-{
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = (uint64_t*)(smem + (size_t)STAGES * STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_base_s = (uint32_t*)(tempty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = (int)cluster_ctarank();
-    const int cluster_id = blockIdx.x / CL, nclusters = gridDim.x / CL;
-    const int m_tiles = (int)(M / BM), n_groups = (int)(N / BN) / CL; // N is a multiple of BN * CL
-    constexpr uint16_t ALL = (uint16_t)((1u << CL) - 1);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CL); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(lb_smem_u32(tmem_base_s)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all(); // every CTA's barriers are initialised before any remote arrival / multicast can target them
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_s;
-
-    if (warp == 0) {
-        if (lane == 0) { // ===== TMA producer: own B tile; rank 0 additionally multicasts the shared A tile =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            for (int mt = cluster_id; mt < m_tiles && ok; mt += nclusters) {
-                for (int grp = 0; grp < n_groups && ok; ++grp) {
-                    const int nt = grp * CL + rank;
-                    const int64_t kend = tri ? (int64_t)(grp + 1) * CL * BN : K; // the whole cluster walks the same k range
-                    const int kblocks = (int)((kend < K ? kend : K) / bke<F16>());
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        if (!mbar_wait(&empty[s], ph ^ 1, err)) { ok = false; break; } // freed by ALL CTAs of the cluster
-                        uint8_t* sa = smem + (size_t)s * STAGE_BYTES;
-                        mbar_expect_tx(&full[s], STAGE_BYTES);
-                        if (rank == 0) tma_load_2d_mcast(sa, &mapA, kb * bke<F16>(), mt * BM, &full[s], ALL);
-                        tma_load_2d(sa + A_BYTES, &mapB, kb * bke<F16>(), nt * BN, &full[s]);
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                }
-            }
-        }
-    }
-    else if (warp == 1) {
-        if (lane == 0) { // ===== MMA issuer =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            int buf = 0; uint32_t tph[2] = {0, 0};
-            for (int mt = cluster_id; mt < m_tiles && ok; mt += nclusters) {
-                for (int grp = 0; grp < n_groups && ok; ++grp) {
-                    const int64_t kend = tri ? (int64_t)(grp + 1) * CL * BN : K;
-                    const int kblocks = (int)((kend < K ? kend : K) / bke<F16>());
-                    if (!mbar_wait(&tempty[buf], tph[buf] ^ 1, err)) { ok = false; break; }
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-                    for (int kb = 0; kb < kblocks; ++kb) {
-                        if (!mbar_wait(&full[s], ph, err)) { ok = false; break; }
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sa = lb_smem_u32(smem + (size_t)s * STAGE_BYTES);
-                        const uint64_t adesc = make_desc(sa), bdesc = make_desc(sa + A_BYTES);
+                    else {
 #pragma unroll
                         for (int k = 0; k < MMAS_PER_STAGE; ++k)
-                            umma<F16>(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (kb | k) != 0);
-                        umma_commit_mcast(&empty[s], ALL); // this CTA is done with slot s: tell every producer of the cluster
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
+                            wgmma_n256<F16>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kb | k) != 0);
                     }
-                    umma_commit(&tfull[buf]);
-                    tph[buf] ^= 1;
-                    buf ^= 1;
+                    wg_commit();
+                    wg_wait<1>(); // the previous stage's wgmmas have read their operands
+                    acc_fence(acc);
+                    if (SPLIT) acc_fence(acc1);
+                    if (prev >= 0 && signal) mbar_arrive(&empty[prev]);
+                    prev = s;
+                    if (++s == C::STAGES) { s = 0; ph ^= 1; }
                 }
-            }
-        }
-    }
-    else {
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        int buf = 0; uint32_t tph[2] = {0, 0}; bool ok = true;
-        for (int mt = cluster_id; mt < m_tiles && ok; mt += nclusters) {
-            float acc = 0.f;
-            for (int grp = 0; grp < n_groups && ok; ++grp) {
-                if (!mbar_wait_warp(&tfull[buf], tph[buf], err)) { ok = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(taddr + c, v);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+                wg_wait<0>();
+                acc_fence(acc);
+                if (SPLIT) acc_fence(acc1);
+                if (signal) mbar_arrive(&empty[prev]);
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float d = __uint_as_float(v[j]);
-                        acc = fmaf(d, d, acc);
+                for (int i = 0; i < NACC; ++i) {
+                    const bool hi_row = (i >> 1) & 1;
+                    if constexpr (SPLIT) {
+                        const double d = fma((double)acc1[i], 1.0 / 2048.0, (double)acc[i]);
+                        if (hi_row) n1 = fma(d, d, n1);
+                        else n0 = fma(d, d, n0);
+                    }
+                    else {
+                        if (hi_row) n1 = fmaf(acc[i], acc[i], n1);
+                        else n0 = fmaf(acc[i], acc[i], n0);
                     }
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[buf]);
-                tph[buf] ^= 1;
-                buf ^= 1;
-            }
-            if (ok) norm2[(int64_t)rank * M + (int64_t)mt * BM + row] = acc;
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all(); // nobody leaves while a peer may still multicast into its shared memory / barriers
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// CTA-pair variant (tcgen05 cta_group::2): the GEMM above is bound by operand delivery from L2 (11.2 TB/s measured at
-// 128 x 256 tiles, the LTS cap of the chip is ~12 TB/s), so the lever is bytes per MAC.  Two CTAs of a cluster form one
-// MMA pair: UMMA M = 256 (each CTA owns 128 candidates = its own A rows and its own TMEM lanes) and every B tile is split
-// between the two CTAs (128 of the 256 rows of L^-1 each), so B is fetched once per 256 candidates.  Each A slab is used
-// for TWO n-tiles (two 256-column accumulators = all 512 TMEM columns): per 128 x 256 x 64-MAC unit a CTA pulls
-// 8 KB (A) + 16 KB (B) instead of 8 + 32 KB.  Only the leader CTA issues MMAs; both CTAs run a TMA producer whose
-// transactions complete on the LEADER's "full" barrier; commits are multicast to both CTAs ("slot free", "accumulators
-// full"); both epilogues report "accumulators drained" to the leader.
-// ---------------------------------------------------------------------------------------------------------
-constexpr int HB_BYTES = (BN / 2) * 128;                    // half of a B tile: 128 rows x 128 B
-constexpr int PAIR_STAGE_BYTES = A_BYTES + 2 * HB_BYTES;    // A + B(n0) half + B(n1) half = 48 KB
-constexpr size_t PAIR_SMEM_BYTES = (size_t)STAGES * PAIR_STAGE_BYTES + 1024 + 256;
-
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t smem_addr, uint32_t cta)
-{
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(cta));
-    return r;
-}
-// TMA load whose bytes complete on a barrier given by its shared::cluster address (the leader's)
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const CUtensorMap* map, int c0, int c1, uint32_t bar_cluster_addr)
-{
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
-                     lb_smem_u32(dst)),
-                 "l"(map), "r"(c0), "r"(c1), "r"(bar_cluster_addr)
-                 : "memory");
-}
-template <bool F16>
-__host__ __device__ constexpr uint32_t idesc_pair()
-{
-    return (1u << 4) | ((F16 ? 0u : 2u) << 7) | ((F16 ? 0u : 2u) << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);
-}
-template <bool F16>
-__device__ __forceinline__ void umma_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
-{
-    if (F16)
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc_pair<true>()), "r"(accumulate)
-            : "memory");
-    else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "setp.ne.b32 p, %4, 0;\n\t"
-            "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-            ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc_pair<false>()), "r"(accumulate)
-            : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(lb_smem_u32(bar)),
-                 "h"((uint16_t)3)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr)
-{
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
-}
-
-// M % 256 == 0, N % 512 == 0.  norm2[c] = sum_n D[c, n]^2 (one partial per candidate).
-template <bool F16>
-__global__ void __launch_bounds__(THREADS, 1)
-pair_gemm_norm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, int64_t M, int64_t N, int64_t K,
-    int tri, float* __restrict__ norm2, int* __restrict__ err)
-{
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = (uint64_t*)(smem + (size_t)STAGES * PAIR_STAGE_BYTES);
-    uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;
-    uint64_t* tempty = tfull + 1;
-    uint32_t* tmem_base_s = (uint32_t*)(tempty + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = (int)cluster_ctarank();
-    const int pair_id = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-    const int m_pairs = (int)(M / (2 * BM)), n_groups = (int)(N / (2 * BN));
-    constexpr int BKE = bke<F16>();
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tfull, 1);
-        mbar_init(tempty, 8); // 4 epilogue warps of each CTA of the pair (leader's copy is the one waited on)
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) { // the same warp of BOTH CTAs performs the pair-wide allocation (all 512 columns)
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(lb_smem_u32(tmem_base_s)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_s;
-
-    auto kblocks_of = [&](int nt) {
-        const int64_t kend = tri ? (int64_t)(nt + 1) * BN : K;
-        return (int)((kend < K ? kend : K) / BKE);
-    };
-
-    if (warp == 0) {
-        if (lane == 0) { // ===== TMA producer (both CTAs): own A rows, own half of both B tiles; bytes land on the leader's barrier =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-                for (int grp = 0; grp < n_groups && ok; ++grp) {
-                    const int n0 = 2 * grp, n1 = n0 + 1;
-                    const int kb0 = kblocks_of(n0), kb1 = kblocks_of(n1);
-                    for (int kb = 0; kb < kb1; ++kb) {
-                        if (!mbar_wait(&empty[s], ph ^ 1, err)) { ok = false; break; }
-                        const bool has0 = kb < kb0;
-                        uint8_t* sa = smem + (size_t)s * PAIR_STAGE_BYTES;
-                        const uint32_t lfull = mapa_u32(lb_smem_u32(&full[s]), 0);
-                        if (rank == 0) mbar_expect_tx(&full[s], 2u * (uint32_t)(A_BYTES + HB_BYTES + (has0 ? HB_BYTES : 0)));
-                        tma_load_2d_pair(sa, &mapA, kb * BKE, mt * 2 * BM + rank * BM, lfull);
-                        if (has0) tma_load_2d_pair(sa + A_BYTES, &mapB, kb * BKE, n0 * BN + rank * (BN / 2), lfull);
-                        tma_load_2d_pair(sa + A_BYTES + HB_BYTES, &mapB, kb * BKE, n1 * BN + rank * (BN / 2), lfull);
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                }
-            }
-        }
-    }
-    else if (warp == 1) {
-        if (lane == 0 && rank == 0) { // ===== MMA issuer: leader CTA only =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            uint32_t tph = 0;
-            for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-                for (int grp = 0; grp < n_groups && ok; ++grp) {
-                    const int kb0 = kblocks_of(2 * grp), kb1 = kblocks_of(2 * grp + 1);
-                    if (!mbar_wait(tempty, tph ^ 1, err)) { ok = false; break; }
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int kb = 0; kb < kb1; ++kb) {
-                        if (!mbar_wait(&full[s], ph, err)) { ok = false; break; }
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sa = lb_smem_u32(smem + (size_t)s * PAIR_STAGE_BYTES);
-                        const uint64_t adesc = make_desc(sa), b0desc = make_desc(sa + A_BYTES), b1desc = make_desc(sa + A_BYTES + HB_BYTES);
-                        if (kb < kb0) {
+                if (!SPLIT && Dout) {
 #pragma unroll
-                            for (int k = 0; k < MMAS_PER_STAGE; ++k)
-                                umma_pair<F16>(tmem_base, adesc + (uint64_t)(2 * k), b0desc + (uint64_t)(2 * k), (kb | k) != 0);
-                        }
-#pragma unroll
-                        for (int k = 0; k < MMAS_PER_STAGE; ++k)
-                            umma_pair<F16>(tmem_base + (uint32_t)BN, adesc + (uint64_t)(2 * k), b1desc + (uint64_t)(2 * k), (kb | k) != 0);
-                        umma_commit_pair(&empty[s]); // slot s is free in both CTAs
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                    umma_commit_pair(tfull); // both accumulators complete, in both CTAs
-                    tph ^= 1;
+                    for (int i = 0; i < NACC; ++i)
+                        Dout[((int64_t)mt * BM + r0 + 8 * ((i >> 1) & 1)) * N + (int64_t)nt * BNT + (i >> 2) * 8 + 2 * (lane & 3) + (i & 1)] = acc[i];
                 }
             }
-        }
-    }
-    else { // ===== epilogue (both CTAs): each thread owns one candidate = one TMEM lane of its CTA =====
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t ltempty = mapa_u32(lb_smem_u32(tempty), 0);
-        uint32_t tph = 0; bool ok = true;
-        for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-            float acc = 0.f;
-            for (int grp = 0; grp < n_groups && ok; ++grp) {
-                if (!mbar_wait_warp(tfull, tph, err)) { ok = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-                for (int c = 0; c < 2 * BN; c += 32) {
-                    uint32_t v[32];
-                    tmem_ld32(taddr + c, v);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const float d = __uint_as_float(v[j]);
-                        acc = fmaf(d, d, acc);
-                    }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(ltempty);
-                tph ^= 1;
-            }
-            if (ok) norm2[(int64_t)mt * 2 * BM + rank * BM + row] = acc;
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all(); // neither CTA leaves (or frees TMEM) while the pair may still be using its memory
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// Split-operand variant of the CTA-pair kernel (LB_PREC_FP16X3): every operand is carried as hi + 2^-11 lo with hi, lo
-// both fp16 (22 significant bits), and
-//     D = A_hi B_hi + 2^-11 (A_hi B_lo + A_lo B_hi)            (the 2^-22 A_lo B_lo term is dropped)
-// is formed from three fp16 MMAs per k-step into TWO fp32 accumulators (acc0 = hi x hi in TMEM columns [0, 256),
-// acc1 = the cross terms in [256, 512)), combined in the epilogue in fp64, where sum_n D^2 is accumulated in fp64 as well.
-// One n-tile (256 rows of L^-1) per pass; otherwise the pipeline of pair_gemm_norm_kernel (both CTAs produce, the leader
-// issues, commits are multicast).  3x the MMA work and 2x the operand bytes of LB_PREC_FP16 buy |d sigma^2| ~ 1e-6 instead
-// of ~2e-3 (tests/test_gpu_config4.py).
-// ---------------------------------------------------------------------------------------------------------
-constexpr int SPLIT_STAGES = 3;
-constexpr int SPLIT_STAGE_BYTES = 2 * A_BYTES + 2 * HB_BYTES; // A_hi, A_lo, B_hi half, B_lo half = 64 KB
-constexpr size_t SPLIT_SMEM_BYTES = (size_t)SPLIT_STAGES * SPLIT_STAGE_BYTES + 1024 + 256;
-
-__global__ void __launch_bounds__(THREADS, 1)
-pair_split_gemm_norm_kernel(const __grid_constant__ CUtensorMap mapAh, const __grid_constant__ CUtensorMap mapAl,
-    const __grid_constant__ CUtensorMap mapBh, const __grid_constant__ CUtensorMap mapBl, int64_t M, int64_t N, int64_t K, int tri,
-    double* __restrict__ norm2, int* __restrict__ err)
-{
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = (uint64_t*)(smem + (size_t)SPLIT_STAGES * SPLIT_STAGE_BYTES);
-    uint64_t* empty = full + SPLIT_STAGES;
-    uint64_t* tfull = empty + SPLIT_STAGES;
-    uint64_t* tempty = tfull + 1;
-    uint32_t* tmem_base_s = (uint32_t*)(tempty + 1);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int rank = (int)cluster_ctarank();
-    const int pair_id = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-    const int m_pairs = (int)(M / (2 * BM)), n_tiles = (int)(N / BN);
-    constexpr int BKE = bke<true>();
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < SPLIT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tfull, 1);
-        mbar_init(tempty, 8);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(lb_smem_u32(tmem_base_s)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_base_s;
-
-    auto kblocks_of = [&](int nt) {
-        const int64_t kend = tri ? (int64_t)(nt + 1) * BN : K;
-        return (int)((kend < K ? kend : K) / BKE);
-    };
-
-    if (warp == 0) {
-        if (lane == 0) { // ===== TMA producer (both CTAs): own A rows (hi, lo), own half of the B tile (hi, lo) =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-                for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                    const int kbn = kblocks_of(nt);
-                    for (int kb = 0; kb < kbn; ++kb) {
-                        if (!mbar_wait(&empty[s], ph ^ 1, err)) { ok = false; break; }
-                        uint8_t* sa = smem + (size_t)s * SPLIT_STAGE_BYTES;
-                        const uint32_t lfull = mapa_u32(lb_smem_u32(&full[s]), 0);
-                        if (rank == 0) mbar_expect_tx(&full[s], 2u * (uint32_t)SPLIT_STAGE_BYTES);
-                        tma_load_2d_pair(sa, &mapAh, kb * BKE, mt * 2 * BM + rank * BM, lfull);
-                        tma_load_2d_pair(sa + A_BYTES, &mapAl, kb * BKE, mt * 2 * BM + rank * BM, lfull);
-                        tma_load_2d_pair(sa + 2 * A_BYTES, &mapBh, kb * BKE, nt * BN + rank * (BN / 2), lfull);
-                        tma_load_2d_pair(sa + 2 * A_BYTES + HB_BYTES, &mapBl, kb * BKE, nt * BN + rank * (BN / 2), lfull);
-                        if (++s == SPLIT_STAGES) { s = 0; ph ^= 1; }
-                    }
-                }
+            // the four threads of a quad hold the same two rows
+            n0 += __shfl_xor_sync(0xffffffffu, n0, 1);
+            n0 += __shfl_xor_sync(0xffffffffu, n0, 2);
+            n1 += __shfl_xor_sync(0xffffffffu, n1, 1);
+            n1 += __shfl_xor_sync(0xffffffffu, n1, 2);
+            if (ok && (lane & 3) == 0) {
+                NormT* norm2 = reinterpret_cast<NormT*>(norm2_);
+                norm2[(int64_t)mt * BM + r0] = n0;
+                norm2[(int64_t)mt * BM + r0 + 8] = n1;
             }
         }
-    }
-    else if (warp == 1) {
-        if (lane == 0 && rank == 0) { // ===== MMA issuer: leader CTA only =====
-            int s = 0; uint32_t ph = 0; bool ok = true;
-            uint32_t tph = 0;
-            for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-                for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                    const int kbn = kblocks_of(nt);
-                    if (!mbar_wait(tempty, tph ^ 1, err)) { ok = false; break; }
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    for (int kb = 0; kb < kbn; ++kb) {
-                        if (!mbar_wait(&full[s], ph, err)) { ok = false; break; }
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        const uint32_t sa = lb_smem_u32(smem + (size_t)s * SPLIT_STAGE_BYTES);
-                        const uint64_t ah = make_desc(sa), al = make_desc(sa + A_BYTES), bh = make_desc(sa + 2 * A_BYTES),
-                                       bl = make_desc(sa + 2 * A_BYTES + HB_BYTES);
-#pragma unroll
-                        for (int k = 0; k < MMAS_PER_STAGE; ++k) umma_pair<true>(tmem_base, ah + (uint64_t)(2 * k), bh + (uint64_t)(2 * k), (kb | k) != 0);
-#pragma unroll
-                        for (int k = 0; k < MMAS_PER_STAGE; ++k) {
-                            umma_pair<true>(tmem_base + (uint32_t)BN, ah + (uint64_t)(2 * k), bl + (uint64_t)(2 * k), (kb | k) != 0);
-                            umma_pair<true>(tmem_base + (uint32_t)BN, al + (uint64_t)(2 * k), bh + (uint64_t)(2 * k), 1);
-                        }
-                        umma_commit_pair(&empty[s]);
-                        if (++s == SPLIT_STAGES) { s = 0; ph ^= 1; }
-                    }
-                    umma_commit_pair(tfull);
-                    tph ^= 1;
-                }
-            }
-        }
-    }
-    else { // ===== epilogue (both CTAs): D = acc0 + 2^-11 acc1 and sum_n D^2, both in fp64 =====
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t ltempty = mapa_u32(lb_smem_u32(tempty), 0);
-        uint32_t tph = 0; bool ok = true;
-        for (int mt = pair_id; mt < m_pairs && ok; mt += npairs) {
-            double acc = 0.0;
-            for (int nt = 0; nt < n_tiles && ok; ++nt) {
-                if (!mbar_wait_warp(tfull, tph, err)) { ok = false; break; }
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-                for (int c = 0; c < BN; c += 32) {
-                    uint32_t v0[32], v1[32];
-                    tmem_ld32(taddr + c, v0);
-                    tmem_ld32(taddr + BN + c, v1);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const double d = fma((double)__uint_as_float(v1[j]), 1.0 / 2048.0, (double)__uint_as_float(v0[j]));
-                        acc = fma(d, d, acc);
-                    }
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(ltempty);
-                tph ^= 1;
-            }
-            if (ok) norm2[(int64_t)mt * 2 * BM + rank * BM + row] = acc;
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
     }
 }
 
@@ -805,7 +316,34 @@ static int make_map(CUtensorMap* map, const void* base, int64_t rows, int64_t K,
     return r == CUDA_SUCCESS ? LB_OK : LB_ERR_CUDA;
 }
 
-LbOncePerDevice g_attr_once;
+// A: M x K (ld lda), B: N x K (ld ldb), row-major; lo planes (split mode) with the same shapes.  M % 128 == 0,
+// N % (256, split: 128) == 0, K % 64 == 0.  grid: persistent CTAs (at most one per 128-candidate tile).
+template <bool F16, bool SPLIT>
+static int launch_gemm_norm(cudaStream_t st, const void* dA, const void* dAlo, int64_t lda, const void* dB, const void* dBlo, int64_t ldb,
+    int64_t M, int64_t N, int64_t K, int tri, void* dNorm2, float* dDout, int* dErr, int grid)
+{
+    using C = Cfg<SPLIT>;
+    if (M % BM || N % C::BNT || K % 64) return LB_ERR_ARG;
+    static LbOncePerDevice attr_once;
+    if (attr_once.need()) {
+        LB_CUDA(cudaFuncSetAttribute(gemm_norm_kernel<F16, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM_BYTES));
+    }
+    alignas(64) CUtensorMap mA, mB, mAlo, mBlo;
+    int rc;
+    if ((rc = make_map(&mA, dA, M, K, lda, BM, F16))) return rc;
+    if ((rc = make_map(&mB, dB, N, K, ldb, C::BNT, F16))) return rc;
+    mAlo = mA;
+    mBlo = mB;
+    if (SPLIT) {
+        if ((rc = make_map(&mAlo, dAlo, M, K, lda, BM, true))) return rc;
+        if ((rc = make_map(&mBlo, dBlo, N, K, ldb, C::BNT, true))) return rc;
+    }
+    const int m_tiles = (int)(M / BM);
+    if (grid > m_tiles) grid = m_tiles;
+    gemm_norm_kernel<F16, SPLIT><<<grid, THREADS, C::SMEM_BYTES, st>>>(mA, mB, mAlo, mBlo, M, N, K, tri, dNorm2, dDout, dErr);
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
 
 } // namespace tf32q
 
@@ -814,155 +352,15 @@ int lb_launch_tf32_gemm_norm(cudaStream_t st, const void* dA, int64_t lda, const
     int tri, float* dNorm2, float* dDout, int* dErr, int grid, int f16)
 {
     using namespace tf32q;
-    if (M % BM || N % BN || K % 64) return LB_ERR_ARG;
-    if (g_attr_once.need()) {
-        LB_CUDA(cudaFuncSetAttribute(tf32_gemm_norm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        LB_CUDA(cudaFuncSetAttribute(tf32_gemm_norm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    }
-    alignas(64) CUtensorMap mapA, mapB;
-    int rc;
-    if ((rc = make_map(&mapA, dA, M, K, lda, BM, f16 != 0))) return rc;
-    if ((rc = make_map(&mapB, dB, N, K, ldb, BN, f16 != 0))) return rc;
-    const int m_tiles = (int)(M / BM);
-    if (grid > m_tiles) grid = m_tiles;
-    if (f16) tf32_gemm_norm_kernel<true><<<grid, THREADS, SMEM_BYTES, st>>>(mapA, mapB, M, N, K, tri, dNorm2, dDout, dErr);
-    else tf32_gemm_norm_kernel<false><<<grid, THREADS, SMEM_BYTES, st>>>(mapA, mapB, M, N, K, tri, dNorm2, dDout, dErr);
-    LB_CUDA(cudaGetLastError());
-    return LB_OK;
+    return f16 ? launch_gemm_norm<true, false>(st, dA, nullptr, lda, dB, nullptr, ldb, M, N, K, tri, dNorm2, dDout, dErr, grid)
+               : launch_gemm_norm<false, false>(st, dA, nullptr, lda, dB, nullptr, ldb, M, N, K, tri, dNorm2, dDout, dErr, grid);
 }
 
-// Clustered launch: N must be a multiple of 256 * CL; dNorm2 holds CL partial rows of M floats.
-template <int CL, bool F16>
-static int launch_cluster(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, int64_t M, int64_t N, int64_t K, int tri,
-    float* dNorm2, int* dErr, int grid)
+// Split-operand launch (fp16 hi / lo planes): dA*: M x K, dB*: N x K row-major halves; M % 128 == 0, N % 128 == 0; dNorm2: M doubles.
+static int lb_launch_split_gemm_norm(cudaStream_t st, const void* dAh, const void* dAl, int64_t lda, const void* dBh, const void* dBl,
+    int64_t ldb, int64_t M, int64_t N, int64_t K, int tri, double* dNorm2, int* dErr, int grid)
 {
-    using namespace tf32q;
-    static LbOncePerDevice attr_once;
-    if (attr_once.need()) {
-        LB_CUDA(cudaFuncSetAttribute(tf32_gemm_norm_cluster_kernel<CL, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    LB_CUDA(cudaLaunchKernelEx(&cfg, tf32_gemm_norm_cluster_kernel<CL, F16>, mapA, mapB, M, N, K, tri, dNorm2, dErr));
-    return LB_OK;
-}
-
-int lb_launch_pair_gemm_norm(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N, int64_t K,
-    int tri, float* dNorm2, int* dErr, int sms, int f16);
-int lb_launch_pair_split_gemm_norm(cudaStream_t st, const void* dAh, const void* dAl, int64_t lda, const void* dBh, const void* dBl, int64_t ldb,
-    int64_t M, int64_t N, int64_t K, int tri, double* dNorm2, int* dErr, int sms);
-
-int lb_launch_tf32_gemm_norm_cluster(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N,
-    int64_t K, int tri, float* dNorm2, int* dErr, int sms, int cl, int f16)
-{
-    using namespace tf32q;
-    if (M % BM || N % (BN * cl) || K % 64 || (cl != 2 && cl != 4)) return LB_ERR_ARG;
-    alignas(64) CUtensorMap mapA, mapB;
-    int rc;
-    if ((rc = make_map(&mapA, dA, M, K, lda, BM, f16 != 0))) return rc;
-    if ((rc = make_map(&mapB, dB, N, K, ldb, BN, f16 != 0))) return rc;
-    const int m_tiles = (int)(M / BM);
-    int nclusters = sms / cl;
-    if (nclusters > m_tiles) nclusters = m_tiles;
-    const int grid = nclusters * cl;
-    if (f16)
-        return cl == 2 ? launch_cluster<2, true>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, grid)
-                       : launch_cluster<4, true>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, grid);
-    return cl == 2 ? launch_cluster<2, false>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, grid)
-                   : launch_cluster<4, false>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, grid);
-}
-
-template <bool F16>
-static int launch_pair(cudaStream_t st, const CUtensorMap& mapA, const CUtensorMap& mapB, int64_t M, int64_t N, int64_t K, int tri,
-    float* dNorm2, int* dErr, int grid)
-{
-    using namespace tf32q;
-    static LbOncePerDevice attr_once;
-    if (attr_once.need()) {
-        LB_CUDA(cudaFuncSetAttribute(pair_gemm_norm_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PAIR_SMEM_BYTES));
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)grid);
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = PAIR_SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    LB_CUDA(cudaLaunchKernelEx(&cfg, pair_gemm_norm_kernel<F16>, mapA, mapB, M, N, K, tri, dNorm2, dErr));
-    return LB_OK;
-}
-
-// CTA-pair (cta_group::2) launch: M % 256 == 0, N % 512 == 0; dNorm2 holds M floats.
-int lb_launch_pair_gemm_norm(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N, int64_t K,
-    int tri, float* dNorm2, int* dErr, int sms, int f16)
-{
-    using namespace tf32q;
-    if (M % (2 * BM) || N % (2 * BN) || K % 64) return LB_ERR_ARG;
-    alignas(64) CUtensorMap mapA, mapB;
-    int rc;
-    if ((rc = make_map(&mapA, dA, M, K, lda, BM, f16 != 0))) return rc;
-    if ((rc = make_map(&mapB, dB, N, K, ldb, BN / 2, f16 != 0))) return rc;
-    int npairs = sms / 2;
-    if (npairs > M / (2 * BM)) npairs = (int)(M / (2 * BM));
-    return f16 ? launch_pair<true>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, 2 * npairs)
-               : launch_pair<false>(st, mapA, mapB, M, N, K, tri, dNorm2, dErr, 2 * npairs);
-}
-
-// Split-operand launch (fp16 hi / lo planes): dA*: M x K, dB*: N x K row-major halves; M % 256 == 0, N % 256 == 0; dNorm2: M doubles.
-int lb_launch_pair_split_gemm_norm(cudaStream_t st, const void* dAh, const void* dAl, int64_t lda, const void* dBh, const void* dBl, int64_t ldb,
-    int64_t M, int64_t N, int64_t K, int tri, double* dNorm2, int* dErr, int sms)
-{
-    using namespace tf32q;
-    if (M % (2 * BM) || N % BN || K % 64) return LB_ERR_ARG;
-    static LbOncePerDevice attr_once;
-    if (attr_once.need()) {
-        LB_CUDA(cudaFuncSetAttribute(pair_split_gemm_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPLIT_SMEM_BYTES));
-    }
-    alignas(64) CUtensorMap mAh, mAl, mBh, mBl;
-    int rc;
-    if ((rc = make_map(&mAh, dAh, M, K, lda, BM, true))) return rc;
-    if ((rc = make_map(&mAl, dAl, M, K, lda, BM, true))) return rc;
-    if ((rc = make_map(&mBh, dBh, N, K, ldb, BN / 2, true))) return rc;
-    if ((rc = make_map(&mBl, dBl, N, K, ldb, BN / 2, true))) return rc;
-    int npairs = sms / 2;
-    if (npairs > M / (2 * BM)) npairs = (int)(M / (2 * BM));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(2 * npairs));
-    cfg.blockDim = dim3(THREADS);
-    cfg.dynamicSmemBytes = SPLIT_SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    LB_CUDA(cudaLaunchKernelEx(&cfg, pair_split_gemm_norm_kernel, mAh, mAl, mBh, mBl, M, N, K, tri, dNorm2, dErr));
-    return LB_OK;
-}
-
-extern "C" int lb_debug_pair_gemm(const void* dA, const void* dB, long long M, long long N, long long K, int tri, float* dNorm2, int f16)
-{
-    int* dErr = nullptr;
-    LB_CUDA(cudaMalloc(&dErr, sizeof(int)));
-    LB_CUDA(cudaMemset(dErr, 0, sizeof(int)));
-    int rc = lb_launch_pair_gemm_norm(0, dA, K, dB, K, M, N, K, tri, dNorm2, dErr, 148, f16);
-    if (rc) { cudaFree(dErr); return rc; }
-    LB_CUDA(cudaDeviceSynchronize());
-    int herr = 0;
-    LB_CUDA(cudaMemcpy(&herr, dErr, sizeof(int), cudaMemcpyDeviceToHost));
-    cudaFree(dErr);
-    return herr ? LB_ERR_TIMEOUT : LB_OK;
+    return tf32q::launch_gemm_norm<true, true>(st, dAh, dAl, lda, dBh, dBl, ldb, M, N, K, tri, dNorm2, nullptr, dErr, grid);
 }
 
 __global__ void debug_exp_kernel(const double* in, double* out, long long n)
@@ -978,21 +376,6 @@ extern "C" int lb_debug_exp(const double* dIn, double* dOut, long long n)
     LB_CUDA(cudaGetLastError());
     LB_CUDA(cudaDeviceSynchronize());
     return LB_OK;
-}
-
-extern "C" int lb_debug_tf32_gemm_cluster(const void* dA, const void* dB, long long M, long long N, long long K, int tri, float* dNorm2,
-    int cl, int f16)
-{
-    int* dErr = nullptr;
-    LB_CUDA(cudaMalloc(&dErr, sizeof(int)));
-    LB_CUDA(cudaMemset(dErr, 0, sizeof(int)));
-    int rc = lb_launch_tf32_gemm_norm_cluster(0, dA, K, dB, K, M, N, K, tri, dNorm2, dErr, 148, cl, f16);
-    if (rc) { cudaFree(dErr); return rc; }
-    LB_CUDA(cudaDeviceSynchronize());
-    int herr = 0;
-    LB_CUDA(cudaMemcpy(&herr, dErr, sizeof(int), cudaMemcpyDeviceToHost));
-    cudaFree(dErr);
-    return herr ? LB_ERR_TIMEOUT : LB_OK;
 }
 
 extern "C" int lb_debug_tf32_gemm(const void* dA, const void* dB, long long M, long long N, long long K, int tri, float* dNorm2,
@@ -1015,7 +398,7 @@ extern "C" int lb_debug_tf32_gemm(const void* dA, const void* dB, long long M, l
 // ===========================================================================
 namespace tf32q {
 
-// fp32 -> tf32 with round-to-nearest: tcgen05.mma.kind::tf32 ignores the low 13 mantissa bits of its operands, i.e. truncates;
+// fp32 -> tf32 with round-to-nearest: the tf32 wgmma ignores the low 13 mantissa bits of its operands, i.e. truncates;
 // a truncated operand is biased low, and the bias of |L^-1 k*|^2 does not average out over the N terms of the sum.
 __device__ __forceinline__ float tf32_rna(float v)
 {
@@ -1034,9 +417,8 @@ constexpr int DCH_WIDE = 16; // input dimensions staged per pass
 // same kernel runs one tile per CTA or as a small persistent grid.
 // Squared distances on the fp64 TENSOR pipe: z_cn = |q_c|^2 + |x_n|^2 - 2 q_c . x_n with the cross term as an
 // mma.m8n8k4.f64 (candidates = M side, training points = N side, input dimensions = K, zero padded to a multiple of 4).
-// ncu on the FMA version of this kernel showed the fp64 ALU pipe 61 % active and the tensor pipe idle, and on the DMMA GEMMs
-// the reverse (profiles/r01_ncu_*): the two are separate pipes, so moving the D-loop (24 of ~55 fp64 operations per pair at
-// D = 12) to DMMA leaves the ALU pipe to exp / scaling / the mean and bias partials.  The cancellation costs ~1e-16 (|q|^2 +
+// Moving the D-loop (24 of ~55 fp64 operations per pair at D = 12) to DMMA leaves the fp64 ALU pipe to exp / scaling / the
+// mean and bias partials.  The cancellation costs ~1e-16 (|q|^2 +
 // |x|^2) absolute on z, i.e. <= 1e-13 relative on k: inside the 1e-9 bar this path states for mu.
 // A thread ends up with candidate g (+ 8 mb) x training points 2t, 2t+1 (+ 8 nb): two consecutive K-major elements = one
 // half2 / float2 store.
@@ -1350,13 +732,12 @@ sigma2_split_kernel(const double* __restrict__ norm2, int64_t M, double kvv, dou
 }
 
 __global__ void __launch_bounds__(256)
-sigma2_t32_kernel(const float* __restrict__ norm2, int nparts, int64_t part_stride, int64_t M, double kvv, double noise,
-    double norm_unscale, const double* __restrict__ bias, double bias_coeff, double* __restrict__ s2)
+sigma2_t32_kernel(const float* __restrict__ norm2, int64_t M, double kvv, double noise, double norm_unscale,
+    const double* __restrict__ bias, double bias_coeff, double* __restrict__ s2)
 {
     const int64_t c = blockIdx.x * (int64_t)256 + threadIdx.x;
     if (c >= M) return;
-    double nrm = 0.0;
-    for (int p = 0; p < nparts; ++p) nrm += (double)norm2[(int64_t)p * part_stride + c]; // partial sums of the cluster's CTAs
+    const double nrm = (double)norm2[c];
     // Rounding both operands to an 11-bit significand adds zero-mean noise e_n to every D[c, n]; sum_n D^2 then carries the
     // positive bias E sum e_n^2 = 2 u_r^2 sum_k k*_k^2 |L^-1 e_k|^2 (u_r^2 = E[relative rounding error^2]), which grows with
     // cond(K) while the zero-mean part does not (DESIGN.md §4.5): subtract its expectation.
@@ -1370,32 +751,7 @@ sigma2_t32_kernel(const float* __restrict__ norm2, int nparts, int64_t part_stri
 int lb_launch_linv(lb_gp* h);
 
 
-// CTAs per cluster sharing one candidate tile (A operand multicast).  Measured at N=16384, 1M candidates: 1 -> 518 ms,
-// 2 -> 467 ms, 4 -> 726 ms (lock-step coupling of four CTAs costs more than the saved HBM stream): default 2;
-// LB_TF32_CLUSTER=1|2|4 overrides.
-int lb_tf32_cluster_size()
-{
-    static int cl = 0;
-    if (!cl) {
-        const char* e = getenv("LB_TF32_CLUSTER");
-        cl = e ? atoi(e) : 2;
-        if (cl != 1 && cl != 2 && cl != 4) cl = 2;
-    }
-    return cl;
-}
-
-// CTA-pair kernel (cta_group::2, pair_gemm_norm_kernel) unless LB_TF32_PAIR=0: config 4 fp16 GEMM 229 -> see DESIGN.md §4.5
-int lb_tf32_pair_mode()
-{
-    static int pm = -1;
-    if (pm < 0) {
-        const char* e = getenv("LB_TF32_PAIR");
-        pm = e ? (atoi(e) != 0) : 1;
-    }
-    return pm;
-}
-
-// Prepare the row-major reduced-precision copy of L^-1 (rows padded with zeros to a multiple of 256 * cluster size).
+// Prepare the row-major reduced-precision copy of L^-1 (rows padded with zeros to a multiple of the 256-row n-tile).
 // fp32 (tf32 MMA) stores L^-1 as is; fp16 stores L^-1 * 2^e with e chosen so that max |.| <= 2^14.
 int lb_tf32_prepare(lb_gp* h)
 {
@@ -1405,8 +761,7 @@ int lb_tf32_prepare(lb_gp* h)
     const bool f16 = (h->precision == 2) || split;
     int rc;
     if (!h->linv_valid && (rc = lb_launch_linv(h))) return rc;
-    const int cl = lb_tf32_pair_mode() ? 2 : lb_tf32_cluster_size(); // the pair kernel walks two 256-row n-tiles per group
-    const int64_t Np = h->Np, Nr = (Np + BN * cl - 1) / (BN * cl) * (BN * cl);
+    const int64_t Np = h->Np, Nr = (Np + BN - 1) / BN * BN;
     const size_t esz = split ? 4 : (f16 ? 2 : 4); // split: two fp16 planes of Nr x Np
     if (!h->dLinv32 || h->linv32_rows != Nr) {
         lb_dfree_sync(h, h->dLinv32);
@@ -1516,8 +871,7 @@ int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all)
 {
     using namespace tf32q;
     const bool split = (h->precision == 3), f16 = (h->precision == 2) || split;
-    const int cl = lb_tf32_pair_mode() ? 2 : lb_tf32_cluster_size();
-    const int64_t Np = h->Np, Nr = (Np + BN * cl - 1) / (BN * cl) * (BN * cl), ldr = lb_linv_columns_width(h, G);
+    const int64_t Np = h->Np, Nr = (Np + BN - 1) / BN * BN, ldr = lb_linv_columns_width(h, G);
     const int T = (int)(Np / LB_TILE);
     const size_t esz = split ? 4 : (f16 ? 2 : 4), el = f16 ? 2 : 4;
     double scale;
@@ -1554,10 +908,6 @@ int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all)
 }
 
 // K*^T chunk (reduced precision, K-major) and mu (M x P, fp64) for Mc candidates.
-// (Tried and dropped: running this build for chunk i+1 on a second stream under the tcgen05 GEMM of chunk i.  Even with a
-// 13 KB / 104-register variant, cp.async staging, dynamic tile hand-out, polite mbarrier waits and the full 228 KB carve-out on
-// the GEMM, the fp64 CTAs made almost no progress while the GEMM CTA was resident and slowed it by 15 %: 272-285 ms per 1M
-// candidates against 256 ms for plain back-to-back launches, profiles/r01_config4_notes.txt.)
 int lb_launch_kstar_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, const double* dQs, int64_t Mcp, float* dKt, double* dMuPart,
     double* dMu, double* dBias, long long* launches)
 {
@@ -1603,7 +953,7 @@ int lb_launch_kstar_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, const doub
     return LB_OK;
 }
 
-// sigma2 (M, fp64 container of a reduced-precision value) from a K*^T chunk: tcgen05 GEMM + row norms, then the clamp / noise of gp.hpp:618-624
+// sigma2 (M, fp64 container of a reduced-precision value) from a K*^T chunk: wgmma GEMM + row norms, then the clamp / noise of gp.hpp:618-624
 int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mcp, const float* dKt, float* dNorm2, int* dErr,
     const double* dBias, double* dS2, long long* launches)
 {
@@ -1612,39 +962,33 @@ int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mc
     const bool f16 = (h->precision == 2) || split;
     const int64_t Np = h->Np;
     const double kscale = f16 ? 1.0 / h->kp.sf2 : 1.0;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    // D was computed from (K* kscale) and (L^-1 scale): |V|^2 = norm / (kscale scale)^2
+    const double unscale = 1.0 / ((kscale * h->linv32_scale) * (kscale * h->linv32_scale));
     int rc;
     if (split) { // hi / lo planes, three MMAs per k-step, fp64 combination and norm (dNorm2 holds Mcp doubles)
-        if (Mcp % (2 * BM) || h->linv32_rows % BN) return LB_ERR_ARG;
         const __half* Ah = reinterpret_cast<const __half*>(dKt);
         const __half* Bh = reinterpret_cast<const __half*>(h->dLinv32);
         {
             LbProfScope ps(h, st, LB_PC_QSTEP);
-            rc = lb_launch_pair_split_gemm_norm(st, Ah, Ah + Mcp * Np, Np, Bh, Bh + h->linv32_rows * Np, Np, Mcp, h->linv32_rows, Np, 1,
+            rc = lb_launch_split_gemm_norm(st, Ah, Ah + Mcp * Np, Np, Bh, Bh + h->linv32_rows * Np, Np, Mcp, h->linv32_rows, Np, 1,
                 reinterpret_cast<double*>(dNorm2), dErr, sms);
         }
         if (rc) return rc;
-        const double un = 1.0 / ((kscale * h->linv32_scale) * (kscale * h->linv32_scale));
-        sigma2_split_kernel<<<(unsigned)((Mc + 255) / 256), 256, 0, st>>>(reinterpret_cast<const double*>(dNorm2), Mc, h->kp.sf2, h->kp.noise, un, dS2);
+        sigma2_split_kernel<<<(unsigned)((Mc + 255) / 256), 256, 0, st>>>(reinterpret_cast<const double*>(dNorm2), Mc, h->kp.sf2, h->kp.noise, unscale, dS2);
         if (launches) *launches += 2;
         LB_CUDA(cudaGetLastError());
         return LB_OK;
     }
-    const bool pair = lb_tf32_pair_mode() && (Mcp % (2 * BM) == 0) && (h->linv32_rows % (2 * BN) == 0);
-    const int cl = pair ? 1 : lb_tf32_cluster_size(); // number of partial norms per candidate
     {
         LbProfScope ps(h, st, LB_PC_QSTEP);
-        if (pair) rc = lb_launch_pair_gemm_norm(st, dKt, Np, h->dLinv32, Np, Mcp, h->linv32_rows, Np, 1, dNorm2, dErr, sms, f16);
-        else if (cl == 1) rc = lb_launch_tf32_gemm_norm(st, dKt, Np, h->dLinv32, Np, Mcp, h->linv32_rows, Np, 1, dNorm2, nullptr, dErr, sms, f16);
-        else rc = lb_launch_tf32_gemm_norm_cluster(st, dKt, Np, h->dLinv32, Np, Mcp, h->linv32_rows, Np, 1, dNorm2, dErr, sms, cl, f16);
+        rc = lb_launch_tf32_gemm_norm(st, dKt, Np, h->dLinv32, Np, Mcp, h->linv32_rows, Np, 1, dNorm2, nullptr, dErr, sms, f16);
     }
     if (rc) return rc;
-    // D was computed from (K* kscale) and (L^-1 scale): |V|^2 = norm / (kscale scale)^2
-    const double unscale = 1.0 / ((kscale * h->linv32_scale) * (kscale * h->linv32_scale));
     // u_r^2 for round-to-nearest with an 11-bit significand and log-uniform mantissas: (2^-22 / 3) * 0.541; both operands: x 2
     const double bias_coeff = 2.0 * (1.0 / 4194304.0 / 3.0) * 0.541;
-    sigma2_t32_kernel<<<(unsigned)((Mc + 255) / 256), 256, 0, st>>>(dNorm2, cl, Mcp, Mc, h->kp.sf2, h->kp.noise, unscale, dBias, bias_coeff, dS2);
+    sigma2_t32_kernel<<<(unsigned)((Mc + 255) / 256), 256, 0, st>>>(dNorm2, Mc, h->kp.sf2, h->kp.noise, unscale, dBias, bias_coeff, dS2);
     if (launches) *launches += 2;
     LB_CUDA(cudaGetLastError());
     return LB_OK;

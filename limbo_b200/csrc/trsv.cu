@@ -11,10 +11,9 @@
 // is bounded: on timeout info[1] is set and LB_ERR_TIMEOUT returned).
 //
 // The dependency chain (T sequential blocks) is what bounds these kernels, not
-// HBM: round 1 measured 0.77 + 1.0 ms for 2 x 1.07 GB (0.18 of the HBM
-// roofline) with a flag per block (poll flag -> barrier -> load x_j: two L2 round
-// trips per step) and the diagonal-block inverse fetched from L2 only after the
-// last x_j had arrived.  Now
+// HBM.  A flag per block (poll flag -> barrier -> load x_j) would cost two L2 round
+// trips per step, and fetching the diagonal-block inverse only after the last x_j
+// had arrived would add a third.  Instead
 //   * the solution is published through a scratch vector pre-filled with a
 //     sentinel: consumers poll the 8-byte VALUES themselves (one round trip, no
 //     ordering between elements needed);

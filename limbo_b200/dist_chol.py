@@ -30,8 +30,7 @@ _PANEL_GROUP = None
 def panel_group():
     """Process group for the panel broadcasts whose NCCL kernels run on a HIGH-PRIORITY stream.  The trailing update keeps
     every SM full (two resident CTAs per SM, thousands of blocks pending); a broadcast kernel launched at default priority is
-    only scheduled once the update has drained, i.e. the exchange step would not overlap the update at all (measured round 2:
-    every broadcast ended right after the previous update, profiles/r02_dchol_timeline_n2.txt).  Collective: every rank must
+    only scheduled once the update has drained, i.e. the exchange step would not overlap the update at all.  Collective: every rank must
     call it (DistCholesky does, at construction).  Falls back to the default group when the option is unavailable."""
     global _PANEL_GROUP
     import torch.distributed as dist

@@ -1,7 +1,7 @@
 """Inversion of the factor spread over the ranks, for the reduced-precision candidate path (BASELINE.json config 4 on several
-GPUs).  sigma^2(v) = k(v,v) - |L^-1 k(v)|^2 (model/gp.hpp:618-624) is scored on the tcgen05 path against a reduced-precision copy
-of ALL of L^-1 on every rank, the candidates being sharded (limbo_b200.dist.sharded_acq_argmax).  Round 1 inverted the factor on
-every rank (45 ms at N = 16384: the Amdahl term once the fit is distributed, dist_fit.py).  The columns of a triangular inverse
+GPUs).  sigma^2(v) = k(v,v) - |L^-1 k(v)|^2 (model/gp.hpp:618-624) is scored on the wgmma path against a reduced-precision copy
+of ALL of L^-1 on every rank, the candidates being sharded (limbo_b200.dist.sharded_acq_argmax).  Inverting the whole factor on
+every rank would be the Amdahl term once the fit is distributed (dist_fit.py).  The columns of a triangular inverse
 are independent, so here rank r computes the 128-column tiles r, r + G, r + 2G, ... with the blocked solve of the batched query
 path on identity columns (N^3 / (3 G) flops on the fp64 tensor cores), casts them to the storage type of the handle's precision,
 and ONE all_gather of the chunks (N^2 / G reduced-precision elements per rank) gives every rank the whole copy.

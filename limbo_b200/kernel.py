@@ -68,7 +68,7 @@ class SquaredExpARD(BaseKernel):
         super().__init__(params, dim)
         self._k = int(get(params, "kernel_squared_exp_ard", "k"))
         if self._k < 0 or self._k > 4:
-            raise NotImplementedError("SquaredExpARD: the B200 backend supports 0 <= k <= 4 Lambda columns")
+            raise NotImplementedError("SquaredExpARD: the CUDA backend supports 0 <= k <= 4 Lambda columns")
         p = np.zeros(dim + dim * self._k + 1)  # squared_exp_ard.hpp:85-87
         p[-1] = math.log(math.sqrt(float(get(params, "kernel_squared_exp_ard", "sigma_sq"))))
         self.set_params(p)

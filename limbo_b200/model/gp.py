@@ -1,5 +1,5 @@
 """limbo_b200.model.GP — drop-in mirror of limbo::model::GP (src/limbo/model/gp.hpp:81-511)
-whose numerical work runs on the B200 through the C ABI (include/limbo_b200.h).
+whose numerical work runs on the GPU through the C ABI (include/limbo_b200.h).
 
 Same member names, argument meaning and error behaviour as the reference's
 template (asserts where the reference asserts).  Extensions that the

@@ -21,7 +21,7 @@
 // a bit-exact target.
 //
 // Every function cites the reference file:line it follows (paths relative to
-// /root/reference/src/limbo/).
+// the reference's src/limbo/).
 #pragma once
 #include <algorithm>
 #include <cfloat>

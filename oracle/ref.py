@@ -1,7 +1,8 @@
 """ctypes front-end of oracle/_ref/libref_gp.so: the reference's OWN GP code
-(/root/reference/src/limbo headers) compiled against the Eigen/Boost stand-in
-(oracle/ref_shim/).  TEST INFRASTRUCTURE ONLY; exists only where the reference
-is mounted (this container) — the GPU box relies on tests/golden/*.npz."""
+(the src/limbo headers of a resibots/limbo checkout) compiled against the Eigen/Boost
+stand-in (oracle/ref_shim/).  TEST INFRASTRUCTURE ONLY; built only where the reference's
+sources are present (LIMBO_REFERENCE_SRC, default: a `reference` checkout next to this
+repository) — elsewhere the tests rely on tests/golden/."""
 from __future__ import annotations
 
 import ctypes as C
@@ -12,7 +13,8 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "_ref", "libref_gp.so")
-REF_SRC = "/root/reference/src/limbo"
+REF_ROOT = os.environ.get("LIMBO_REFERENCE_SRC", os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference", "src"))
+REF_SRC = os.path.join(REF_ROOT, "limbo")
 
 
 def available() -> bool:
@@ -21,7 +23,7 @@ def available() -> bool:
 
 def build() -> str:
     if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "CXX=g++"], check=True, capture_output=True)
+        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "CXX=g++", f"REF={REF_ROOT}"], check=True, capture_output=True)
     return LIB_PATH
 
 

@@ -1,7 +1,7 @@
 // oracle/ref_shim/ref_driver.cpp — TEST INFRASTRUCTURE ONLY.
 //
 // Runs the REFERENCE'S OWN hot-path code (headers included from
-// /root/reference/src where they lie: limbo/model/gp.hpp, kernel/*.hpp,
+// the reference's src/ where they lie: limbo/model/gp.hpp, kernel/*.hpp,
 // mean/data.hpp, acqui/ucb.hpp, acqui/ei.hpp, model/gp/kernel_lf_opt.hpp,
 // opt/rprop.hpp) with the dense linear algebra supplied by the stand-in in
 // ./Eigen.  Used to pin oracle/limbo_oracle.hpp (tests/test_oracle_vs_ref.py)

@@ -1,8 +1,8 @@
 // tests/cpp/dropin_test.cpp — the drop-in claim, compiled: the reference's OWN policy templates
 // (acqui::UCB, acqui::EI, model::gp::KernelLFOpt / KernelLooOpt / KernelMeanLFOpt<Params, opt::Rprop>, kernel::*, mean::* from
-// /root/reference/src/limbo) instantiated over limbo_b200::model::GP and, side by side, over the
+// the reference's src/limbo) instantiated over limbo_b200::model::GP and, side by side, over the
 // reference's limbo::model::GP; results must agree to the fp64 bar.  Needs a GPU to run.
-// (Eigen is the stand-in from oracle/ref_shim because the image has no Eigen.)
+// (Eigen is the stand-in from oracle/ref_shim so that no Eigen install is needed.)
 #include <cstdio>
 #include <limbo/acqui/ei.hpp>
 #include <limbo/acqui/ucb.hpp>

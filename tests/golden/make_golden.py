@@ -1,7 +1,7 @@
 """Generates tests/golden/*.npz by running the REFERENCE'S OWN code
-(oracle/_ref/libref_gp.so = /root/reference/src/limbo headers compiled against the
-Eigen/Boost stand-in, see oracle/ref_shim/) on seeded inputs.  Run in the container that
-mounts /root/reference:   python tests/golden/make_golden.py
+(oracle/_ref/libref_gp.so = the reference's src/limbo headers compiled against the
+Eigen/Boost stand-in, see oracle/ref_shim/) on seeded inputs.  Run where __graft_entry__.build()
+has built that library:   python tests/golden/make_golden.py
 The fixtures pin the kernel formulas, noise placement, mean::Data, clamp, +noise, log-lik,
 gradient, UCB / EI (with the reference's f_max loop) and the incremental Cholesky path."""
 import os

@@ -1,7 +1,7 @@
 """Generates tests/golden/loo/*.npz from the REFERENCE'S OWN code (oracle/_ref/libref_gp.so, see make_golden.py):
  * loo_*       : GP::compute_log_loo_cv / compute_kernel_grad_log_loo_cv            (gp.hpp:339-399)
  * meangrad_*  : GP::compute_log_lik / compute_mean_grad_log_lik with mean::FunctionARD<mean::Constant>  (gp.hpp:313-330)
-Run in the container that mounts /root/reference:   python tests/golden/make_golden_loo.py"""
+Run where oracle/_ref/libref_gp.so is built:   python tests/golden/make_golden_loo.py"""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """Golden vectors produced by the REFERENCE'S OWN code (tests/golden/make_golden.py runs
-/root/reference/src/limbo's gp.hpp / kernels / acqui / rprop compiled against the Eigen stand-in).
+the reference's src/limbo gp.hpp / kernels / acqui / rprop compiled against the Eigen stand-in).
  * CPU (`not gpu`): the oracle restatement reproduces every fixture;
  * GPU (`gpu`)    : the CUDA path reproduces every fixture through the reference-facing API.
 Tolerances: 1e-10 absolute on K, mu, sigma^2, UCB, EI (BASELINE.json); alpha / log-lik / gradient

@@ -1,6 +1,6 @@
 """Multi-GPU Cholesky building blocks (limbo_b200/dist_chol.py, potrf.cu lb_dchol_*) on ONE GPU (world = 1: same panel /
 pack / update kernels, streams and look-ahead as on 8 GPUs, no NCCL) against the single-GPU factor of lb_fit and the oracle.
-The multi-rank run is tools/dist_chol_run.py under torchrun (profiles/r01_config5_*.json); the rank logic itself is
+The multi-rank run is tools/dist_chol_run.py under torchrun; the rank logic itself is
 covered on CPU by tests/test_dist_gloo.py."""
 import numpy as np
 import pytest

@@ -1,13 +1,11 @@
-"""TF32 prediction path (BASELINE.json config 4): sigma^2 from a tcgen05 tf32 GEMM with fp32 accumulation, against the
+"""TF32 prediction path (BASELINE.json config 4): sigma^2 from a wgmma tf32 GEMM with fp32 accumulation, against the
 fp64 DMMA path on the same model.  Stated tolerances (tf32 has a 10-bit mantissa; sigma^2 = k(v,v) - |L^-1 k*|^2
 subtracts two O(1) numbers, SURVEY.md §7):  |d sigma^2| <= 4e-3 k(v,v),  |d mu| <= 1e-9 (the mean is accumulated in fp64 from fp64 kernel values);
 the acquisition argmax is judged on the EI value, not on index equality.
 The sigma^2 error is the rounding of the two operands to an 11-bit significand (identical for tf32 and fp16, both rounded to
 nearest).  |L^-1 k*|^2 picks up (a) zero-mean noise and (b) a positive bias 2 u_r^2 sum_k k*_k^2 |L^-1 e_k|^2 that grows with
-cond(K); (b) is subtracted in expectation (sigma2_t32_kernel; the weights come out of the K* build).  Measured maxima
-(tools/reduced_precision_error.py), without -> with the correction: 4.2e-3 -> 2.8e-3 (Exp, N = 513), 2.5e-3 -> 2.0e-3
-(SE-ARD, N = 1000, D = 12), 2.9e-3 -> 2.3e-3 (Matern-5/2, N = 700), 6.4e-3 -> 2.8e-3 (SE-ARD l = 1, N = 4096, D = 6);
-mean error 1e-3 -> 1e-4."""
+cond(K); (b) is subtracted in expectation (sigma2_t32_kernel; the weights come out of the K* build).
+tools/reduced_precision_error.py prints the errors with and without that correction."""
 import numpy as np
 import pytest
 

@@ -1,7 +1,7 @@
 // tools/microbench.cu — measures the fp64 roofline denominators this backend is
 // judged against on the actual box (MEASURED_PEAKS.json only holds HBM copy and
 // bf16): DMMA (mma.sync f64) and DFMA peak, HBM write-only and copy bandwidth.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o microbench tools/microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o microbench tools/microbench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); return 1; } } while (0)

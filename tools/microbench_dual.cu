@@ -1,9 +1,8 @@
 // tools/microbench_dual.cu — can the fp64 tensor pipe (DMMA, mma.sync f64) and the fp64 ALU pipe (DFMA) run at the same
-// time on sm_100a, and how much of each?  (ncu showed the fp64 ALU pipe at 0 % while the DMMA kernels are bound by the tensor
-// pipe: VERDICT round 1, item 5.)  Three arrangements, all register resident (no memory traffic):
+// time on sm_90a, and how much of each?  Three arrangements, all register resident (no memory traffic):
 //   split : W_T warps of a CTA issue only DMMA, W_A warps only DFMA (warp specialisation);
 //   mixed : every warp interleaves R DFMA per DMMA.8x8x4 in its instruction stream;
-// Prints one JSON object.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/microbench_dual tools/microbench_dual.cu
+// Prints one JSON object.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/microbench_dual tools/microbench_dual.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #define CK(x) do { cudaError_t e = (x); if (e != cudaSuccess) { printf("CUDA error %s at %d\n", cudaGetErrorString(e), __LINE__); return 1; } } while (0)

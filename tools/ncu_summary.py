@@ -1,4 +1,4 @@
-"""Summarise ncu captures into small text files for profiles/.
+"""Summarise ncu captures into small text files.
   python tools/ncu_summary.py launches <csv>            -> per-kernel totals and shares
   python tools/ncu_summary.py kernel <file.ncu-rep>     -> key metrics + top stall reasons + hottest SASS lines
 """
