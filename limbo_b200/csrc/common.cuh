@@ -199,23 +199,35 @@ __device__ __forceinline__ uint32_t lb_smem_u32(const void* p)
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// fp64 tensor-core MMA (DMMA).  wgmma has no f64 kind; on sm_90a the fp64
-// tensor path is warp-level mma.sync, which ptxas lowers to DMMA.8x8x4.
-//   A frag (16x8, row): a[i]: row = g + 8*(i&1), col = t + 4*(i>>1)
-//   B frag (8x8,  col): b[i]: k = t + 4*i, n = g
-//   C frag (16x8)     : c[i]: row = g + 8*(i>>1), col = 2*t + (i&1)
-// with g = lane>>2, t = lane&3.
-__device__ __forceinline__ void lb_dmma_16x8x8(double (&c)[4], const double (&a)[4], const double (&b)[2])
+// fp64 tensor-core MMA (DMMA).  wgmma has no f64 kind; on sm_90a the fp64 tensor path is warp-level mma.sync.
+// The m16n8k{4,8,16} f64 shapes exist from sm_90 on, and ptxas keeps each of them as ONE native instruction
+// (DMMA.16x8x4 / DMMA.16x8x8 / DMMA.16x8x16).  Fragments of m16n8kK (KS = K):
+//   A frag (16xK, row): a[i], i < KS/2: row = g + 8*(i&1), col = t + 4*(i>>1)
+//   B frag (Kx8,  col): b[i], i < KS/4: k = t + 4*i, n = g
+//   C frag (16x8)     : c[i], i < 4   : row = g + 8*(i>>1), col = 2*t + (i&1)
+// with g = lane>>2, t = lane&3.  The C fragment is the same for every K (and equals two stacked m8n8k4 C fragments).
+template <int KS>
+__device__ __forceinline__ void lb_dmma_16x8(double (&c)[4], const double (&a)[KS / 2], const double (&b)[KS / 4])
 {
-    asm volatile(
-        "mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-        : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
-        : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+    static_assert(KS == 4 || KS == 8 || KS == 16, "f64 mma.sync shapes: m16n8k4, m16n8k8, m16n8k16");
+    if constexpr (KS == 4)
+        asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+    else if constexpr (KS == 8)
+        asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+    else
+        asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                     "{%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+                     : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                     : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                       "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
 }
 
-// The native SASS shape.  ptxas lowers one m16n8k8 into FOUR chained DMMA.8x8x4 (k0-3 -> temp -> k4-7 per row
-// half), i.e. no instruction-level parallelism inside a warp; issuing m8n8k4 ourselves, one independent tile after
-// the other, keeps dependent DMMAs a whole tile-sweep apart.
+// m8n8k4 (DMMA.8x8x4), the only f64 shape before sm_90.  The GEMM core and the diagonal-block kernel use the
+// m16n8kK shapes above; the single-point / slab query kernels and the tf32 path's K* dot products still issue this one.
 //   a: A[row g][k t]   b: B[k t][n g]   c0,c1: C[row g][cols 2t, 2t+1]
 __device__ __forceinline__ void lb_dmma_8x8x4(double& c0, double& c1, double a, double b)
 {

@@ -24,12 +24,14 @@ namespace lbg {
 
 constexpr int BM = 128;
 constexpr int STAGES = 3;
+// k extent of one DMMA: every product of the core is a chain of m16n8k<MMA_K> steps (DESIGN.md §4.1).  All callers
+// share it, so a tile's accumulator sees the same sequence of DMMAs whatever the launch scheme (the bit-identity of
+// the pair / quad / distributed factorisations rests on that).
+constexpr int MMA_K = 4;
 
-// DF_ = number of n8-tiles per warp (0 or 1, the last ones) whose 32 x 8 strip is computed with plain DFMA instead of DMMA
-// (the LB_SYRK_DF=1 experiment: part of the tile on the fp64 ALU pipe beside DMMA; off by default).
-template <int BN_, int WN_, int BK_, int DF_ = 0>
+template <int BN_, int WN_, int BK_>
 struct Cfg {
-    static constexpr int BN = BN_, WN = WN_, BK = BK_, DF = DF_;
+    static constexpr int BN = BN_, WN = WN_, BK = BK_;
     static constexpr int THREADS = 128 * WN;
     static constexpr int NT = BN / (8 * WN);      // n8 tiles per warp
     static constexpr int PITCH_A_OC = BM + 4;     // [BK][128+4]
@@ -39,48 +41,44 @@ struct Cfg {
     static constexpr int B_STAGE = (BN * PITCH_KC > BK * PITCH_B_OC) ? BN * PITCH_KC : BK * PITCH_B_OC;
     static constexpr size_t PIPE_BYTES = (size_t)STAGES * (A_STAGE + B_STAGE) * sizeof(double);
     static constexpr int A_PIPE_DOUBLES = STAGES * A_STAGE; // offset of the B stages
-    static_assert(BN % (8 * WN) == 0 && BK % 8 == 0, "tile shape");
+    static_assert(BN % (8 * WN) == 0 && BK % MMA_K == 0, "tile shape");
     static_assert(PITCH_KC % 16 == 4 && PITCH_A_OC % 16 == 4 && PITCH_B_OC % 16 == 4, "conflict-free pitches");
 };
 using CfgWide = Cfg<128, 4, 32>;  // 512 threads, 1 CTA / SM
 using CfgDual = Cfg<64, 2, 16>;   // 256 threads, 2 CTAs / SM
-using CfgDualDF = Cfg<64, 2, 16, 1>; // same, one n8-tile of every warp on the fp64 ALU pipe (experiment: DESIGN.md §4.1)
 using CfgStep = Cfg<64, 4, 32>;   // 512 threads, 64-wide right-hand sides (multi-launch TRSM path)
 
 // Per-thread copy plan for one operand: which 16-byte chunks of a (NOUTER x BK) slab this thread moves.  The
 // chunk -> (global offset, shared offset) mapping is the same for every k-slab, so it is computed once; per
 // pipeline stage only a base pointer advances (the per-stage index arithmetic used to sit between the CTA
-// barrier and the first DMMA of every stage).
+// barrier and the first DMMA of every stage).  Chunk q of a thread is chunk 0 moved by q * THREADS / CPR
+// outer rows (KC) or k rows (outer-contiguous), so the plan is one offset pair and one global stride: three
+// registers instead of three per chunk, which the k loop of the 128-register configurations needs.
 template <typename C, bool KC, int NOUTER, int PITCH_OC>
 struct TilePlan {
     static constexpr int CHUNKS = NOUTER * C::BK / 2;
     static constexpr int PER_THREAD = (CHUNKS + C::THREADS - 1) / C::THREADS;
-    int64_t goff[PER_THREAD];
-    int soff[PER_THREAD];
+    static constexpr int CPR = KC ? C::BK / 2 : NOUTER / 2; // chunks per row of the slab
+    static constexpr int ROWS_PER_Q = C::THREADS / CPR;
+    static constexpr int SSTEP = ROWS_PER_Q * (KC ? C::PITCH_KC : PITCH_OC);
+    static_assert(C::THREADS % CPR == 0, "every chunk of a thread sits in the same column of the slab");
+    int64_t goff, gstep;
+    int soff;
     __device__ __forceinline__ void init(int64_t ld)
     {
-#pragma unroll
-        for (int q = 0; q < PER_THREAD; ++q) {
-            const int c = threadIdx.x + q * C::THREADS;
-            if (KC) { // element (o, k) at g[k + o*ld]; smem [o][k]
-                constexpr int CPR = C::BK / 2;
-                const int o = c / CPR, kc = c - o * CPR;
-                goff[q] = (int64_t)o * ld + 2 * kc;
-                soff[q] = o * C::PITCH_KC + 2 * kc;
-            }
-            else { // element (o, k) at g[o + k*ld]; smem [k][o]
-                constexpr int CPR = NOUTER / 2;
-                const int k = c / CPR, oc = c - k * CPR;
-                goff[q] = (int64_t)k * ld + 2 * oc;
-                soff[q] = k * PITCH_OC + 2 * oc;
-            }
-        }
+        const int row = threadIdx.x / CPR, cc = threadIdx.x - row * CPR;
+        // KC: element (o, k) at g[k + o*ld], smem [o][k]; otherwise element (o, k) at g[o + k*ld], smem [k][o]
+        goff = (int64_t)row * ld + 2 * cc;
+        gstep = (int64_t)ROWS_PER_Q * ld;
+        soff = row * (KC ? C::PITCH_KC : PITCH_OC) + 2 * cc;
     }
     __device__ __forceinline__ void issue(double* s, const double* __restrict__ g) const
     {
+        s += soff;
+        g += goff;
 #pragma unroll
         for (int q = 0; q < PER_THREAD; ++q)
-            if (CHUNKS % C::THREADS == 0 || (int)threadIdx.x + q * C::THREADS < CHUNKS) lb_cp_async16(s + soff[q], g + goff[q]);
+            if (CHUNKS % C::THREADS == 0 || (int)threadIdx.x + q * C::THREADS < CHUNKS) lb_cp_async16(s + q * SSTEP, g + q * gstep);
     }
 };
 
@@ -99,63 +97,48 @@ struct Acc {
     }
 };
 
+// One k-step of MMA_K for the warp tile: the A fragments of both m16 tiles, the B fragments of the NT n8 tiles, then
+// 2*NT independent DMMA.16x8xMMA_K.  fa(dm, dk) / fb(dn, dk) read the operand at row / column (base + dm / dn) and
+// k (k0 + t + dk) of this thread, base including g: a[mt][i] is row 16 mt + g + 8 (i&1), k t + 4 (i>>1); b[nt][i] is
+// k t + 4 i, column 8 nt + g.  Those are the words MMA_K/4 steps of k4 fragment loads read, so the padded pitches
+// stay bank-conflict free.
+template <typename C, bool NEG_A, typename FA, typename FB>
+__device__ __forceinline__ void mma_kstep(Acc<C>& acc, FA fa, FB fb)
+{
+    double a[2][MMA_K / 2], b[C::NT][MMA_K / 4];
+#pragma unroll
+    for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int i = 0; i < MMA_K / 2; ++i) {
+            a[mt][i] = fa(mt * 16 + 8 * (i & 1), 4 * (i >> 1));
+            if (NEG_A) a[mt][i] = -a[mt][i];
+        }
+#pragma unroll
+    for (int nt = 0; nt < C::NT; ++nt)
+#pragma unroll
+        for (int i = 0; i < MMA_K / 4; ++i) b[nt][i] = fb(nt * 8, 4 * i);
+#pragma unroll
+    for (int nt = 0; nt < C::NT; ++nt)
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt) lb_dmma_16x8<MMA_K>(acc.v[mt][nt], a[mt], b[nt]);
+}
+
 template <typename C, bool A_KC, bool B_KC, bool NEG_A>
 __device__ __forceinline__ void compute_stage(Acc<C>& acc, const double* sA, const double* sB)
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int wm = warp & 3, wn = warp >> 2;
-    const int m_base = wm * 32, n_base = wn * (C::BN / C::WN);
-    constexpr int NTM = C::NT - C::DF; // n8-tiles on the tensor pipe
-#pragma unroll
-    for (int k0 = 0; k0 < C::BK; k0 += 4) {
-        // one k4 step: 4 A values (rows g, g+8 of both m16 tiles), NTM B values, then 4*NTM independent DMMA.8x8x4
-        double a[2][2], b[NTM > 0 ? NTM : 1];
-#pragma unroll
-        for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                int m = m_base + mt * 16 + g + 8 * i;
-                int k = k0 + t;
-                a[mt][i] = A_KC ? sA[m * C::PITCH_KC + k] : sA[k * C::PITCH_A_OC + m];
-                if (NEG_A) a[mt][i] = -a[mt][i];
-            }
-#pragma unroll
-        for (int nt = 0; nt < NTM; ++nt) {
-            int n = n_base + nt * 8 + g;
-            int k = k0 + t;
-            b[nt] = B_KC ? sB[n * C::PITCH_KC + k] : sB[k * C::PITCH_B_OC + n];
-        }
-#pragma unroll
-        for (int nt = 0; nt < NTM; ++nt)
-#pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {
-                lb_dmma_8x8x4(acc.v[mt][nt][0], acc.v[mt][nt][1], a[mt][0], b[nt]);
-                lb_dmma_8x8x4(acc.v[mt][nt][2], acc.v[mt][nt][3], a[mt][1], b[nt]);
-            }
-        if (C::DF > 0) {
-            // the last n8-tile on the fp64 ALU pipe, same accumulator layout as a DMMA C fragment: rows g, g+8 (per m16 tile),
-            // columns 2t, 2t+1; every lane needs all four k of the step (the 4 lanes of a row / the 8 lanes of a column pair
-            // read the same words: broadcast)
-            constexpr int nt = C::NT - 1;
-            const int n = n_base + nt * 8 + 2 * t;
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const int k = k0 + kk;
-                const double bx = B_KC ? sB[n * C::PITCH_KC + k] : sB[k * C::PITCH_B_OC + n];
-                const double by = B_KC ? sB[(n + 1) * C::PITCH_KC + k] : sB[k * C::PITCH_B_OC + n + 1];
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int m = m_base + mt * 16 + g + 8 * i;
-                        double av = A_KC ? sA[m * C::PITCH_KC + k] : sA[k * C::PITCH_A_OC + m];
-                        if (NEG_A) av = -av;
-                        acc.v[mt][nt][2 * i] = fma(av, bx, acc.v[mt][nt][2 * i]);
-                        acc.v[mt][nt][2 * i + 1] = fma(av, by, acc.v[mt][nt][2 * i + 1]);
-                    }
-            }
-        }
+    const int m_base = wm * 32 + g, n_base = wn * (C::BN / C::WN) + g;
+    // two k-steps per trip: fully unrolled, ptxas hoists the fragment loads of the whole stage and the 128-register
+    // configurations spill inside the k loop (the m16n8k4 operands sit in aligned register pairs / quads)
+#pragma unroll 2
+    for (int k0 = 0; k0 < C::BK; k0 += MMA_K) {
+        const int k = k0 + t;
+        mma_kstep<C, NEG_A>(
+            acc,
+            [&](int dm, int dk) { return A_KC ? sA[(m_base + dm) * C::PITCH_KC + k + dk] : sA[(k + dk) * C::PITCH_A_OC + m_base + dm]; },
+            [&](int dn, int dk) { return B_KC ? sB[(n_base + dn) * C::PITCH_KC + k + dk] : sB[(k + dk) * C::PITCH_B_OC + n_base + dn]; });
     }
 }
 
@@ -247,7 +230,7 @@ __device__ __forceinline__ void mainloop_resB(Acc<C>& acc, const double* __restr
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int g = lane >> 2, t = lane & 3;
     const int wm = warp & 3, wn = warp >> 2;
-    const int m_base = wm * 32, n_base = wn * (C::BN / C::WN);
+    const int m_base = wm * 32 + g, n_base = wn * (C::BN / C::WN) + g;
     TilePlan<C, false, BM, C::PITCH_A_OC> pa;
     pa.init(lda);
 #pragma unroll
@@ -263,21 +246,11 @@ __device__ __forceinline__ void mainloop_resB(Acc<C>& acc, const double* __restr
         lb_cp_async_commit();
         const double* sA = smem_pipe + (kt % STAGES) * C::A_STAGE;
 #pragma unroll
-        for (int k0 = 0; k0 < C::BK; k0 += 4) {
-            double a[2][2], b[C::NT];
-#pragma unroll
-            for (int mt = 0; mt < 2; ++mt)
-#pragma unroll
-                for (int i = 0; i < 2; ++i) a[mt][i] = sA[(k0 + t) * C::PITCH_A_OC + m_base + mt * 16 + g + 8 * i];
-#pragma unroll
-            for (int nt = 0; nt < C::NT; ++nt) b[nt] = sBres[(n_base + nt * 8 + g) * PB + kt * C::BK + k0 + t];
-#pragma unroll
-            for (int nt = 0; nt < C::NT; ++nt)
-#pragma unroll
-                for (int mt = 0; mt < 2; ++mt) {
-                    lb_dmma_8x8x4(acc.v[mt][nt][0], acc.v[mt][nt][1], a[mt][0], b[nt]);
-                    lb_dmma_8x8x4(acc.v[mt][nt][2], acc.v[mt][nt][3], a[mt][1], b[nt]);
-                }
+        for (int k0 = 0; k0 < C::BK; k0 += MMA_K) {
+            const int k = k0 + t;
+            mma_kstep<C, false>(
+                acc, [&](int dm, int dk) { return sA[(k + dk) * C::PITCH_A_OC + m_base + dm]; },
+                [&](int dn, int dk) { return sBres[(n_base + dn) * PB + kt * C::BK + k + dk]; });
         }
     }
     lb_cp_async_wait<0>();

@@ -23,15 +23,20 @@ constexpr size_t POTF2_SMEM = (size_t)(LB_TILE * PS + 10 * XB + LB_TILE) * sizeo
 
 __device__ __forceinline__ int blk(int ib, int jb) { return ib * (ib + 1) / 2 + jb; }
 
-// One warp: c(16x8) += sum_k A(m,k) B(k,n), K a multiple of 8; fa(m,k), fb(k,n) read shared memory.
+// One warp: c(16x8) += sum_k A(m,k) B(k,n), K a multiple of lbg::MMA_K; fa(m,k), fb(k,n) read shared memory.
+// The same DMMA shape as the tile GEMM core (gemm.cuh).
 template <typename FA, typename FB>
 __device__ __forceinline__ void warp_mma(double (&c)[4], int K, FA fa, FB fb)
 {
+    constexpr int KS = lbg::MMA_K;
     const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-    for (int k0 = 0; k0 < K; k0 += 4) {
-        const double a0 = fa(g, k0 + t), a1 = fa(g + 8, k0 + t), b = fb(k0 + t, g);
-        lb_dmma_8x8x4(c[0], c[1], a0, b);
-        lb_dmma_8x8x4(c[2], c[3], a1, b);
+    for (int k0 = 0; k0 < K; k0 += KS) {
+        double a[KS / 2], b[KS / 4];
+#pragma unroll
+        for (int i = 0; i < KS / 2; ++i) a[i] = fa(g + 8 * (i & 1), k0 + t + 4 * (i >> 1));
+#pragma unroll
+        for (int i = 0; i < KS / 4; ++i) b[i] = fb(k0 + t + 4 * i, g);
+        lb_dmma_16x8<KS>(c, a, b);
     }
 }
 
@@ -271,21 +276,6 @@ syrk_kernel(double* __restrict__ L, int64_t ld, int kb, int kd, int j0, int nc, 
 }
 
 using SyrkCfg = lbg::CfgDual;
-using SyrkCfgDF = lbg::CfgDualDF; // same tile, one n8-tile per warp on the fp64 ALU pipe (LB_SYRK_DF=1)
-static_assert(SyrkCfg::PIPE_BYTES == SyrkCfgDF::PIPE_BYTES && SyrkCfg::THREADS == SyrkCfgDF::THREADS, "same launch shape");
-
-inline bool syrk_df()
-{
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("LB_SYRK_DF"); v = (e && atoi(e) != 0) ? 1 : 0; }
-    return v != 0;
-}
-// trailing-update launch with the configuration chosen at run time
-#define LB_SYRK_LAUNCH(grid, stream, ...)                                                                              \
-    do {                                                                                                               \
-        if (syrk_df()) syrk_kernel<SyrkCfgDF><<<(grid), SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, (stream)>>>(__VA_ARGS__); \
-        else syrk_kernel<SyrkCfg><<<(grid), SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, (stream)>>>(__VA_ARGS__);            \
-    } while (0)
 constexpr int SYRK_SPLIT = LB_TILE / SyrkCfg::BN;
 
 LbOncePerDevice g_attr_once;
@@ -295,7 +285,6 @@ int set_attrs()
     LB_CUDA(cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)POTF2_SMEM));
     LB_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lbg::CfgWide::PIPE_BYTES));
     LB_CUDA(cudaFuncSetAttribute(syrk_kernel<SyrkCfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SyrkCfg::PIPE_BYTES));
-    LB_CUDA(cudaFuncSetAttribute(syrk_kernel<SyrkCfgDF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SyrkCfg::PIPE_BYTES));
     LB_CUDA(cudaFuncSetAttribute(syrk_kernel<lbg::CfgWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lbg::CfgWide::PIPE_BYTES));
     return LB_OK;
 }
@@ -361,7 +350,7 @@ static int launch_pair_panel(lb_gp* h, cudaStream_t side, int k, int T, int64_t 
         }
         {
             LbProfScope ps(h, side, LB_PC_SYRK_COL);
-            LB_SYRK_LAUNCH((T - k - 1) * SYRK_SPLIT, side, h->dL, ld, k, 1, k + 1, 1, T);
+            syrk_kernel<SyrkCfg><<<(T - k - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 1, k + 1, 1, T);
         }
         {
             LbProfScope ps(h, side, LB_PC_POTF2);
@@ -396,7 +385,7 @@ static int launch_potrf_quads(lb_gp* h)
             const int nc2 = (T - (k + 2) < 2) ? (T - (k + 2)) : 2;
             {
                 LbProfScope ps(h, side, LB_PC_SYRK_COL);
-                LB_SYRK_LAUNCH(syrk_tiles(T, k + 2, nc2) * SYRK_SPLIT, side, h->dL, ld, k, 2, k + 2, nc2, T);
+                syrk_kernel<SyrkCfg><<<syrk_tiles(T, k + 2, nc2) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 2, k + 2, nc2, T);
             }
             h->launches++;
             if ((rc = launch_pair_panel(h, side, k + 2, T, ld))) return rc;
@@ -413,7 +402,7 @@ static int launch_potrf_quads(lb_gp* h)
         if (wide < 0) { const char* e = getenv("LB_SYRK_WIDE"); wide = (e && atoi(e) != 0) ? 1 : 0; }
         {
             LbProfScope ps(h, main, LB_PC_SYRK);
-            LB_SYRK_LAUNCH(syrk_tiles(T, j0, nca) * SYRK_SPLIT, main, h->dL, ld, k, 4, j0, nca, T);
+            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nca) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0, nca, T);
         }
         h->launches++;
         if (side != main) {
@@ -428,7 +417,7 @@ static int launch_potrf_quads(lb_gp* h)
                 syrk_kernel<lbg::CfgWide><<<syrk_tiles(T, j0 + nca, ncb), lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca,
                     ncb, T);
             else
-                LB_SYRK_LAUNCH(syrk_tiles(T, j0 + nca, ncb) * SYRK_SPLIT, main, h->dL, ld, k, 4, j0 + nca, ncb, T);
+                syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0 + nca, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca, ncb, T);
             h->launches++;
         }
     }
@@ -490,7 +479,7 @@ int lb_launch_potrf(lb_gp* h)
             }
             {
                 LbProfScope ps(h, side, LB_PC_SYRK_COL);
-                LB_SYRK_LAUNCH((T - k - 1) * SYRK_SPLIT, side, h->dL, ld, k, 1, k + 1, 1, T);
+                syrk_kernel<SyrkCfg><<<(T - k - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 1, k + 1, 1, T);
             }
             {
                 LbProfScope ps(h, side, LB_PC_POTF2);
@@ -517,7 +506,7 @@ int lb_launch_potrf(lb_gp* h)
         if (sa != main && side != main) LB_CUDA(cudaStreamWaitEvent(sa, h->ev[1 + (p & 1)], 0));
         {
             LbProfScope ps(h, sa, LB_PC_SYRK);
-            LB_SYRK_LAUNCH(syrk_tiles(T, j0, nca) * SYRK_SPLIT, sa, h->dL, ld, k, 2, j0, nca, T);
+            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nca) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, sa>>>(h->dL, ld, k, 2, j0, nca, T);
         }
         h->launches++;
         if (side != main) {
@@ -530,13 +519,13 @@ int lb_launch_potrf(lb_gp* h)
             const int left_end = cstar < jb ? jb : cstar; // columns [jb, left_end) on main, [left_end, T) on the second stream
             if (left_end > jb) {
                 LbProfScope ps(h, main, LB_PC_SYRK);
-                LB_SYRK_LAUNCH(syrk_tiles(T, jb, left_end - jb) * SYRK_SPLIT, main, h->dL, ld, k, 2, jb, left_end - jb, T);
+                syrk_kernel<SyrkCfg><<<syrk_tiles(T, jb, left_end - jb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 2, jb, left_end - jb, T);
                 h->launches++;
             }
             if (T - left_end > 0) {
                 if (side != main) LB_CUDA(cudaStreamWaitEvent(second, h->ev[1 + (p & 1)], 0)); // the panel it multiplies with
                 LbProfScope ps(h, second, LB_PC_SYRK);
-                LB_SYRK_LAUNCH(syrk_tiles(T, left_end, T - left_end) * SYRK_SPLIT, second, h->dL, ld, k, 2, left_end, T - left_end, T);
+                syrk_kernel<SyrkCfg><<<syrk_tiles(T, left_end, T - left_end) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, second>>>(h->dL, ld, k, 2, left_end, T - left_end, T);
                 h->launches++;
             }
         }
@@ -544,7 +533,7 @@ int lb_launch_potrf(lb_gp* h)
             const int ncb = T - jb;
             if (ncb > 0) {
                 LbProfScope ps(h, sa, LB_PC_SYRK);
-                LB_SYRK_LAUNCH(syrk_tiles(T, jb, ncb) * SYRK_SPLIT, sa, h->dL, ld, k, 2, jb, ncb, T);
+                syrk_kernel<SyrkCfg><<<syrk_tiles(T, jb, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, sa>>>(h->dL, ld, k, 2, jb, ncb, T);
                 h->launches++;
             }
         }
@@ -700,7 +689,7 @@ int lb_dchol_panel(lb_gp* h, double* dCols, int64_t Nd, int kpair, double* dInvD
     double* Ib = dInvD - (int64_t)kpair * LB_TILE * LB_TILE;
     potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(Lb, Nd, kpair, Ib, dInfo, 1);
     trsm_panel_kernel<<<T - kpair - 1, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, st>>>(Lb, Nd, kpair, Ib);
-    LB_SYRK_LAUNCH((T - kpair - 1) * SYRK_SPLIT, st, Lb, Nd, kpair, 1, kpair + 1, 1, T);
+    syrk_kernel<SyrkCfg><<<(T - kpair - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, st>>>(Lb, Nd, kpair, 1, kpair + 1, 1, T);
     potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(Lb, Nd, kpair + 1, Ib, dInfo, 1);
     h->launches += 4;
     if (kpair + 2 < T) {
