@@ -1,13 +1,14 @@
 // limbo_b200/csrc/gemm.cuh — fp64 tensor-core (DMMA) tile GEMM building block.
 //
 // A CTA accumulates a 128 x BN tile  acc (+/-)= A(128 x K) * B(K x BN)  with a 3-stage cp.async
-// pipeline.  Configurations (Cfg<BN, WN, BK>):
-//   * warps: 4 along M x WN along N  (THREADS = 128 * WN); warp tile 32 x (BN / WN);
-//     both configurations keep >= 2 DMMA-issuing warps per SM sub-partition, so that the dependent
-//     DMMAs of one warp do not leave the pipe idle:
-//       Cfg<128, 4, 32>: 512 threads, one CTA per SM, 4 warps per sub-partition;
-//       Cfg< 64, 2, 16>: 256 threads, TWO CTAs per SM (77 KB smem, <= 128 regs): while one CTA
-//                        is in its C-tile prologue / store epilogue the other one computes.
+// pipeline.  Configurations (Cfg<BN, WN, BK, WM, CTAS>):
+//   * warps: WM along M x WN along N  (THREADS = 32 * WM * WN); warp tile (128 / WM) x (BN / WN), i.e.
+//     MT = 8 / WM m16 tiles by NT n8 tiles, MT * NT independent DMMA chains per warp; CTAS CTAs per SM:
+//       Cfg<128, 4, 32, 4, 1>: 512 threads, one CTA per SM, 4 warps per sub-partition, 32 x 32 warp tiles;
+//       Cfg< 64, 2, 16, 2, 2>: 128 threads, TWO CTAs per SM (90 KB smem, <= 255 regs), 64 x 32 warp tiles:
+//                              2 warps per sub-partition with 16 chains each (the m16n8k4 rate of 8 warps
+//                              per SM, DESIGN.md §4.1), and while one CTA is in its C-tile prologue / store
+//                              epilogue the other one computes.
 //   * operands "outer-contiguous" (the m / n index is the unit-stride one, i.e. a column-major
 //     block) or "K-contiguous"; shared tiles are padded by 4 doubles so every 64-bit fragment
 //     load is bank-conflict free (DESIGN.md §4.1).
@@ -29,11 +30,14 @@ constexpr int STAGES = 3;
 // the pair / quad / distributed factorisations rests on that).
 constexpr int MMA_K = 4;
 
-template <int BN_, int WN_, int BK_>
+template <int BN_, int WN_, int BK_, int WM_ = 4, int CTAS_ = 1>
 struct Cfg {
-    static constexpr int BN = BN_, WN = WN_, BK = BK_;
-    static constexpr int THREADS = 128 * WN;
+    static constexpr int BN = BN_, WN = WN_, BK = BK_, WM = WM_;
+    static constexpr int CTAS_PER_SM = CTAS_;     // __launch_bounds__ minimum blocks per SM
+    static constexpr int THREADS = 32 * WM * WN;
+    static constexpr int MT = BM / (16 * WM);     // m16 tiles per warp
     static constexpr int NT = BN / (8 * WN);      // n8 tiles per warp
+    static constexpr int WTM = 16 * MT, WTN = 8 * NT; // warp tile
     static constexpr int PITCH_A_OC = BM + 4;     // [BK][128+4]
     static constexpr int PITCH_B_OC = BN + 4;     // [BK][BN+4]
     static constexpr int PITCH_KC = BK + 4;       // [outer][BK+4]
@@ -41,12 +45,12 @@ struct Cfg {
     static constexpr int B_STAGE = (BN * PITCH_KC > BK * PITCH_B_OC) ? BN * PITCH_KC : BK * PITCH_B_OC;
     static constexpr size_t PIPE_BYTES = (size_t)STAGES * (A_STAGE + B_STAGE) * sizeof(double);
     static constexpr int A_PIPE_DOUBLES = STAGES * A_STAGE; // offset of the B stages
-    static_assert(BN % (8 * WN) == 0 && BK % MMA_K == 0, "tile shape");
+    static_assert(BN % (8 * WN) == 0 && BM % (32 * WM) == 0 && (WM & (WM - 1)) == 0 && BK % MMA_K == 0, "tile shape");
     static_assert(PITCH_KC % 16 == 4 && PITCH_A_OC % 16 == 4 && PITCH_B_OC % 16 == 4, "conflict-free pitches");
 };
-using CfgWide = Cfg<128, 4, 32>;  // 512 threads, 1 CTA / SM
-using CfgDual = Cfg<64, 2, 16>;   // 256 threads, 2 CTAs / SM
-using CfgStep = Cfg<64, 4, 32>;   // 512 threads, 64-wide right-hand sides (multi-launch TRSM path)
+using CfgWide = Cfg<128, 4, 32>;       // 512 threads, 1 CTA / SM, 32 x 32 warp tiles
+using CfgDual = Cfg<64, 2, 16, 2, 2>;  // 128 threads, 2 CTAs / SM, 64 x 32 warp tiles
+using CfgStep = Cfg<64, 4, 32>;        // 512 threads, 64-wide right-hand sides (multi-launch TRSM path)
 
 // Per-thread copy plan for one operand: which 16-byte chunks of a (NOUTER x BK) slab this thread moves.  The
 // chunk -> (global offset, shared offset) mapping is the same for every k-slab, so it is computed once; per
@@ -82,14 +86,14 @@ struct TilePlan {
     }
 };
 
-// Accumulators of one warp: 2 m16-tiles x NT n8-tiles.
+// Accumulators of one warp: MT m16-tiles x NT n8-tiles.
 template <typename C>
 struct Acc {
-    double v[2][C::NT][4];
+    double v[C::MT][C::NT][4];
     __device__ __forceinline__ void zero()
     {
 #pragma unroll
-        for (int a = 0; a < 2; ++a)
+        for (int a = 0; a < C::MT; ++a)
 #pragma unroll
             for (int b = 0; b < C::NT; ++b)
 #pragma unroll
@@ -97,17 +101,23 @@ struct Acc {
     }
 };
 
-// One k-step of MMA_K for the warp tile: the A fragments of both m16 tiles, the B fragments of the NT n8 tiles, then
-// 2*NT independent DMMA.16x8xMMA_K.  fa(dm, dk) / fb(dn, dk) read the operand at row / column (base + dm / dn) and
+// Origin of this warp's tile in the CTA tile; warps are numbered M-fastest.
+template <typename C>
+__device__ __forceinline__ int warp_row0() { return ((int)(threadIdx.x >> 5) & (C::WM - 1)) * C::WTM; }
+template <typename C>
+__device__ __forceinline__ int warp_col0() { return ((int)(threadIdx.x >> 5) / C::WM) * C::WTN; }
+
+// One k-step of MMA_K for the warp tile: the A fragments of the MT m16 tiles, the B fragments of the NT n8 tiles, then
+// MT*NT independent DMMA.16x8xMMA_K.  fa(dm, dk) / fb(dn, dk) read the operand at row / column (base + dm / dn) and
 // k (k0 + t + dk) of this thread, base including g: a[mt][i] is row 16 mt + g + 8 (i&1), k t + 4 (i>>1); b[nt][i] is
 // k t + 4 i, column 8 nt + g.  Those are the words MMA_K/4 steps of k4 fragment loads read, so the padded pitches
 // stay bank-conflict free.
 template <typename C, bool NEG_A, typename FA, typename FB>
 __device__ __forceinline__ void mma_kstep(Acc<C>& acc, FA fa, FB fb)
 {
-    double a[2][MMA_K / 2], b[C::NT][MMA_K / 4];
+    double a[C::MT][MMA_K / 2], b[C::NT][MMA_K / 4];
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+    for (int mt = 0; mt < C::MT; ++mt)
 #pragma unroll
         for (int i = 0; i < MMA_K / 2; ++i) {
             a[mt][i] = fa(mt * 16 + 8 * (i & 1), 4 * (i >> 1));
@@ -120,18 +130,18 @@ __device__ __forceinline__ void mma_kstep(Acc<C>& acc, FA fa, FB fb)
 #pragma unroll
     for (int nt = 0; nt < C::NT; ++nt)
 #pragma unroll
-        for (int mt = 0; mt < 2; ++mt) lb_dmma_16x8<MMA_K>(acc.v[mt][nt], a[mt], b[nt]);
+        for (int mt = 0; mt < C::MT; ++mt) lb_dmma_16x8<MMA_K>(acc.v[mt][nt], a[mt], b[nt]);
 }
 
 template <typename C, bool A_KC, bool B_KC, bool NEG_A>
 __device__ __forceinline__ void compute_stage(Acc<C>& acc, const double* sA, const double* sB)
 {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int wm = warp & 3, wn = warp >> 2;
-    const int m_base = wm * 32 + g, n_base = wn * (C::BN / C::WN) + g;
+    const int m_base = warp_row0<C>() + g, n_base = warp_col0<C>() + g;
     // two k-steps per trip: fully unrolled, ptxas hoists the fragment loads of the whole stage and the 128-register
-    // configurations spill inside the k loop (the m16n8k4 operands sit in aligned register pairs / quads)
+    // configurations spill inside the k loop (the m16n8k4 operands sit in aligned register pairs / quads); CfgDual
+    // (255 registers) fits either way, and measured faster by two (DESIGN.md §4.1)
 #pragma unroll 2
     for (int k0 = 0; k0 < C::BK; k0 += MMA_K) {
         const int k = k0 + t;
@@ -190,17 +200,17 @@ __device__ __forceinline__ void mainloop(Acc<C>& acc, const double* __restrict__
 template <typename C, typename F>
 __device__ __forceinline__ void for_each_acc(Acc<C>& acc, F&& f)
 {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int wm = warp & 3, wn = warp >> 2;
+    const int row0 = warp_row0<C>(), col0 = warp_col0<C>();
 #pragma unroll
-    for (int mt = 0; mt < 2; ++mt)
+    for (int mt = 0; mt < C::MT; ++mt)
 #pragma unroll
         for (int nt = 0; nt < C::NT; ++nt)
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-                int row = wm * 32 + mt * 16 + g + 8 * (i >> 1);
-                int col = wn * (C::BN / C::WN) + nt * 8 + 2 * t + (i & 1);
+                int row = row0 + mt * 16 + g + 8 * (i >> 1);
+                int col = col0 + nt * 8 + 2 * t + (i & 1);
                 f(row, col, acc.v[mt][nt][i]);
             }
 }
@@ -227,10 +237,9 @@ __device__ __forceinline__ void mainloop_resB(Acc<C>& acc, const double* __restr
 {
     constexpr int PB = BM + 4;
     constexpr int nk = BM / C::BK;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int wm = warp & 3, wn = warp >> 2;
-    const int m_base = wm * 32 + g, n_base = wn * (C::BN / C::WN) + g;
+    const int m_base = warp_row0<C>() + g, n_base = warp_col0<C>() + g;
     TilePlan<C, false, BM, C::PITCH_A_OC> pa;
     pa.init(lda);
 #pragma unroll

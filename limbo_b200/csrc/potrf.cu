@@ -254,10 +254,10 @@ trsm_panel_kernel(double* __restrict__ L, int64_t ld, int k, const double* __res
 // (kd = 1: one 128-column panel, K = 128; kd = 2: two panels at once, K = 256 —
 // half the C traffic and half the tile prologues per flop).  C is preloaded into
 // the accumulators so its latency overlaps the operand pipeline's prologue.
-// Cfg = CfgDual: 128 x 64 tiles, 256 threads, two CTAs per SM (one CTA's C-tile prologue / store epilogue
+// Cfg = CfgDual: 128 x 64 tiles, 128 threads, two CTAs per SM (one CTA's C-tile prologue / store epilogue
 // hides under the other's DMMA stream).
 template <typename C>
-__global__ void __launch_bounds__(C::THREADS, (C::THREADS == 256) ? 2 : 1)
+__global__ void __launch_bounds__(C::THREADS, C::CTAS_PER_SM)
 syrk_kernel(double* __restrict__ L, int64_t ld, int kb, int kd, int j0, int nc, int T)
 {
     extern __shared__ __align__(16) double smem[];
@@ -285,7 +285,6 @@ int set_attrs()
     LB_CUDA(cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)POTF2_SMEM));
     LB_CUDA(cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lbg::CfgWide::PIPE_BYTES));
     LB_CUDA(cudaFuncSetAttribute(syrk_kernel<SyrkCfg>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SyrkCfg::PIPE_BYTES));
-    LB_CUDA(cudaFuncSetAttribute(syrk_kernel<lbg::CfgWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lbg::CfgWide::PIPE_BYTES));
     return LB_OK;
 }
 
@@ -398,8 +397,6 @@ static int launch_potrf_quads(lb_gp* h)
         // ---- a(q): the next quad's block columns, K = 512 ----
         const int j0 = k + 4;
         const int nca = (T - j0 < 4) ? (T - j0) : 4;
-        static int wide = -1; // experiment: 128 x 128 tiles, 512 threads, one CTA per SM for the K = 512 main-stream updates
-        if (wide < 0) { const char* e = getenv("LB_SYRK_WIDE"); wide = (e && atoi(e) != 0) ? 1 : 0; }
         {
             LbProfScope ps(h, main, LB_PC_SYRK);
             syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nca) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0, nca, T);
@@ -413,11 +410,7 @@ static int launch_potrf_quads(lb_gp* h)
         const int ncb = T - j0 - nca;
         if (ncb > 0) {
             LbProfScope ps(h, main, LB_PC_SYRK);
-            if (wide)
-                syrk_kernel<lbg::CfgWide><<<syrk_tiles(T, j0 + nca, ncb), lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca,
-                    ncb, T);
-            else
-                syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0 + nca, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca, ncb, T);
+            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0 + nca, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca, ncb, T);
             h->launches++;
         }
     }
@@ -599,7 +592,7 @@ dchol_pack_kernel(const double* __restrict__ cols, int64_t ld, int64_t row0, dou
 // C[i, j(l)] -= P[i,:] P[j(l),:]^T for the local block columns l in [l0, l1) whose global index j(l) > kpair+1, i >= j(l).
 // P is the packed panel: row block b of the global matrix sits at panel row (b - (kpair + 2)) * 128, ld = ldp, K = 256.
 template <typename C>
-__global__ void __launch_bounds__(C::THREADS, (C::THREADS == 256) ? 2 : 1)
+__global__ void __launch_bounds__(C::THREADS, C::CTAS_PER_SM)
 dchol_update_kernel(double* __restrict__ Lloc, int64_t ld, const double* __restrict__ P, int64_t ldp, int kpair, int l0, int l1, int rank,
     int G, int T)
 {

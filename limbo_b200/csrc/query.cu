@@ -739,7 +739,7 @@ constexpr int SB = 16;
 // factor spread over inv_G GPUs by 128-column tiles, lb_launch_linv_columns).  Column tile c is zero above row tile c: super-blocks
 // above it are skipped and the K range starts at the super-block that holds it.
 template <typename C, bool INV>
-__global__ void __launch_bounds__(C::THREADS, (C::THREADS == 256) ? 2 : 1)
+__global__ void __launch_bounds__(C::THREADS, C::CTAS_PER_SM)
 panel_update_kernel(const double* __restrict__ L, int64_t ld, const double* __restrict__ V, double* __restrict__ Tbuf, int64_t ldt, int s0,
     int nrows, int ct0, int inv_rank, int inv_G)
 {
@@ -762,7 +762,7 @@ panel_update_kernel(const double* __restrict__ L, int64_t ld, const double* __re
 
 // V[s0 + i, ct] = sum_{k <= i} Linv[s0 + i, s0 + k] Tbuf[k, ct];  normpart[(s0 + i) * Mp + c] = sum over the tile's 128 rows of V^2
 template <typename C, bool INV>
-__global__ void __launch_bounds__(C::THREADS, (C::THREADS == 256) ? 2 : 1)
+__global__ void __launch_bounds__(C::THREADS, C::CTAS_PER_SM)
 panel_solve_kernel(const double* __restrict__ Linv, int64_t ld, const double* __restrict__ Tbuf, int64_t ldt, double* __restrict__ V, int s0,
     int nrows, double* __restrict__ normpart, int64_t Mp, int ct0, int inv_rank, int inv_G)
 {
@@ -779,27 +779,36 @@ panel_solve_kernel(const double* __restrict__ Linv, int64_t ld, const double* __
     acc.zero();
     lbg::mainloop<C, false, true>(acc, Linv + (int64_t)(s0 + i) * LB_TILE + (int64_t)(s0 + k0) * LB_TILE * ld, ld,
         Tbuf + (int64_t)k0 * LB_TILE + (int64_t)ct * C::BN * ldt, ldt, (i + 1 - k0) * LB_TILE, smem);
-    lbg::store_acc<C>(acc, V + (int64_t)(s0 + i) * LB_TILE + (int64_t)ct * C::BN * ld, ld);
-    if (INV) return;
-    // column norms of the tile: per thread (2 m16 tiles x 2 row halves), then the 8 row lanes, then the 4 row warps
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (INV) {
+        lbg::store_acc<C>(acc, V + (int64_t)(s0 + i) * LB_TILE + (int64_t)ct * C::BN * ld, ld);
+        return;
+    }
+    // column norms of the tile, per 32-row slice: per thread (2 m16 tiles x 2 row halves), then the 8 row lanes, then the
+    // 4 slices in a fixed order.  A warp tile spans SL slices; each one is reduced on its own, so the sums (and sigma^2) do
+    // not depend on the warp layout.  The tile is stored after the norms: the other order spills 8 bytes at 255 registers.
+    constexpr int SL = C::MT / 2;
+    static_assert(C::MT % 2 == 0 && C::THREADS >= C::BN, "norm epilogue: whole 32-row slices per warp, a thread per column");
+    const int lane = threadIdx.x & 31;
     const int g = lane >> 2, t = lane & 3;
-    const int wm = warp & 3, wn = warp >> 2;
+    const int slice0 = lbg::warp_row0<C>() / 32, col0 = lbg::warp_col0<C>();
     double* sRed = smem; // [4][BN]
 #pragma unroll
-    for (int nt = 0; nt < C::NT; ++nt)
+    for (int sl = 0; sl < SL; ++sl)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            double sq = 0.0;
+        for (int nt = 0; nt < C::NT; ++nt)
 #pragma unroll
-            for (int mt = 0; mt < 2; ++mt) {
-                sq = fma(acc.v[mt][nt][e], acc.v[mt][nt][e], sq);
-                sq = fma(acc.v[mt][nt][2 + e], acc.v[mt][nt][2 + e], sq);
+            for (int e = 0; e < 2; ++e) {
+                double sq = 0.0;
+#pragma unroll
+                for (int mt = 2 * sl; mt < 2 * sl + 2; ++mt) {
+                    sq = fma(acc.v[mt][nt][e], acc.v[mt][nt][e], sq);
+                    sq = fma(acc.v[mt][nt][2 + e], acc.v[mt][nt][2 + e], sq);
+                }
+#pragma unroll
+                for (int o = 4; o < 32; o <<= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+                if (g == 0) sRed[(slice0 + sl) * C::BN + col0 + nt * 8 + 2 * t + e] = sq;
             }
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-            if (g == 0) sRed[wm * C::BN + wn * (C::BN / C::WN) + nt * 8 + 2 * t + e] = sq;
-        }
+    lbg::store_acc<C>(acc, V + (int64_t)(s0 + i) * LB_TILE + (int64_t)ct * C::BN * ld, ld);
     __syncthreads();
     if ((int)threadIdx.x < C::BN) {
         const double sum = ((sRed[threadIdx.x] + sRed[C::BN + threadIdx.x]) + sRed[2 * C::BN + threadIdx.x]) + sRed[3 * C::BN + threadIdx.x];
@@ -835,11 +844,8 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
     long long* launches)
 {
     using namespace panel;
-    using CW = lbg::CfgWide;
     using CD = lbg::CfgDual;
     if (g_once.need()) {
-        LB_CUDA(cudaFuncSetAttribute(panel_update_kernel<CW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::PIPE_BYTES));
-        LB_CUDA(cudaFuncSetAttribute(panel_solve_kernel<CW, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CW::PIPE_BYTES));
         LB_CUDA(cudaFuncSetAttribute(panel_update_kernel<CD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CD::PIPE_BYTES));
         LB_CUDA(cudaFuncSetAttribute(panel_solve_kernel<CD, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CD::PIPE_BYTES));
     }
@@ -871,14 +877,7 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
         const char* e2 = getenv("LB_PANEL_SIDE");   // 1: second group on the high-priority side stream instead of a normal-priority one
         use_side = (e2 && atoi(e2) != 0) ? 1 : 0;
     }
-    // LB_PANEL_CFG=1: 128 x 128 tiles (CfgWide); default 128 x 64 tiles, two CTAs per SM (same bits: the tile shape does not
-    // change any element's accumulation order).  H100 SXM, 400 W power limit, N = 16384, ms per batch (Dual / Wide): M = 1250:
-    // 16.6 / 19.0, 2500: 28.9 / 30.3, 10^4: 123.7 / 116.4 - inside the process-to-process spread for large batches, so the
-    // default stays the one that is better for small ones.
-    static int cfg_mode = -1;
-    if (cfg_mode < 0) { const char* e = getenv("LB_PANEL_CFG"); cfg_mode = e ? atoi(e) : 0; }
-    const bool dual = cfg_mode != 1;
-    const int wmul = dual ? 2 : 1; // 64-wide column tiles per 128 candidates
+    constexpr int wmul = LB_TILE / CD::BN; // 64-wide column tiles per 128 candidates
     // Groups of column tiles, each walking the chain on its own stream.  A launch of all column tiles under one round of the machine
     // (M = 640 at N = 16384: 160 CTAs for 264 slots): four equal groups, so that the groups, drifting apart, keep the SMs full.
     // Otherwise one stream, unless LB_PANEL_SPLIT=<1..99> asks for two groups (that percentage / the rest).  LB_PANEL_GROUPS=<1..4>
@@ -890,7 +889,7 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
     if (force_groups < 0) { const char* e = getenv("LB_PANEL_GROUPS"); force_groups = e ? atoi(e) : 0; }
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
-    const int slots = sms * (dual ? 2 : 1);
+    const int slots = sms * CD::CTAS_PER_SM;
     int ngroups = 1;
     if (ctiles >= 4 && (int64_t)ctiles * wmul * SB < (int64_t)slots) ngroups = 4;
     else if (split_pct < 100 && ctiles >= 4) ngroups = 2;
@@ -929,14 +928,8 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
             for (int g = 0; g < ngroups; ++g) {
                 const int c0 = gbeg[g] * wmul, nc = (gbeg[g + 1] - gbeg[g]) * wmul;
                 if (nc <= 0) continue;
-                if (dual) {
-                    panel_update_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dL, ld, dV, dT, ldt, s0, nrows, c0, 0, 1);
-                    panel_solve_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dLinv, ld, dT, ldt, dV, s0, nrows, dNorm, Mp, c0, 0, 1);
-                }
-                else {
-                    panel_update_kernel<CW, false><<<nrows * nc, CW::THREADS, CW::PIPE_BYTES, sts[g]>>>(h->dL, ld, dV, dT, ldt, s0, nrows, c0, 0, 1);
-                    panel_solve_kernel<CW, false><<<nrows * nc, CW::THREADS, CW::PIPE_BYTES, sts[g]>>>(h->dLinv, ld, dT, ldt, dV, s0, nrows, dNorm, Mp, c0, 0, 1);
-                }
+                panel_update_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dL, ld, dV, dT, ldt, s0, nrows, c0, 0, 1);
+                panel_solve_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dLinv, ld, dT, ldt, dV, s0, nrows, dNorm, Mp, c0, 0, 1);
                 if (launches) *launches += 2;
             }
         }
