@@ -129,6 +129,20 @@ int lb_acq_argmax(const lb_gp* h, int acq_id, const double* acq_params, int64_t 
 int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* dXq_rowmajor,
     const double* dMean_at_q, double mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
 
+/* experimental/acqui/eci.hpp:76-107 over an objective and a constraint model, FirstElem aggregator:
+ *   ECI = Pf * EI,  EI as LB_ACQ_EI on obj,  Pf = Phi((mu_c[0] - 1) / sigma_c) on con (eci.hpp:116-130).
+ * eci_params = {f_max, jitter}; con may be NULL (no constraints: Pf = 1), as may a con without samples.  An obj without samples
+ * scores 0 everywhere (index 0).  obj and con must be distinct handles on the same device with the same input dimension; both
+ * are locked for the call, and their queries run on their own streams.  The means are added as in lb_acq_argmax (an array of
+ * M first components, or NULL and a constant).  Ties resolve to the lowest index. */
+int lb_eci_argmax(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq_rowmajor,
+    const double* obj_mean_at_q, double obj_mean_const, const double* con_mean_at_q, double con_mean_const,
+    double* acq_out, double* best_val, int64_t* best_idx);
+/* same, device pointers (eci_params stays on the host); no synchronisation, results on obj's stream */
+int lb_eci_argmax_dev(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* dXq_rowmajor,
+    const double* dObj_mean_at_q, double obj_mean_const, const double* dCon_mean_at_q, double con_mean_const,
+    double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
+
 /* GP::compute_log_lik (gp.hpp:267-282) */
 int lb_log_lik(lb_gp* h, double* out);
 /* GP::compute_kernel_grad_log_lik (gp.hpp:285-311); grad has n_hparams

@@ -175,6 +175,29 @@ namespace limbo_b200 {
                 lb_check(lb_acq_argmax(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, nullptr, &best, &idx), "lb_acq_argmax");
                 return std::make_pair(best, (long)idx);
             }
+            // fused ECI + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem aggregator): this GP is the objective,
+            // `con` the constraint model, whose first output gives Pf (Pf = 1 while it has no samples).  Both mean functors run on
+            // the host.  Without objective samples every value is 0 and the first candidate wins (eci.hpp:86).
+            template <typename ConstraintGP>
+            std::pair<double, long> eci_argmax(const ConstraintGP& con, double f_max, double jitter, const std::vector<Eigen::VectorXd>& vs) const
+            {
+                if (_samples.empty()) return std::make_pair(0.0, 0L);
+                const long M = (long)vs.size();
+                const int D = (int)vs[0].size();
+                const bool use_con = !con._samples.empty();
+                std::vector<double> xq((size_t)M * D), mean0((size_t)M), cmean0(use_con ? (size_t)M : 0);
+                for (long i = 0; i < M; ++i) {
+                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
+                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
+                    if (use_con) cmean0[(size_t)i] = con._mean_function(vs[i], con)(0);
+                }
+                double params[2] = {f_max, jitter}, best = 0;
+                int64_t idx = 0;
+                lb_check(lb_eci_argmax(_h, con._h, params, M, xq.data(), mean0.data(), 0.0, use_con ? cmean0.data() : nullptr, 0.0, nullptr,
+                             &best, &idx),
+                    "lb_eci_argmax");
+                return std::make_pair(best, (long)idx);
+            }
 
             int dim_in() const { assert(_dim_in != -1); return _dim_in; }
             int dim_out() const { assert(_dim_out != -1); return _dim_out; }
@@ -337,6 +360,7 @@ namespace limbo_b200 {
             }
 
         protected:
+            template <typename, typename, typename, typename> friend class GP; // eci_argmax reads the constraint GP's handle and mean
             lb_gp* _h = nullptr;
             int _dim_in;
             int _dim_out;

@@ -5,6 +5,8 @@
 //     using Acq_t  = limbo_b200::acqui::UCB<Params, GP_t>;            // or EI
 //     bayes_opt::BOptimizer<Params, modelfun<GP_t>, acquifun<Acq_t>, acquiopt<limbo_b200::opt::BatchedRandom<Params>>> opt;
 //
+// and, for constrained BO, limbo_b200::acqui::ECI<Params, GP_t, GPc_t> with experimental::bayes_opt::CBOptimizer (INTEGRATION.md).
+//
 // Why: the reference's optimiser contract (opt/optimizer.hpp:84-96; call site bayes_opt/boptimizer.hpp:151-156) hands the
 // policy nothing but a closure `f(x, gradient)` that evaluates ONE point, so every reference policy (RandomPoint,
 // GridSearch, NLOpt, CMA-ES) reaches the model one query() at a time, which leaves a GPU idle.  BatchedRandom keeps the
@@ -19,9 +21,12 @@
 #ifndef LIMBO_B200_OPT_BATCHED_RANDOM_HPP
 #define LIMBO_B200_OPT_BATCHED_RANDOM_HPP
 
+#include <algorithm>
 #include <cmath>
+#include <limits>
 #include <random>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include <Eigen/Core>
@@ -38,6 +43,11 @@ namespace limbo_b200 {
             BO_PARAM(int, refinements, 2);
             BO_PARAM(double, shrink, 0.1);
         };
+    }
+
+    namespace model {
+        template <typename Params, typename KernelFunction, typename MeanFunction, typename HyperParamsOptimizer>
+        class GP;
     }
 
     namespace opt {
@@ -124,16 +134,24 @@ namespace limbo_b200 {
                 for (int i = 0; i < dim_out; ++i) { a(i) = 0.37 + 1.3 * i; b(i) = -2.5 - 0.7 * i; }
                 return afun(a) == a(0) && afun(b) == b(0);
             }
-            template <typename Model>
-            inline void answer_batch(const Model& model, int acq_id, double p0, double p1)
+            // files argmax(candidates) -> (best value, best index) in the pending request, if any
+            template <typename Argmax>
+            inline void answer_batch(const Argmax& argmax)
             {
                 opt::BatchRequest* req = opt::current_batch();
                 if (!req || req->answered || !req->candidates || req->candidates->empty()) return;
-                auto res = model.acq_argmax(acq_id, p0, p1, *req->candidates);
+                auto res = argmax(*req->candidates);
                 req->best_value = res.first;
                 req->best_index = res.second;
                 req->answered = true;
             }
+            template <typename Model>
+            inline void answer_batch(const Model& model, int acq_id, double p0, double p1)
+            {
+                answer_batch([&](const std::vector<Eigen::VectorXd>& c) { return model.acq_argmax(acq_id, p0, p1, c); });
+            }
+            template <typename M> struct is_device_gp : std::false_type {};
+            template <typename P, typename K, typename Mf, typename H> struct is_device_gp<model::GP<P, K, Mf, H>> : std::true_type {};
         }
 
         // acqui::UCB (acqui/ucb.hpp:83-90), batch-aware
@@ -204,6 +222,84 @@ namespace limbo_b200 {
             const Model& _model;
             mutable int _nb_samples;
             mutable double _f_max;
+        };
+
+        // experimental::acqui::ECI (experimental/acqui/eci.hpp:76-130), with the reference's constructor so that
+        // experimental::bayes_opt::CBOptimizer builds it.  When both models are limbo_b200::model::GP and afun acts like FirstElem,
+        // it answers BatchedRandom's request with one fused device pass over both models (GP::eci_argmax -> lb_eci_argmax);
+        // otherwise it evaluates one point at a time, exactly as eci.hpp does.
+        template <typename Params, typename Model, typename ConstraintModel>
+        class ECI {
+        public:
+            ECI(const Model& model, const ConstraintModel& constraint_model, int iteration = 0)
+                : _model(model), _constraint_model(constraint_model), _nb_samples(-1), _f_max(0.0) {}
+            size_t dim_in() const { return _model.dim_in(); }
+            size_t dim_out() const { return _model.dim_out(); }
+
+            template <typename AggregatorFunction>
+            limbo::opt::eval_t operator()(const Eigen::VectorXd& v, const AggregatorFunction& afun, bool gradient) const
+            {
+                assert(!gradient);
+                if constexpr (detail::is_device_gp<Model>::value && detail::is_device_gp<ConstraintModel>::value) {
+                    if (opt::current_batch() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
+                        _update_f_max(afun);
+                        detail::answer_batch([&](const std::vector<Eigen::VectorXd>& c) {
+                            return _model.eci_argmax(_constraint_model, _f_max, Params::acqui_eci::jitter(), c);
+                        });
+                    }
+                }
+                Eigen::VectorXd mu;
+                double sigma_sq;
+                std::tie(mu, sigma_sq) = _model.query(v);
+                const double sigma = std::sqrt(sigma_sq);
+                if (sigma < 1e-10 || _model.samples().size() < 1) return limbo::opt::no_grad(0.0);
+                _update_f_max(afun);
+                const double X = afun(mu) - _f_max - Params::acqui_eci::jitter();
+                const double Z = X / sigma;
+                const double phi = std::exp(-0.5 * std::pow(Z, 2.0)) / std::sqrt(2.0 * M_PI);
+                const double Phi = 0.5 * std::erfc(-Z / std::sqrt(2));
+                return limbo::opt::no_grad(_pf(v, afun) * (X * Phi + sigma * phi));
+            }
+
+        protected:
+            const Model& _model;
+            const ConstraintModel& _constraint_model;
+            mutable int _nb_samples;
+            mutable double _f_max;
+
+            // f_max = max_i afun(mu(x_i)) (eci.hpp:91-99); one batched query on a device GP, one mu() per sample otherwise
+            template <typename AggregatorFunction>
+            void _update_f_max(const AggregatorFunction& afun) const
+            {
+                if (_nb_samples == (int)_model.nb_samples()) return;
+                _f_max = -std::numeric_limits<double>::max();
+                if constexpr (detail::is_device_gp<Model>::value) {
+                    Eigen::MatrixXd mus;
+                    Eigen::VectorXd s2;
+                    _model.query_batch(_model.samples(), mus, s2);
+                    for (long i = 0; i < (long)mus.rows(); ++i) {
+                        Eigen::VectorXd m((Eigen::Index)mus.cols());
+                        for (long p = 0; p < (long)mus.cols(); ++p) m(p) = mus(i, p);
+                        _f_max = std::max(_f_max, (double)afun(m));
+                    }
+                }
+                else
+                    for (const auto& s : _model.samples()) _f_max = std::max(_f_max, (double)afun(_model.mu(s)));
+                _nb_samples = (int)_model.nb_samples();
+            }
+
+            // eci.hpp:116-130
+            template <typename AggregatorFunction>
+            double _pf(const Eigen::VectorXd& v, const AggregatorFunction& afun) const
+            {
+                Eigen::VectorXd mu;
+                double sigma_sq;
+                std::tie(mu, sigma_sq) = _constraint_model.query(v);
+                const double sigma = std::sqrt(sigma_sq);
+                if (sigma < 1e-10 || _constraint_model.samples().size() < 1) return 1.0;
+                const double Z = (afun(mu) - 1.0) / sigma;
+                return 0.5 * std::erfc(-Z / std::sqrt(2));
+            }
         };
     } // namespace acqui
 } // namespace limbo_b200

@@ -20,7 +20,7 @@ GET_K, GET_L, GET_ALPHA, GET_KINV = 0, 1, 2, 3
 DECLARED_SYMBOLS = [
     "lb_create", "lb_destroy", "lb_clone", "lb_set_stream", "lb_sync", "lb_launch_count", "lb_set_data",
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
-    "lb_acq_argmax", "lb_acq_argmax_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_compute_inv_kernel", "lb_log_loo_cv",
+    "lb_acq_argmax", "lb_acq_argmax_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get",
     "lb_nb_samples", "lb_strerror", "lb_last_cuda_error",
 ]
@@ -80,6 +80,8 @@ def load() -> C.CDLL:
         "lb_query_dev": ([p, i64, dp, dp, dp], i32),
         "lb_acq_argmax": ([p, i32, dp, i64, dp, dp, dbl, dp, dp, dp], i32),
         "lb_acq_argmax_dev": ([p, i32, dp, i64, dp, dp, dbl, dp, dp, dp], i32),
+        "lb_eci_argmax": ([p, p, dp, i64, dp, dp, dbl, dp, dbl, dp, dp, dp], i32),
+        "lb_eci_argmax_dev": ([p, p, dp, i64, dp, dp, dbl, dp, dbl, dp, dp, dp], i32),
         "lb_log_lik": ([p, dp], i32),
         "lb_kernel_grad_log_lik": ([p, i32, dp], i32),
         "lb_compute_inv_kernel": ([p], i32),

@@ -1,4 +1,4 @@
-"""Acquisition functions mirroring src/limbo/acqui/{ucb,gp_ucb,ei}.hpp.  The scalar
+"""Acquisition functions mirroring src/limbo/acqui/{ucb,gp_ucb,ei}.hpp and src/limbo/experimental/acqui/eci.hpp.  The scalar
 ``__call__(v, afun, gradient)`` keeps the reference contract (one point, any host
 aggregator); ``argmax_batch`` is the batched device path (FirstElem aggregator)."""
 from __future__ import annotations
@@ -48,8 +48,10 @@ class GP_UCB(UCB):
         return self._beta
 
 
-class EI:
-    def __init__(self, model, iteration: int = 0, params=None):
+class _Improvement:
+    """What EI and ECI share: the objective model and f_max = max_i afun(mu(x_i)) over its samples."""
+
+    def __init__(self, model, params=None):
         self._model, self._params = model, params
         self._nb_samples = -1
         self._f_max = 0.0
@@ -60,11 +62,16 @@ class EI:
     def dim_out(self):
         return self._model.dim_out()
 
-    def _update_f_max(self, afun) -> None:  # ei.hpp:100-108, batched: N mu() calls in one pass
+    def _update_f_max(self, afun) -> None:  # ei.hpp:100-108, eci.hpp:91-99; batched: N mu() calls in one pass
         if self._nb_samples != self._model.nb_samples():
             mu, _ = self._model.query_batch(np.stack(self._model.samples(), axis=0))
             self._f_max = max(afun(m) for m in mu)
             self._nb_samples = self._model.nb_samples()
+
+
+class EI(_Improvement):
+    def __init__(self, model, iteration: int = 0, params=None):
+        super().__init__(model, params)
 
     def __call__(self, v, afun=first_elem, gradient: bool = False):  # ei.hpp:85-116
         assert not gradient
@@ -86,3 +93,45 @@ class EI:
         self._update_f_max(first_elem)
         return self._model.acq_argmax_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], Xq,
                                             return_values)
+
+
+class ECI(_Improvement):
+    """Expected constrained improvement (experimental/acqui/eci.hpp): EI on `model` weighted by the probability Pf that the first
+    output of `constraint_model` exceeds 1.  Pf = 1 when the constraint model has no samples or is None."""
+
+    def __init__(self, model, constraint_model, iteration: int = 0, params=None):
+        super().__init__(model, params)
+        self._constraint_model = constraint_model
+
+    def _jitter(self) -> float:
+        return float(get(self._params, "acqui_eci", "jitter"))
+
+    def __call__(self, v, afun=first_elem, gradient: bool = False):  # eci.hpp:76-107
+        assert not gradient
+        mu, sigma_sq = self._model.query(v)
+        sigma = math.sqrt(sigma_sq)
+        if sigma < 1e-10 or len(self._model.samples()) < 1:
+            return opt.no_grad(0.0)
+        self._update_f_max(afun)
+        X = afun(mu) - self._f_max - self._jitter()
+        Z = X / sigma
+        phi = math.exp(-0.5 * math.pow(Z, 2.0)) / math.sqrt(2.0 * math.pi)
+        Phi = 0.5 * math.erfc(-Z / math.sqrt(2))
+        return opt.no_grad(self._pf(v, afun) * (X * Phi + sigma * phi))
+
+    def _pf(self, v, afun) -> float:  # eci.hpp:116-130
+        if self._constraint_model is None:
+            return 1.0
+        mu, sigma_sq = self._constraint_model.query(v)
+        sigma = math.sqrt(sigma_sq)
+        if sigma < 1e-10 or len(self._constraint_model.samples()) < 1:
+            return 1.0
+        Z = (afun(mu) - 1.0) / sigma
+        return 0.5 * math.erfc(-Z / math.sqrt(2))
+
+    def argmax_batch(self, Xq, return_values: bool = False):
+        if len(self._model.samples()) < 1:
+            vals = np.zeros(len(Xq))
+            return (0.0, 0, vals) if return_values else (0.0, 0)
+        self._update_f_max(first_elem)
+        return self._model.eci_argmax_batch(self._constraint_model, self._f_max, self._jitter(), Xq, return_values)

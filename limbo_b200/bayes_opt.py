@@ -118,3 +118,83 @@ class BOptimizer:
 
     def observations(self):
         return self._observations
+
+
+class CBOptimizer(BOptimizer):
+    """Constrained Bayesian optimisation, mirroring experimental::bayes_opt::CBOptimizer
+    (src/limbo/experimental/bayes_opt/cboptimizer.hpp:149-260).  Every observation holds `dim_out` objective values followed
+    by `nb_constraints` constraint values; an observation is feasible when the product of its constraint values is > 0.  The
+    objective model and a constraint model (default: GP(dim_in, nb_constraints, kernel=Exp, mean=Constant)) are both updated
+    every iteration, and the acquisition (default acqui.ECI) is built over the pair.
+
+    Three deliberate deviations from the reference:
+      (a) the new observation is split into its objective and constraint parts every iteration before add_sample; the
+          reference adds ``_obs[0].back()`` (cboptimizer.hpp:181), which is stale unless something called best_observation();
+      (b) best_sample() returns the sample paired with the best feasible observation; the reference indexes the samples with
+          the position in the feasible-only list (cboptimizer.hpp:228);
+      (c) with nb_constraints == 0 every observation is feasible; the reference indexes an empty constraint list
+          (cboptimizer.hpp:244)."""
+
+    def __init__(self, model, constraint_model=None, params=None, acqui=_acqui.ECI, acqui_opt=None,
+                 rng: np.random.Generator | None = None):
+        super().__init__(model, params, acqui, acqui_opt, rng)
+        self._constraint_model = constraint_model
+        self._dim_out, self._nb_constraints = 1, 0
+
+    def _split(self, observation) -> tuple[np.ndarray, np.ndarray]:  # cboptimizer.hpp:251-272
+        o = np.asarray(observation, dtype=np.float64)
+        assert o.size == self._dim_out + self._nb_constraints
+        return o[: self._dim_out], o[self._dim_out:]
+
+    def optimize(self, sfun, dim_in: int, dim_out: int = 1, nb_constraints: int = 0, afun=_acqui.first_elem,
+                 reset: bool = True) -> None:
+        # cboptimizer.hpp:149-192
+        self._dim_out, self._nb_constraints = int(dim_out), int(nb_constraints)
+        if self._constraint_model is None and self._nb_constraints > 0:
+            from . import kernel as _kernel, mean as _mean
+            from .model import GP
+            self._constraint_model = GP(dim_in, self._nb_constraints, params=self._params, kernel=_kernel.Exp, mean=_mean.Constant)
+        if reset:
+            self._samples, self._observations = [], []
+            self._current_iteration = 0
+        if self._total_iterations == 0 or reset:
+            for _ in range(int(_get(self._params, "init_randomsampling", "samples"))):
+                self.eval_and_add(sfun, self._rng.random(dim_in))
+        if self._observations:
+            parts = [self._split(o) for o in self._observations]
+            self._model.compute(np.stack(self._samples), np.stack([p[0] for p in parts]))
+            if self._nb_constraints > 0:
+                self._constraint_model.compute(np.stack(self._samples), np.stack([p[1] for p in parts]))
+        con = self._constraint_model if self._nb_constraints > 0 else None
+        hp_period = int(get(self._params, "bayes_opt_cboptimizer", "hp_period"))
+        bounded = bool(get(self._params, "bayes_opt_cboptimizer", "bounded"))
+        max_it = int(_get(self._params, "stop_maxiterations", "iterations"))
+        while self._current_iteration < max_it:
+            acqui = self._acqui_cls(self._model, con, self._current_iteration, params=self._params)
+            x = self._acqui_opt(acqui, dim_in, bounded)
+            self.eval_and_add(sfun, x)
+            obj, cons = self._split(self._observations[-1])  # deviation (a)
+            self._model.add_sample(self._samples[-1], obj)
+            if con is not None:
+                con.add_sample(self._samples[-1], cons)
+            if hp_period > 0 and (self._current_iteration + 1) % hp_period == 0:
+                self._model.optimize_hyperparams()
+                if con is not None:
+                    con.optimize_hyperparams()
+            self._current_iteration += 1
+            self._total_iterations += 1
+
+    def _best_index(self, afun) -> int:  # cboptimizer.hpp:197-248, deviations (b) and (c)
+        parts = [self._split(o) for o in self._observations]
+        feasible = [i for i, (_, c) in enumerate(parts) if np.prod(c) > 0]  # prod of no constraints = 1
+        candidates = feasible if feasible else list(range(len(parts)))
+        return max(candidates, key=lambda i: afun(parts[i][0]))  # the first maximum, as std::max_element
+
+    def best_observation(self, afun=_acqui.first_elem) -> np.ndarray:
+        return self._split(self._observations[self._best_index(afun)])[0]
+
+    def best_sample(self, afun=_acqui.first_elem) -> np.ndarray:
+        return self._samples[self._best_index(afun)]
+
+    def constraint_model(self):
+        return self._constraint_model

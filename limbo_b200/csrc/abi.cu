@@ -37,6 +37,9 @@ int lb_launch_query_fused(const lb_gp* h, cudaStream_t st, int64_t M, const doub
 int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu, int mu_stride,
     const double* dMeanAtQ, double mean_const, const double* dS2, double* dAcq, double* dBlkVal, long long* dBlkIdx,
     double* dBestVal, long long* dBestIdx, long long* launches);
+int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
+    double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
+    const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches);
 
 static thread_local std::string g_last_cuda_error;
 void lb_set_last_cuda_error(cudaError_t e, const char* file, int line)
@@ -108,6 +111,7 @@ struct Extra {
     double* hPoint = nullptr;  // pinned, mapped host buffer for the one-point query (mu[P], sigma^2)
     double* dPoint = nullptr;  // its device alias
     int point_cap = 0;
+    cudaEvent_t ev_eci[2] = {}; // lb_eci_argmax's fork / join events, created on first use (the events of h->ev belong to the fit)
 };
 
 } // namespace
@@ -390,6 +394,7 @@ int lb_destroy(lb_gp* hh)
     lb_pool_free(h->dLambda);
     lb_pool_free(h->ex.dMisc);
     if (h->ex.hPoint) cudaFreeHost(h->ex.hPoint);
+    for (cudaEvent_t e : h->ex.ev_eci) if (e) cudaEventDestroy(e);
     for (cudaStream_t* ps : {&h->aux, &h->aux2, &h->aux3})
         if (*ps) { cudaStreamSynchronize(*ps); cudaStreamDestroy(*ps); *ps = nullptr; }
     Shell sh;
@@ -790,17 +795,12 @@ extern "C" int lb_debug_set_query_panel_min(long long m)
     return LB_OK;
 }
 
-static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_dev, double* mu_out, double* s2_out,
-    bool out_dev, int acq_id, const double* acq_params, const double* mean_at_q, double mean_const, double* acq_out,
-    double* best_val, int64_t* best_idx, bool with_acq)
+// Fills h's query workspace, w.dMu (M x P, k^T alpha) and w.dS2 (M), for M candidates on h->stream: the prior, the
+// reduced-precision path, the panel path for large batches, the fused slab path or the multi-launch path.  Xq is row-major
+// M x D, a device pointer when xq_dev.  The caller holds h->ex.qmutex and has checked the handle's state.  A reduced-precision
+// fill leaves its timeout flag in w.dErr (query_timed_out).
+static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
 {
-    if (!hc || M < 0) return LB_ERR_ARG;
-    if (M == 0) return LB_OK;
-    if (!Xq) return LB_ERR_ARG;
-    lb_gp_full* h = full(hc);
-    if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
-    LB_DEVICE(h);
-    std::lock_guard<std::mutex> lock(h->ex.qmutex);
     QueryWs& w = h->ex.ws;
     cudaStream_t st = h->stream;
     const int D = h->D, De = h->kp.D, P = h->P > 0 ? h->P : 1; // raw / staged input dimension
@@ -810,24 +810,6 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
     if ((rc = ensure(h, &w.dS2, &w.s2_bytes, sizeof(double) * M))) return rc;
     const bool prior = (h->N == 0 || !h->fitted);
     if (prior && h->N != 0) return LB_ERR_STATE;
-    if (M == 1 && !prior && !xq_dev && !out_dev && !with_acq && h->precision == LB_PREC_FP64 && lb_query_fused_supported(h) && !h->force_unfused) {
-        // one launch, one synchronisation (query.cu: query_point_kernel)
-        Extra& ex = h->ex;
-        if (ex.point_cap < P + 1) {
-            if (ex.hPoint) cudaFreeHost(ex.hPoint);
-            ex.hPoint = ex.dPoint = nullptr;
-            LB_CUDA(cudaHostAlloc((void**)&ex.hPoint, sizeof(double) * (P + 1 + 7), cudaHostAllocMapped));
-            LB_CUDA(cudaHostGetDevicePointer((void**)&ex.dPoint, ex.hPoint, 0));
-            ex.point_cap = P + 1 + 7;
-        }
-        if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * LB_TILE))) return rc;
-        if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_query_fused_scratch_doubles(h, 1)))) return rc;
-        if ((rc = lb_launch_query_point(h, st, Xq, w.dQs, w.dV, ex.dPoint, &h->launches))) return rc;
-        LB_CUDA(cudaStreamSynchronize(st));
-        if (mu_out) std::memcpy(mu_out, ex.hPoint, sizeof(double) * P);
-        if (s2_out) *s2_out = ex.hPoint[P];
-        return LB_OK;
-    }
     if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma2 = k(v,v) + noise
         LB_CUDA(cudaMemsetAsync(w.dMu, 0, sizeof(double) * M * P, st));
         fill_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w.dS2, M, h->kp.sf2 + h->kp.noise);
@@ -867,12 +849,6 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
                 h->launches++;
                 if ((rc = lb_launch_kstar_tf32(h, st, mc, w.dQs, mcp, w.dKt, w.dV, w.dMu + m0 * P, dBiasUse, &h->launches))) return rc;
                 if ((rc = lb_launch_sigma_tf32(h, st, mc, mcp, w.dKt, w.dNorm2, w.dErr, dBiasUse, w.dS2 + m0, &h->launches))) return rc;
-            }
-            if (!out_dev) {
-                int herr = 0;
-                LB_CUDA(cudaMemcpyAsync(&herr, w.dErr, sizeof(int), cudaMemcpyDeviceToHost, st));
-                LB_CUDA(cudaStreamSynchronize(st));
-                if (herr) return LB_ERR_TIMEOUT;
             }
         }
         else if (M >= query_panel_min() && !h->force_unfused) {
@@ -921,28 +897,91 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
         }
         }
     }
+    return LB_OK;
+}
+
+// per-block (value, index) records of an M-candidate argmax and the final record, in h's query workspace (caller holds qmutex)
+static int ensure_argmax_bufs(lb_gp_full* h, int64_t M)
+{
+    QueryWs& w = h->ex.ws;
+    const int nblk = (int)((M + 255) / 256);
+    if ((size_t)nblk > w.blk_cap) {
+        lb_dfree_sync(h, w.dBlkVal); lb_dfree_sync(h, w.dBlkIdx);
+        w.dBlkVal = nullptr; w.dBlkIdx = nullptr; w.blk_cap = 0;
+        LB_ALLOC(h, w.dBlkVal, sizeof(double) * nblk);
+        LB_ALLOC(h, w.dBlkIdx, sizeof(long long) * nblk);
+        w.blk_cap = nblk;
+    }
+    if (!w.dBest) {
+        LB_ALLOC(h, w.dBest, sizeof(double));
+        LB_ALLOC(h, w.dBestIdx, sizeof(long long));
+    }
+    return LB_OK;
+}
+
+// A device copy of mean_at_q (M values) on h's stream, or mean_at_q itself when it already is a device pointer (or NULL)
+static int mean_on_device(lb_gp_full* h, cudaStream_t st, const double* mean_at_q, int64_t M, bool dev, const double** out)
+{
+    *out = mean_at_q;
+    if (!mean_at_q || dev) return LB_OK;
+    QueryWs& w = h->ex.ws;
+    int rc = ensure(h, &w.dMean, &w.mean_bytes, sizeof(double) * M);
+    if (rc) return rc;
+    LB_CUDA(cudaMemcpyAsync(w.dMean, mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
+    *out = w.dMean;
+    return LB_OK;
+}
+
+// LB_ERR_TIMEOUT when the last reduced-precision fill of h marked its results invalid (synchronises h->stream)
+static int query_timed_out(lb_gp_full* h)
+{
+    if (h->precision == LB_PREC_FP64 || h->N == 0 || !h->ex.ws.dErr) return LB_OK; // N == 0: the prior, no flag written
+    int herr = 0;
+    LB_CUDA(cudaMemcpyAsync(&herr, h->ex.ws.dErr, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaStreamSynchronize(h->stream));
+    return herr ? LB_ERR_TIMEOUT : LB_OK;
+}
+
+static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_dev, double* mu_out, double* s2_out,
+    bool out_dev, int acq_id, const double* acq_params, const double* mean_at_q, double mean_const, double* acq_out,
+    double* best_val, int64_t* best_idx, bool with_acq)
+{
+    if (!hc || M < 0) return LB_ERR_ARG;
+    if (M == 0) return LB_OK;
+    if (!Xq) return LB_ERR_ARG;
+    lb_gp_full* h = full(hc);
+    if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex);
+    QueryWs& w = h->ex.ws;
+    cudaStream_t st = h->stream;
+    const int De = h->kp.D, P = h->P > 0 ? h->P : 1;
+    int rc;
+    const bool prior = (h->N == 0 || !h->fitted);
+    if (M == 1 && !prior && !xq_dev && !out_dev && !with_acq && h->precision == LB_PREC_FP64 && lb_query_fused_supported(h) && !h->force_unfused) {
+        // one launch, one synchronisation (query.cu: query_point_kernel)
+        Extra& ex = h->ex;
+        if (ex.point_cap < P + 1) {
+            if (ex.hPoint) cudaFreeHost(ex.hPoint);
+            ex.hPoint = ex.dPoint = nullptr;
+            LB_CUDA(cudaHostAlloc((void**)&ex.hPoint, sizeof(double) * (P + 1 + 7), cudaHostAllocMapped));
+            LB_CUDA(cudaHostGetDevicePointer((void**)&ex.dPoint, ex.hPoint, 0));
+            ex.point_cap = P + 1 + 7;
+        }
+        if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * LB_TILE))) return rc;
+        if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_query_fused_scratch_doubles(h, 1)))) return rc;
+        if ((rc = lb_launch_query_point(h, st, Xq, w.dQs, w.dV, ex.dPoint, &h->launches))) return rc;
+        LB_CUDA(cudaStreamSynchronize(st));
+        if (mu_out) std::memcpy(mu_out, ex.hPoint, sizeof(double) * P);
+        if (s2_out) *s2_out = ex.hPoint[P];
+        return LB_OK;
+    }
+    if ((rc = query_fill(h, M, Xq, xq_dev))) return rc;
+    if (!out_dev && (rc = query_timed_out(h))) return rc;
     if (with_acq) {
-        const int nblk = (int)((M + 255) / 256);
-        if ((size_t)nblk > w.blk_cap) {
-            lb_dfree_sync(h, w.dBlkVal); lb_dfree_sync(h, w.dBlkIdx);
-            w.dBlkVal = nullptr; w.dBlkIdx = nullptr; w.blk_cap = 0;
-            LB_ALLOC(h, w.dBlkVal, sizeof(double) * nblk);
-            LB_ALLOC(h, w.dBlkIdx, sizeof(long long) * nblk);
-            w.blk_cap = nblk;
-        }
-        if (!w.dBest) {
-            LB_ALLOC(h, w.dBest, sizeof(double));
-            LB_ALLOC(h, w.dBestIdx, sizeof(long long));
-        }
+        if ((rc = ensure_argmax_bufs(h, M))) return rc;
         const double* dMean = nullptr;
-        if (mean_at_q) {
-            if (out_dev) dMean = mean_at_q;
-            else {
-                if ((rc = ensure(h, &w.dMean, &w.mean_bytes, sizeof(double) * M))) return rc;
-                LB_CUDA(cudaMemcpyAsync(w.dMean, mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
-                dMean = w.dMean;
-            }
-        }
+        if ((rc = mean_on_device(h, st, mean_at_q, M, out_dev, &dMean))) return rc;
         double* dAcq = nullptr;
         if (acq_out) {
             if (out_dev) dAcq = acq_out;
@@ -1002,6 +1041,131 @@ int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int6
     if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_UNSUPPORTED;
     return query_common(h, M, dXq, true, nullptr, nullptr, true, acq_id, acq_params, dMean_at_q, mean_const, dAcq_out,
         dBest_val, dBest_idx, true);
+}
+
+static int ensure_eci_events(lb_gp_full* h)
+{
+    for (cudaEvent_t& e : h->ex.ev_eci)
+        if (!e) LB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    return LB_OK;
+}
+
+// experimental/acqui/eci.hpp:76-130 over the objective handle o and the constraint handle c (NULL: no constraint model).  Both
+// handles' qmutex are held.  The objective's query runs on o's stream, the constraint's on c's stream (they may overlap), and
+// the fused epilogue (query.cu: eci_kernel) on o's stream once both are done.  dev: every pointer is a device pointer and the
+// call does not synchronise.
+static int eci_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double jitter, int64_t M, const double* Xq, bool dev,
+    const double* obj_mean_at_q, double obj_mean_const, const double* con_mean_at_q, double con_mean_const, double* acq_out,
+    double* best_val, int64_t* best_idx)
+{
+    cudaStream_t st = o->stream;
+    QueryWs& w = o->ex.ws;
+    int rc;
+    if (o->N == 0) { // eci.hpp:86: no objective samples, every value is 0 and the first candidate wins
+        if (dev) {
+            if (acq_out) LB_CUDA(cudaMemsetAsync(acq_out, 0, sizeof(double) * M, st));
+            LB_CUDA(cudaMemsetAsync(best_val, 0, sizeof(double), st));
+            LB_CUDA(cudaMemsetAsync(best_idx, 0, sizeof(int64_t), st));
+        }
+        else {
+            if (acq_out) std::fill(acq_out, acq_out + M, 0.0);
+            *best_val = 0.0;
+            *best_idx = 0;
+        }
+        return LB_OK;
+    }
+    if (o->D <= 0 || !o->kernel_set) return LB_ERR_STATE;
+    const bool use_con = c && c->N > 0; // eci.hpp:124: Pf = 1 without constraint samples
+    if (use_con && c->D != o->D) return LB_ERR_ARG;
+    if (use_con && !c->kernel_set) return LB_ERR_STATE;
+    if ((rc = ensure_eci_events(o))) return rc;
+    if (use_con && (rc = ensure_eci_events(c))) return rc;
+    const double* dXq = Xq;
+    if (!dev) { // one upload, read by both queries
+        if ((rc = ensure(o, &w.dQraw, &w.qraw_bytes, sizeof(double) * M * o->D))) return rc;
+        LB_CUDA(cudaMemcpyAsync(w.dQraw, Xq, sizeof(double) * M * o->D, cudaMemcpyHostToDevice, st));
+        dXq = w.dQraw;
+    }
+    if (use_con) {
+        LB_CUDA(cudaEventRecord(o->ex.ev_eci[0], st));
+        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[0], 0));
+    }
+    rc = query_fill(o, M, dXq, true);
+    int rc_con = (rc == LB_OK && use_con) ? query_fill(c, M, dXq, true) : LB_OK;
+    if (use_con) { // o's stream waits for the constraint's mu / sigma^2 (and for c's last read of o's candidate buffer)
+        LB_CUDA(cudaEventRecord(c->ex.ev_eci[0], c->stream));
+        LB_CUDA(cudaStreamWaitEvent(st, c->ex.ev_eci[0], 0));
+    }
+    if (rc) return rc;
+    if (rc_con) return rc_con;
+    if (!dev) {
+        if ((rc = query_timed_out(o))) return rc;
+        if (use_con && (rc = query_timed_out(c))) return rc;
+    }
+    if ((rc = ensure_argmax_bufs(o, M))) return rc;
+    const double* dMeanObj = nullptr;
+    const double* dMeanCon = nullptr;
+    if ((rc = mean_on_device(o, st, obj_mean_at_q, M, dev, &dMeanObj))) return rc;
+    if (use_con && (rc = mean_on_device(c, st, con_mean_at_q, M, dev, &dMeanCon))) return rc;
+    double* dAcq = acq_out;
+    if (acq_out && !dev) {
+        if ((rc = ensure(o, &w.dAcq, &w.acq_bytes, sizeof(double) * M))) return rc;
+        dAcq = w.dAcq;
+    }
+    double* dBV = dev ? best_val : w.dBest;
+    long long* dBI = dev ? (long long*)best_idx : w.dBestIdx;
+    const int Po = o->P > 0 ? o->P : 1, Pc = (use_con && c->P > 0) ? c->P : 1;
+    rc = lb_launch_eci_full(st, f_max, jitter, M, w.dMu, Po, dMeanObj, obj_mean_const, w.dS2, use_con ? c->ex.ws.dMu : nullptr, Pc,
+        dMeanCon, con_mean_const, use_con ? c->ex.ws.dS2 : nullptr, dAcq, w.dBlkVal, w.dBlkIdx, dBV, dBI, &o->launches);
+    if (use_con) { // a later call on c must not overwrite the buffers the epilogue reads before it has run
+        LB_CUDA(cudaEventRecord(o->ex.ev_eci[1], st));
+        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[1], 0));
+    }
+    if (rc) return rc;
+    if (!dev) {
+        if (acq_out) LB_CUDA(cudaMemcpyAsync(acq_out, w.dAcq, sizeof(double) * M, cudaMemcpyDeviceToHost, st));
+        long long bi = 0;
+        LB_CUDA(cudaMemcpyAsync(best_val, w.dBest, sizeof(double), cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(&bi, w.dBestIdx, sizeof(long long), cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaStreamSynchronize(st));
+        *best_idx = (int64_t)bi;
+    }
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+
+static int eci_common(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq, bool dev,
+    const double* obj_mean_at_q, double obj_mean_const, const double* con_mean_at_q, double con_mean_const, double* acq_out,
+    double* best_val, int64_t* best_idx)
+{
+    if (!obj || obj == con || !eci_params || M <= 0 || !Xq || !best_val || !best_idx) return LB_ERR_ARG;
+    if (con && con->device != obj->device) return LB_ERR_ARG;
+    lb_gp_full* o = full(obj);
+    lb_gp_full* c = con ? full(con) : nullptr;
+    LB_DEVICE(o);
+    if (!c) {
+        std::lock_guard<std::mutex> lock(o->ex.qmutex);
+        return eci_locked(o, nullptr, eci_params[0], eci_params[1], M, Xq, dev, obj_mean_at_q, obj_mean_const, nullptr, 0.0, acq_out,
+            best_val, best_idx);
+    }
+    std::scoped_lock lock(o->ex.qmutex, c->ex.qmutex); // deadlock-free whatever order other callers pass the pair in
+    return eci_locked(o, c, eci_params[0], eci_params[1], M, Xq, dev, obj_mean_at_q, obj_mean_const, con_mean_at_q, con_mean_const,
+        acq_out, best_val, best_idx);
+}
+
+int lb_eci_argmax(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq_rowmajor,
+    const double* obj_mean_at_q, double obj_mean_const, const double* con_mean_at_q, double con_mean_const, double* acq_out,
+    double* best_val, int64_t* best_idx)
+{
+    return eci_common(obj, con, eci_params, M, Xq_rowmajor, false, obj_mean_at_q, obj_mean_const, con_mean_at_q, con_mean_const,
+        acq_out, best_val, best_idx);
+}
+int lb_eci_argmax_dev(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* dXq_rowmajor,
+    const double* dObj_mean_at_q, double obj_mean_const, const double* dCon_mean_at_q, double con_mean_const, double* dAcq_out,
+    double* dBest_val, int64_t* dBest_idx)
+{
+    return eci_common(obj, con, eci_params, M, dXq_rowmajor, true, dObj_mean_at_q, obj_mean_const, dCon_mean_at_q, con_mean_const,
+        dAcq_out, dBest_val, dBest_idx);
 }
 
 int lb_log_lik(lb_gp* hh, double* out)

@@ -158,38 +158,34 @@ colnorm_kernel(const double* __restrict__ V, int64_t Np, double kvv, double nois
     }
 }
 
-// acquisition value per candidate (FirstElem aggregator, bo_base.hpp:99-105)
-//   acq_id 0: UCB / GP_UCB  mu + p0 * sqrt(s2)                 ucb.hpp:89, gp_ucb.hpp:102
-//   acq_id 1: EI  (p0 = f_max, p1 = jitter)                    ei.hpp:92-115
-__device__ __forceinline__ double acq_value(int acq_id, double mu, double s2, double p0, double p1)
+// expected improvement of mu over f_max + jitter, 0 when sigma < 1e-10: ei.hpp:92-115, and the factor eci.hpp:86-106 weights
+__device__ __forceinline__ double ei_factor(double mu, double s2, double f_max, double jitter)
 {
-    if (acq_id == 0) return mu + p0 * sqrt(s2);
     double sigma = sqrt(s2);
     if (sigma < 1e-10) return 0.0;
-    double X = mu - p0 - p1;
+    double X = mu - f_max - jitter;
     double Z = X / sigma;
     double phi = exp(-0.5 * (Z * Z)) / sqrt(2.0 * M_PI);
     double Phi = 0.5 * erfc(-Z / sqrt(2.0));
     return X * Phi + sigma * phi;
 }
 
-__global__ void __launch_bounds__(256)
-acq_kernel(int acq_id, double p0, double p1, int64_t M, const double* __restrict__ mu0, int mu_stride,
-    const double* __restrict__ mean_at_q, double mean_const, const double* __restrict__ s2, double* __restrict__ acq,
-    double* __restrict__ blk_val, long long* __restrict__ blk_idx)
+// acquisition value per candidate (FirstElem aggregator, bo_base.hpp:99-105)
+//   acq_id 0: UCB / GP_UCB  mu + p0 * sqrt(s2)                 ucb.hpp:89, gp_ucb.hpp:102
+//   acq_id 1: EI  (p0 = f_max, p1 = jitter)                    ei.hpp:92-115
+__device__ __forceinline__ double acq_value(int acq_id, double mu, double s2, double p0, double p1)
+{
+    if (acq_id == 0) return mu + p0 * sqrt(s2);
+    return ei_factor(mu, s2, p0, p1);
+}
+
+// (value, index) of a 256-thread block's best candidate into blk_val / blk_idx[blockIdx.x].  NaN never wins; the lowest
+// index wins ties.  Threads without a candidate pass (-DBL_MAX, LLONG_MAX).
+__device__ __forceinline__ void block_argmax(double v, long long idx, double* __restrict__ blk_val, long long* __restrict__ blk_idx)
 {
     __shared__ double sv[256];
     __shared__ long long si[256];
-    int64_t m = blockIdx.x * (int64_t)256 + threadIdx.x;
-    double v = -DBL_MAX;
-    long long idx = LLONG_MAX;
-    if (m < M) {
-        double mu = mu0[m * mu_stride] + (mean_at_q ? mean_at_q[m] : mean_const);
-        v = acq_value(acq_id, mu, s2[m], p0, p1);
-        if (acq) acq[m] = v;
-        idx = m;
-        if (!(v == v)) { v = -DBL_MAX; } // NaN never wins
-    }
+    if (!(v == v)) { v = -DBL_MAX; }
     sv[threadIdx.x] = v;
     si[threadIdx.x] = idx;
     __syncthreads();
@@ -208,6 +204,59 @@ acq_kernel(int acq_id, double p0, double p1, int64_t M, const double* __restrict
         blk_val[blockIdx.x] = sv[0];
         blk_idx[blockIdx.x] = si[0];
     }
+}
+
+__global__ void __launch_bounds__(256)
+acq_kernel(int acq_id, double p0, double p1, int64_t M, const double* __restrict__ mu0, int mu_stride,
+    const double* __restrict__ mean_at_q, double mean_const, const double* __restrict__ s2, double* __restrict__ acq,
+    double* __restrict__ blk_val, long long* __restrict__ blk_idx)
+{
+    int64_t m = blockIdx.x * (int64_t)256 + threadIdx.x;
+    double v = -DBL_MAX;
+    long long idx = LLONG_MAX;
+    if (m < M) {
+        double mu = mu0[m * mu_stride] + (mean_at_q ? mean_at_q[m] : mean_const);
+        v = acq_value(acq_id, mu, s2[m], p0, p1);
+        if (acq) acq[m] = v;
+        idx = m;
+    }
+    block_argmax(v, idx, blk_val, blk_idx);
+}
+
+// experimental/acqui/eci.hpp:76-130 per candidate, FirstElem aggregator: the objective's EI factor times the probability
+// that the constraint model's first output exceeds 1,
+//   Pf = Phi((mu_c - 1) / sigma_c), or 1 when sigma_c < 1e-10 or there is no constraint model (mu_con == nullptr).
+// mu_obj / mu_con are k^T alpha (strides p_obj / p_con); the host mean functors' first output is added here, from an array or
+// a constant, as in acq_kernel.
+__global__ void __launch_bounds__(256)
+eci_kernel(double f_max, double jitter, int64_t M, const double* __restrict__ mu_obj, int p_obj, const double* __restrict__ mean_obj,
+    double mean_obj_const, const double* __restrict__ s2_obj, const double* __restrict__ mu_con, int p_con,
+    const double* __restrict__ mean_con, double mean_con_const, const double* __restrict__ s2_con, double* __restrict__ acq,
+    double* __restrict__ blk_val, long long* __restrict__ blk_idx)
+{
+    int64_t m = blockIdx.x * (int64_t)256 + threadIdx.x;
+    double v = -DBL_MAX;
+    long long idx = LLONG_MAX;
+    if (m < M) {
+        const double s2 = s2_obj[m];
+        v = 0.0;
+        if (!(sqrt(s2) < 1e-10)) { // eci.hpp:86: 0 before the constraint model is consulted
+            double pf = 1.0;
+            if (mu_con) {
+                const double sigma_c = sqrt(s2_con[m]);
+                if (!(sigma_c < 1e-10)) {
+                    const double mu_c = mu_con[m * p_con] + (mean_con ? mean_con[m] : mean_con_const);
+                    const double Z = (mu_c - 1.0) / sigma_c;
+                    pf = 0.5 * erfc(-Z / sqrt(2.0));
+                }
+            }
+            const double mu = mu_obj[m * p_obj] + (mean_obj ? mean_obj[m] : mean_obj_const);
+            v = pf * ei_factor(mu, s2, f_max, jitter);
+        }
+        if (acq) acq[m] = v;
+        idx = m;
+    }
+    block_argmax(v, idx, blk_val, blk_idx);
 }
 
 __global__ void __launch_bounds__(256)
@@ -308,6 +357,19 @@ int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_
 {
     const int nblk = (int)((M + 255) / 256);
     acq_kernel<<<nblk, 256, 0, st>>>(acq_id, p0, p1, M, dMu, mu_stride, dMeanAtQ, mean_const, dS2, dAcq, dBlkVal, dBlkIdx);
+    argmax_final_kernel<<<1, 256, 0, st>>>(nblk, dBlkVal, dBlkIdx, dBestVal, dBestIdx);
+    if (launches) *launches += 2;
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+
+int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
+    double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
+    const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches)
+{
+    const int nblk = (int)((M + 255) / 256);
+    eci_kernel<<<nblk, 256, 0, st>>>(f_max, jitter, M, dMuObj, p_obj, dMeanObj, mean_obj_const, dS2Obj, dMuCon, p_con, dMeanCon,
+        mean_con_const, dS2Con, dAcq, dBlkVal, dBlkIdx);
     argmax_final_kernel<<<1, 256, 0, st>>>(nblk, dBlkVal, dBlkIdx, dBestVal, dBestIdx);
     if (launches) *launches += 2;
     LB_CUDA(cudaGetLastError());

@@ -206,12 +206,8 @@ class GP:
         ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
         if ap.size < 2:
             ap = np.append(ap, 0.0)
-        if self._mean_function.is_constant():
-            mptr, mconst = None, float(np.asarray(self._mean_function(Xq[0], self))[0])
-            mean0 = None
-        else:
-            mean0 = np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0])
-            mptr, mconst = _ptr(mean0), 0.0
+        mean0, mconst = self._first_mean(Xq)
+        mptr = _ptr(mean0) if mean0 is not None else None
         vals = np.empty(M) if return_values else None
         best = C.c_double()
         idx = C.c_int64()
@@ -221,6 +217,36 @@ class GP:
         if return_values:
             return best.value, idx.value, vals
         return best.value, idx.value
+
+    def eci_argmax_batch(self, constraint_model, f_max: float, jitter: float, Xq, return_values: bool = False):
+        """Fused batched expected constrained improvement + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem
+        aggregator): this GP is the objective, `constraint_model` (a GP on the same device, or None for no constraints) gives
+        Pf from its first output.  Returns (best_value, best_index[, values])."""
+        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        M = Xq.shape[0]
+        ep = np.array([f_max, jitter], dtype=np.float64)
+        mean0, mconst = self._first_mean(Xq)
+        con_h, cmean0, cconst = None, None, 0.0
+        if constraint_model is not None:
+            con_h = constraint_model._h
+            if constraint_model.nb_samples() > 0:
+                cmean0, cconst = constraint_model._first_mean(Xq)
+        vals = np.empty(M) if return_values else None
+        best = C.c_double()
+        idx = C.c_int64()
+        _lib.check(self._lib.lb_eci_argmax(self._h, con_h, _ptr(ep), M, _ptr(Xq), _ptr(mean0) if mean0 is not None else None, mconst,
+                                           _ptr(cmean0) if cmean0 is not None else None, cconst,
+                                           _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
+                   "lb_eci_argmax")
+        if return_values:
+            return best.value, idx.value, vals
+        return best.value, idx.value
+
+    def _first_mean(self, Xq):
+        """First output of the mean functor at every candidate, as (array, 0.0), or (None, constant) for a constant mean."""
+        if self._mean_function.is_constant():
+            return None, float(np.asarray(self._mean_function(Xq[0], self))[0])
+        return np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0]), 0.0
 
     # ---- accessors gp.hpp:194-238 ----
     def dim_in(self) -> int:

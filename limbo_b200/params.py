@@ -37,6 +37,9 @@ class defaults:
     class acqui_ei:  # acqui/ei.hpp:57-60
         jitter = 0.0
 
+    class acqui_eci:  # experimental/acqui/eci.hpp:57-62
+        jitter = 0.0
+
     class opt_rprop:  # opt/rprop.hpp:58-65
         iterations = 300
         eps_stop = 0.0
@@ -47,6 +50,10 @@ class defaults:
 
     class bayes_opt_boptimizer:  # bayes_opt/boptimizer.hpp:68-72
         hp_period = -1
+
+    class bayes_opt_cboptimizer:  # experimental/bayes_opt/cboptimizer.hpp:68-73
+        hp_period = -1
+        bounded = True
 
 
 class Params:
