@@ -143,6 +143,19 @@ int lb_eci_argmax_dev(const lb_gp* obj, const lb_gp* con, const double* eci_para
     const double* dObj_mean_at_q, double obj_mean_const, const double* dCon_mean_at_q, double con_mean_const,
     double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
 
+/* model::SparsifiedGP::_sparsify (model/sparsified_gp.hpp:121-183): while more than max_points of the N points (row-major N x D)
+ * remain, remove the densest one, the point whose k = D nearest remaining neighbours have the smallest sum of Euclidean distances
+ * (lowest index on equal sums), until max_points remain or no sum is below DBL_MAX.  Runs on h's device and stream with its pool
+ * under h's query lock; h's model state is not touched.  kept (room for N): the n_kept kept indices, ascending; removed /
+ * removed_score (room for N - max_points each, may be NULL): the removal order and the sum each removed point had when it was
+ * chosen.  N <= max_points keeps every point and launches nothing.  LB_ERR_ARG when max_points < D or a coordinate is not finite
+ * (both undefined in the reference); LB_ERR_UNSUPPORTED when D > 64; LB_ERR_TIMEOUT when a device-side wait timed out. */
+int lb_sparsify(const lb_gp* h, int64_t N, int D, const double* X_rowmajor, int64_t max_points, int64_t* kept, int64_t* n_kept,
+    int64_t* removed, double* removed_score);
+/* same, device pointers except n_kept (host); synchronises h's stream */
+int lb_sparsify_dev(const lb_gp* h, int64_t N, int D, const double* dX_rowmajor, int64_t max_points, int64_t* dKept,
+    int64_t* n_kept, int64_t* dRemoved, double* dRemovedScore);
+
 /* GP::compute_log_lik (gp.hpp:267-282) */
 int lb_log_lik(lb_gp* h, double* out);
 /* GP::compute_kernel_grad_log_lik (gp.hpp:285-311); grad has n_hparams

@@ -40,6 +40,8 @@ int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_
 int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
     double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
     const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches);
+int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const double* dX, int64_t max_points, long long* dKept,
+    int64_t* n_kept, long long* dRemoved, double* dRemovedScore, long long* launches);
 
 static thread_local std::string g_last_cuda_error;
 void lb_set_last_cuda_error(cudaError_t e, const char* file, int line)
@@ -1166,6 +1168,63 @@ int lb_eci_argmax_dev(const lb_gp* obj, const lb_gp* con, const double* eci_para
 {
     return eci_common(obj, con, eci_params, M, dXq_rowmajor, true, dObj_mean_at_q, obj_mean_const, dCon_mean_at_q, con_mean_const,
         dAcq_out, dBest_val, dBest_idx);
+}
+
+// model::SparsifiedGP::_sparsify (sparsified_gp.hpp:121-183) on h's device and stream, under h's query lock (the call uses h's
+// stream but not its model state).  N <= max_points keeps every point and launches nothing.
+static int sparsify_common(const lb_gp* hc, int64_t N, int D, const double* X, int64_t max_points, int64_t* kept, int64_t* n_kept,
+    int64_t* removed, double* removed_score, bool dev)
+{
+    if (!hc || N < 0 || D < 1 || max_points < 0 || !n_kept || (N > 0 && (!X || !kept))) return LB_ERR_ARG;
+    if (D > LB_MAX_D || N >= INT32_MAX) return LB_ERR_UNSUPPORTED;
+    if (max_points < D) return LB_ERR_ARG; // the reference's partial_sort would run past end()
+    lb_gp_full* h = full(hc);
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex);
+    cudaStream_t st = h->stream;
+    if (N <= max_points) {
+        std::vector<int64_t> all((size_t)N);
+        for (int64_t i = 0; i < N; ++i) all[(size_t)i] = i;
+        if (dev && N > 0) {
+            LB_CUDA(cudaMemcpyAsync(kept, all.data(), sizeof(int64_t) * N, cudaMemcpyHostToDevice, st));
+            LB_CUDA(cudaStreamSynchronize(st));
+        }
+        else if (N > 0) std::memcpy(kept, all.data(), sizeof(int64_t) * N);
+        *n_kept = N;
+        return LB_OK;
+    }
+    if (dev) return lb_run_sparsify(h, st, N, D, X, max_points, (long long*)kept, n_kept, (long long*)removed, removed_score, &h->launches);
+    double* dX = nullptr;
+    long long *dKept = nullptr, *dRm = nullptr;
+    double* dRs = nullptr;
+    int rc = LB_OK;
+    if (!(rc = lb_dalloc(h, &dX, sizeof(double) * N * D)) && !(rc = lb_dalloc(h, &dKept, sizeof(long long) * N)) &&
+        (!removed || !(rc = lb_dalloc(h, &dRm, sizeof(long long) * N))) && (!removed_score || !(rc = lb_dalloc(h, &dRs, sizeof(double) * N)))) {
+        cudaError_t e = cudaMemcpyAsync(dX, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) { lb_set_last_cuda_error(e, __FILE__, __LINE__); rc = LB_ERR_CUDA; }
+        if (!rc) rc = lb_run_sparsify(h, st, N, D, dX, max_points, dKept, n_kept, dRm, dRs, &h->launches);
+        const int64_t nr = rc ? 0 : N - *n_kept;
+        if (!rc && (e = cudaMemcpyAsync(kept, dKept, sizeof(int64_t) * *n_kept, cudaMemcpyDeviceToHost, st)) == cudaSuccess && nr > 0) {
+            if (removed) e = cudaMemcpyAsync(removed, dRm, sizeof(int64_t) * nr, cudaMemcpyDeviceToHost, st);
+            if (e == cudaSuccess && removed_score) e = cudaMemcpyAsync(removed_score, dRs, sizeof(double) * nr, cudaMemcpyDeviceToHost, st);
+        }
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (!rc && e != cudaSuccess) { lb_set_last_cuda_error(e, __FILE__, __LINE__); rc = LB_ERR_CUDA; }
+    }
+    cudaStreamSynchronize(st);
+    for (void* q : {(void*)dX, (void*)dKept, (void*)dRm, (void*)dRs}) lb_pool_free(q);
+    return rc;
+}
+
+int lb_sparsify(const lb_gp* h, int64_t N, int D, const double* X_rowmajor, int64_t max_points, int64_t* kept, int64_t* n_kept,
+    int64_t* removed, double* removed_score)
+{
+    return sparsify_common(h, N, D, X_rowmajor, max_points, kept, n_kept, removed, removed_score, false);
+}
+int lb_sparsify_dev(const lb_gp* h, int64_t N, int D, const double* dX_rowmajor, int64_t max_points, int64_t* dKept, int64_t* n_kept,
+    int64_t* dRemoved, double* dRemovedScore)
+{
+    return sparsify_common(h, N, D, dX_rowmajor, max_points, dKept, n_kept, dRemoved, dRemovedScore, true);
 }
 
 int lb_log_lik(lb_gp* hh, double* out)

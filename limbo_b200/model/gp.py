@@ -61,7 +61,7 @@ class GP:
     # ---- copy semantics (kernel_lf_opt.hpp:79 copies the GP per evaluation) ----
     def copy(self) -> "GP":
         import copy as _copy
-        g = GP.__new__(GP)
+        g = type(self).__new__(type(self))
         g.__dict__.update({k: v for k, v in self.__dict__.items() if k not in ("_h", "_host_cache")})
         g._kernel_function = _copy.deepcopy(self._kernel_function)
         g._mean_function = _copy.deepcopy(self._mean_function)

@@ -48,6 +48,9 @@ class defaults:
         repeats = 10
         epsilon = 1e-2
 
+    class model_sparse_gp:  # model/sparsified_gp.hpp:56-60
+        max_points = 200
+
     class bayes_opt_boptimizer:  # bayes_opt/boptimizer.hpp:68-72
         hp_period = -1
 
