@@ -156,6 +156,32 @@ int lb_sparsify(const lb_gp* h, int64_t N, int D, const double* X_rowmajor, int6
 int lb_sparsify_dev(const lb_gp* h, int64_t N, int D, const double* dX_rowmajor, int64_t max_points, int64_t* dKept,
     int64_t* n_kept, int64_t* dRemoved, double* dRemovedScore);
 
+/* experimental::model::SPGP (experimental/model/spgp.hpp): Snelson and Ghahramani's sparse GP with M pseudo-inputs, single
+ * output, SE-ARD.  Same conventions as lb_gp; lb_spgp_query and lb_spgp_acq_argmax may be called from several threads, the other
+ * calls need exclusive access.  w is the reference's parameter vector (HyperParams, spgp.hpp:94-101) of n_w = (M+1) D + 2
+ * entries: [xb (M x D, column-major), log b (D; b = inverse squared length scales), log c (signal variance), log sig (noise
+ * variance)].  lb_spgp_lik and lb_spgp_compute return LB_ERR_ARG for M < 1, M > N, n_w != (M+1) D + 2 or a non-finite w, and
+ * the 1-based index (> 0) of the first non-positive pivot of Q = K(xb, xb) + jitter I, or else of A = sig I + V V^T. */
+typedef struct lb_spgp lb_spgp;
+int lb_spgp_create(lb_spgp** out, int device);
+int lb_spgp_destroy(lb_spgp* s);
+/* SPGP::_init data (spgp.hpp:353-370): N samples (row-major N x D) and y_zm = observations - mean (N).  LB_ERR_UNSUPPORTED
+ * when D > 64, LB_ERR_ARG for a non-finite value. */
+int lb_spgp_set_data(lb_spgp* s, int64_t N, int D, const double* X_rowmajor, const double* y_zm);
+/* SPGP::_likelihood(w, grad != NULL) (spgp.hpp:446-580) with inverse = true: f = -fw and grad = -dfw (n_w entries).  The value
+ * keeps the reference's integer (N - M) / 2 in the log(sig) term. */
+int lb_spgp_lik(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double jitter, double* f, double* grad);
+/* SPGP::_compute(false) (spgp.hpp:389-407) at HyperParams(w): leaves L, Lm and bet on the device for the queries. */
+int lb_spgp_compute(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double jitter);
+/* SPGP::_predict (spgp.hpp:582-610) for Mq candidates (row-major Mq x D): mu_minus_mean (Mq, without mean(v)) and sigma2 (Mq,
+ * + sig when optimized != 0).  LB_ERR_STATE before lb_spgp_compute. */
+int lb_spgp_query(const lb_spgp* s, int64_t Mq, const double* Xq_rowmajor, int optimized, double* mu_minus_mean, double* sigma2);
+/* lb_acq_argmax over lb_spgp_query's mu and sigma^2 (ties to the lowest index). */
+int lb_spgp_acq_argmax(const lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* Xq_rowmajor, int optimized,
+    const double* mean_at_q, double mean_const, double* acq_out, double* best_val, int64_t* best_idx);
+/* kernels launched by this model so far */
+long long lb_spgp_launch_count(const lb_spgp* s);
+
 /* GP::compute_log_lik (gp.hpp:267-282) */
 int lb_log_lik(lb_gp* h, double* out);
 /* GP::compute_kernel_grad_log_lik (gp.hpp:285-311); grad has n_hparams

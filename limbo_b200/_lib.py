@@ -22,7 +22,8 @@ DECLARED_SYMBOLS = [
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
     "lb_acq_argmax", "lb_acq_argmax_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
-    "lb_nb_samples", "lb_strerror", "lb_last_cuda_error",
+    "lb_nb_samples", "lb_strerror", "lb_last_cuda_error", "lb_spgp_create", "lb_spgp_destroy", "lb_spgp_set_data", "lb_spgp_lik",
+    "lb_spgp_compute", "lb_spgp_query", "lb_spgp_acq_argmax", "lb_spgp_launch_count",
 ]
 
 _lib = None
@@ -94,6 +95,14 @@ def load() -> C.CDLL:
         "lb_debug_sparsify_timing": ([i32], i32),
         "lb_debug_sparsify_last_ms": ([dp], i32),
         "lb_nb_samples": ([p], i64),
+        "lb_spgp_create": ([C.POINTER(p), i32], i32),
+        "lb_spgp_destroy": ([p], i32),
+        "lb_spgp_set_data": ([p, i64, i32, dp, dp], i32),
+        "lb_spgp_lik": ([p, i64, i64, dp, dbl, dp, dp], i32),
+        "lb_spgp_compute": ([p, i64, i64, dp, dbl], i32),
+        "lb_spgp_query": ([p, i64, dp, i32, dp, dp], i32),
+        "lb_spgp_acq_argmax": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
+        "lb_spgp_launch_count": ([p], C.c_longlong),
         "lb_strerror": ([i32], C.c_char_p),
         "lb_last_cuda_error": ([], C.c_char_p),
     }

@@ -51,6 +51,16 @@ class defaults:
     class model_sparse_gp:  # model/sparsified_gp.hpp:56-60
         max_points = 200
 
+    class model_spgp:  # experimental/model/spgp.hpp:64-73
+        jitter = 0.000001
+        samples_percent = 10
+        min_m = 1
+        # the reference's hyper-parameters before the first compute (spgp.hpp:112-114, 165-167); no prediction reads them: without
+        # samples it uses the kernel functor, and every compute / add_sample optimises.  Kept for Params compatibility.
+        sig = 0.01
+        pred_kernel_sigma_sq = 0.5
+        pred_kernel_l = 0.5
+
     class bayes_opt_boptimizer:  # bayes_opt/boptimizer.hpp:68-72
         hp_period = -1
 
