@@ -64,6 +64,7 @@ def load() -> C.CDLL:
         "lb_debug_append_count": ([p], C.c_longlong),
         "lb_debug_pool_mallocs": ([], C.c_longlong),
         "lb_debug_pool_hits": ([], C.c_longlong),
+        "lb_debug_pool_live": ([], C.c_longlong),
         "lb_pool_trim": ([], i32),
         "lb_debug_set_query_panel_min": ([C.c_longlong], i32),
         "lb_set_data": ([p, i64, i32, i32, dp, dp], i32),

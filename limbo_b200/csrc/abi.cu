@@ -93,27 +93,23 @@ void lb_prof_end(const lb_gp* h, cudaStream_t st, int cls)
 namespace {
 
 struct QueryWs { // per-handle query workspace (guarded by qmutex)
-    double* dQraw = nullptr; size_t qraw_bytes = 0;   // M x D row-major staging
-    double* dQs = nullptr; size_t qs_bytes = 0;       // D x Mp
-    double* dV = nullptr; size_t v_bytes = 0;         // Np x Mc
-    double* dMu = nullptr; size_t mu_bytes = 0;       // M x P
-    double* dS2 = nullptr; size_t s2_bytes = 0;       // M
-    double* dAcq = nullptr; size_t acq_bytes = 0;     // M
-    double* dBlkVal = nullptr; long long* dBlkIdx = nullptr; size_t blk_cap = 0;
-    double* dBest = nullptr; // [0] value ; long long index follows
-    long long* dBestIdx = nullptr;
-    double* dMean = nullptr; size_t mean_bytes = 0;
-    double* dFront = nullptr; size_t front_bytes = 0; // lb_ehvi_argmax: the front sorted by f[0] (k x 2)
-    float* dKt = nullptr; size_t kt_bytes = 0;         // TF32 path: K*^T chunk (Mc x Np fp32)
-    float* dNorm2 = nullptr; size_t norm2_bytes = 0;
-    double* dBias = nullptr; size_t bias_bytes = 0;    // reduced-precision path: rounding-bias weight per candidate
-    int* dErr = nullptr;
+    DevBuf<double> dQraw;  // M x D row-major staging
+    DevBuf<double> dQs;    // D x Mp
+    DevBuf<double> dV;     // Np x Mc
+    DevBuf<double> dMu;    // M x P
+    DevBuf<double> dS2;    // M
+    ArgmaxWs am;           // acquisition values (M), host means uploaded (M), argmax records
+    DevBuf<double> dFront; // lb_ehvi_argmax: the front sorted by f[0] (k x 2)
+    DevBuf<float> dKt;     // TF32 path: K*^T chunk (Mc x Np fp32)
+    DevBuf<float> dNorm2;
+    DevBuf<double> dBias;  // reduced-precision path: rounding-bias weight per candidate
+    DevBuf<int> dErr;
 };
 
 struct Extra {
     std::mutex qmutex;
     QueryWs ws;
-    double* dMisc = nullptr; // small scalars (loglik outputs, grad)
+    DevBuf<double> dMisc; // small scalars (loglik outputs, grad)
     cudaStream_t own = nullptr; // the handle's own stream (h->stream may point at a caller's stream)
     double lambda_host[LB_MAX_D * LB_MAX_LAMBDA] = {}; // host mirror of dLambda (lb_set_kernel compares against it)
     long long n_append = 0; // incremental updates actually taken (tests)
@@ -133,18 +129,11 @@ static inline lb_gp_full* full(const lb_gp* h) { return static_cast<lb_gp_full*>
 
 namespace {
 
+// handle workspaces grow with 256 bytes of slack
 template <typename T>
-int ensure(const lb_gp* h, T** p, size_t* cap, size_t bytes)
+int ensure(const lb_gp* h, DevBuf<T>& b, size_t bytes)
 {
-    if (*cap >= bytes && *p) return LB_OK;
-    lb_dfree_sync(h, *p); // kernels in flight may still use the old buffer
-    *p = nullptr;
-    *cap = 0;
-    const size_t want = bytes + 256;
-    int rc = lb_dalloc(h, p, want);
-    if (rc) return rc;
-    *cap = want;
-    return LB_OK;
+    return b.reserve(h, bytes, 256);
 }
 
 // Make *p private to h before h writes it (copy-on-write for buffers lb_clone shares).  preserve = keep the contents;
@@ -265,23 +254,15 @@ __global__ void append_row_kernel(double* __restrict__ L, int64_t np, int64_t n,
 }
 
 // callers synchronise the handle's stream first
-void free_ws(QueryWs& w)
-{
-    void* all[] = {w.dQraw, w.dQs, w.dV, w.dMu, w.dS2, w.dAcq, w.dBlkVal, w.dBlkIdx, w.dBest, w.dBestIdx, w.dMean, w.dKt, w.dNorm2,
-        w.dErr, w.dBias};
-    for (void* p : all) lb_pool_free(p);
-    w = QueryWs();
-}
-
 void free_model(lb_gp* h)
 {
-    void* all[] = {h->dX, h->dXs, h->dY, h->dL, h->dInvD, h->dAlpha, h->dLinv, h->dKinv, h->dFlags, h->dLinv32, h->dWork, h->dLinvW, h->dTrsvX};
-    h->dTrsvX = nullptr; h->trsvx_np = 0;
-    for (void* p : all) lb_pool_free(p); // shared buffers (lb_clone) only lose this handle's reference
-    h->dWork = nullptr; h->work_np = 0; h->dLinvW = nullptr; h->linvw_np = 0;
-    h->dLinv32 = nullptr; h->linv32_valid = false; h->linv32_rows = 0;
-    h->dX = h->dXs = h->dY = h->dL = h->dInvD = h->dAlpha = h->dLinv = h->dKinv = nullptr;
-    h->dFlags = nullptr;
+    void* shared[] = {h->dX, h->dXs, h->dY, h->dL, h->dInvD, h->dAlpha};
+    for (void* p : shared) lb_pool_free(p); // buffers lb_clone shares only lose this handle's reference
+    h->dX = h->dXs = h->dY = h->dL = h->dInvD = h->dAlpha = nullptr;
+    // the private buffers sized by Np
+    h->dLinv.release(); h->dKinv.release(); h->dFlags.release(); h->dLinv32.release(); h->dWork.release(); h->dLinvW.release();
+    h->dTrsvX.release();
+    h->linv32_valid = false;
     h->Np = 0;
 }
 
@@ -290,7 +271,8 @@ int alloc_model(lb_gp* h, int64_t Np, int D, int P)
     const int64_t T = Np / LB_TILE;
     LB_ALLOC(h, h->dX, sizeof(double) * D * Np);
     LB_ALLOC(h, h->dY, sizeof(double) * P * Np);
-    LB_ALLOC(h, h->dFlags, sizeof(int) * (T + 8));
+    int rc = h->dFlags.resize(h, sizeof(int) * (T + 8));
+    if (rc) return rc;
     h->Np = Np;
     return LB_OK; // Xs, L, invD, alpha: ensure_fit_buffers (a clone that refits never needs its source's copies)
 }
@@ -314,7 +296,7 @@ int ensure_fit_buffers(lb_gp* h)
 int check_info(lb_gp* h)
 {
     int info[2] = {0, 0};
-    LB_CUDA(cudaMemcpyAsync(info, h->dInfo, sizeof(info), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(info, h->dInfo.get(), sizeof(info), cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     if (info[1]) return LB_ERR_TIMEOUT;
     if (info[0] > 0) return info[0];
@@ -331,7 +313,7 @@ int upload_kernel_scaled(lb_gp* h)
 
 int lb_ensure_scratch(lb_gp* h, size_t bytes)
 {
-    return ensure(h, &h->dScratch, &h->scratch_bytes, bytes);
+    return ensure(h, h->dScratch, bytes);
 }
 
 extern "C" {
@@ -353,7 +335,7 @@ int lb_create(lb_gp** out, int device, int precision)
     lb_gp_full* h = new (std::nothrow) lb_gp_full();
     if (!h) return LB_ERR_ALLOC;
     h->device = device;
-    DeviceGuard guard(h);
+    DeviceGuard guard(device);
     if (!guard.ok) { delete h; return LB_ERR_CUDA; }
     h->precision = precision;
     Shell sh;
@@ -377,11 +359,11 @@ int lb_create(lb_gp** out, int device, int precision)
     h->own_stream = true;
     h->side = sh.side;
     for (int i = 0; i < LB_NEV; ++i) h->ev[i] = sh.ev[i];
-    if (lb_dalloc(h, &h->dInfo, 4 * sizeof(int)) || lb_dalloc(h, &h->ex.dMisc, (LB_MAX_HPARAMS + 16) * sizeof(double))) {
+    if (h->dInfo.resize(h, 4 * sizeof(int)) || h->ex.dMisc.resize(h, (LB_MAX_HPARAMS + 16) * sizeof(double))) {
         lb_destroy(h);
         return LB_ERR_ALLOC;
     }
-    cudaMemsetAsync(h->dInfo, 0, 4 * sizeof(int), h->stream);
+    cudaMemsetAsync(h->dInfo.get(), 0, 4 * sizeof(int), h->stream);
     h->kp.id = LB_K_SE_ARD;
     *out = h;
     return LB_OK;
@@ -391,17 +373,13 @@ int lb_destroy(lb_gp* hh)
 {
     if (!hh) return LB_OK;
     lb_gp_full* h = full(hh);
-    DeviceGuard guard(h);
+    DeviceGuard guard(h->device);
     cudaStreamSynchronize(h->stream);
     if (h->ex.own && h->ex.own != h->stream) cudaStreamSynchronize(h->ex.own);
     if (h->side) cudaStreamSynchronize(h->side);
     lb_profile_enable(h, 0);
     free_model(h);
-    free_ws(h->ex.ws);
-    lb_pool_free(h->dInfo);
-    lb_pool_free(h->dScratch);
-    lb_pool_free(h->dLambda);
-    lb_pool_free(h->ex.dMisc);
+    h->ex.ws = QueryWs{}; // the remaining private buffers go back with the handle (delete h)
     if (h->ex.hPoint) cudaFreeHost(h->ex.hPoint);
     for (cudaEvent_t e : h->ex.ev_eci) if (e) cudaEventDestroy(e);
     for (cudaStream_t* ps : {&h->aux, &h->aux2, &h->aux3})
@@ -443,9 +421,9 @@ int lb_sync(lb_gp* h)
     lb_gp_full* f = full(h);
     if (f->ex.ws.dErr) {
         int herr = 0;
-        LB_CUDA(cudaMemcpy(&herr, f->ex.ws.dErr, sizeof(int), cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(&herr, f->ex.ws.dErr.get(), sizeof(int), cudaMemcpyDeviceToHost));
         if (herr) {
-            LB_CUDA(cudaMemset(f->ex.ws.dErr, 0, sizeof(int)));
+            LB_CUDA(cudaMemset(f->ex.ws.dErr.get(), 0, sizeof(int)));
             return LB_ERR_TIMEOUT;
         }
     }
@@ -476,16 +454,17 @@ static int set_data_common(lb_gp* h, int64_t N, int D, int P, const double* X, c
     h->N = N; h->D = D; h->P = P;
     h->kp.Draw = D;
     h->kp.D = D + h->kp.klam;
-    h->fitted = false; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = false;
+    lb_factor_changed(h);
     const double* dXr = X;
     const double* dYr = Y;
     if (!dev && N > 0) {
         int rc = lb_ensure_scratch(h, sizeof(double) * (size_t)N * (D + P));
         if (rc) return rc;
-        LB_CUDA(cudaMemcpyAsync(h->dScratch, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
-        LB_CUDA(cudaMemcpyAsync(h->dScratch + N * D, Y, sizeof(double) * N * P, cudaMemcpyHostToDevice, h->stream));
-        dXr = h->dScratch;
-        dYr = h->dScratch + N * D;
+        LB_CUDA(cudaMemcpyAsync(h->dScratch.get(), X, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
+        LB_CUDA(cudaMemcpyAsync(h->dScratch.get() + N * D, Y, sizeof(double) * N * P, cudaMemcpyHostToDevice, h->stream));
+        dXr = h->dScratch.get();
+        dYr = h->dScratch.get() + N * D;
     }
     dim3 g1((unsigned)((Np + 255) / 256), (unsigned)D), g2((unsigned)((Np + 255) / 256), (unsigned)P);
     pack_soa_kernel<<<g1, 256, 0, h->stream>>>(dXr, N, D, h->dX, Np, h->kp, 0);
@@ -511,12 +490,13 @@ int lb_dchol_set_points(lb_gp* h, int64_t N, int D, const double* X)
     h->N = N; h->D = D; h->P = 0;
     h->kp.Draw = D;
     h->kp.D = D + h->kp.klam;
-    h->fitted = false; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = false;
+    lb_factor_changed(h);
     int rc = lb_ensure_scratch(h, sizeof(double) * (size_t)N * D);
     if (rc) return rc;
-    LB_CUDA(cudaMemcpyAsync(h->dScratch, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
+    LB_CUDA(cudaMemcpyAsync(h->dScratch.get(), X, sizeof(double) * N * D, cudaMemcpyHostToDevice, h->stream));
     dim3 g1((unsigned)((Np + 255) / 256), (unsigned)D);
-    pack_soa_kernel<<<g1, 256, 0, h->stream>>>(h->dScratch, N, D, h->dX, Np, h->kp, 0);
+    pack_soa_kernel<<<g1, 256, 0, h->stream>>>(h->dScratch.get(), N, D, h->dX, Np, h->kp, 0);
     h->launches++;
     LB_CUDA(cudaStreamSynchronize(h->stream));
     LB_CUDA(cudaGetLastError());
@@ -563,13 +543,14 @@ int lb_set_kernel(lb_gp* h, int kernel_id, const double* p, int n_hparams, doubl
         kp.sf2 = std::exp(2.0 * p[n_hparams - 1]);
         kp.l = 1.0;
         if (klam > 0) { // _A(i, j) = p((j + 1) * D + i): already column-major
-            if (!h->dLambda) LB_ALLOC(h, h->dLambda, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA);
+            int rc = h->dLambda.reserve(h, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA);
+            if (rc) return rc;
             double* lh = full(h)->ex.lambda_host;
             lambda_same = (old.klam == klam) && std::memcmp(lh, p + h->D, sizeof(double) * h->D * klam) == 0;
             std::memcpy(lh, p + h->D, sizeof(double) * h->D * klam);
-            LB_CUDA(cudaMemcpyAsync(h->dLambda, p + h->D, sizeof(double) * h->D * klam, cudaMemcpyHostToDevice, h->stream));
+            LB_CUDA(cudaMemcpyAsync(h->dLambda.get(), p + h->D, sizeof(double) * h->D * klam, cudaMemcpyHostToDevice, h->stream));
             LB_CUDA(cudaStreamSynchronize(h->stream));
-            kp.lambda = h->dLambda;
+            kp.lambda = h->dLambda.get();
         }
     }
     else { // matern_five_halves.hpp:97-102 and siblings
@@ -588,7 +569,10 @@ int lb_set_kernel(lb_gp* h, int kernel_id, const double* p, int n_hparams, doubl
         && old.sf2 == kp.sf2 && old.l == kp.l && old.noise == kp.noise && old.c1 == kp.c1 && old.c2 == kp.c2;
     if (same && kernel_id == LB_K_SE_ARD)
         for (int d = 0; d < h->D; ++d) same = same && (old.inv_ell[d] == kp.inv_ell[d]);
-    if (!same) { h->fitted = false; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false; }
+    if (!same) {
+        h->fitted = false;
+        lb_factor_changed(h);
+    }
     return LB_OK;
 }
 
@@ -603,7 +587,8 @@ int lb_fit(lb_gp* h)
     if ((rc = lb_launch_scale_x(h))) return rc;
     if ((rc = lb_launch_kbuild(h, h->dL))) return rc;
     if ((rc = lb_launch_potrf(h))) return rc;
-    h->fitted = true; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = true;
+    lb_factor_changed(h);
     if ((rc = lb_launch_solve_alpha(h))) return rc;
     return check_info(h);
 }
@@ -618,7 +603,8 @@ int lb_fit_async(lb_gp* h) // same as lb_fit without the final host sync / info 
     if ((rc = lb_launch_scale_x(h))) return rc;
     if ((rc = lb_launch_kbuild(h, h->dL))) return rc;
     if ((rc = lb_launch_potrf(h))) return rc;
-    h->fitted = true; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = true;
+    lb_factor_changed(h);
     return lb_launch_solve_alpha(h);
 }
 
@@ -682,11 +668,12 @@ int lb_load_factor(lb_gp* h, const double* L_colmajor, const double* alpha_colma
     identity_pad_kernel<<<1024, 256, 0, h->stream>>>(h->dL, Np, N);
     LB_CUDA(cudaMemsetAsync(h->dAlpha, 0, sizeof(double) * Np * h->P, h->stream));
     LB_CUDA(cudaMemcpy2DAsync(h->dAlpha, Np * 8, alpha_colmajor, N * 8, N * 8, h->P, cudaMemcpyHostToDevice, h->stream));
-    LB_CUDA(cudaMemsetAsync(h->dInfo, 0, 2 * sizeof(int), h->stream));
+    LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), h->stream));
     h->launches++;
     for (int k = 0; k < T; ++k)
         if ((rc = lb_launch_potf2_block(h, k, 0))) return rc;
-    h->fitted = true; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = true;
+    lb_factor_changed(h);
     return check_info(h);
 }
 
@@ -699,9 +686,9 @@ int lb_refit_alpha(lb_gp* h, const double* Y)
     if (rc) return rc;
     if ((rc = make_unique(h, &h->dY, sizeof(double) * h->P * h->Np, false))) return rc;
     if ((rc = make_unique(h, &h->dAlpha, sizeof(double) * h->P * h->Np, false))) return rc;
-    LB_CUDA(cudaMemcpyAsync(h->dScratch, Y, sizeof(double) * h->N * h->P, cudaMemcpyHostToDevice, h->stream));
+    LB_CUDA(cudaMemcpyAsync(h->dScratch.get(), Y, sizeof(double) * h->N * h->P, cudaMemcpyHostToDevice, h->stream));
     dim3 g2((unsigned)((h->Np + 255) / 256), (unsigned)h->P);
-    pad_cols_kernel<<<g2, 256, 0, h->stream>>>(h->dScratch, h->N, h->P, h->dY, h->Np);
+    pad_cols_kernel<<<g2, 256, 0, h->stream>>>(h->dScratch.get(), h->N, h->P, h->dY, h->Np);
     h->launches++;
     if ((rc = lb_launch_solve_alpha(h))) return rc;
     return check_info(h);
@@ -718,7 +705,7 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
     if (n + 1 > h->Np) { // grow by one tile, keep the factor
         const int64_t oldNp = h->Np, newNp = oldNp + LB_TILE;
         const int64_t oldT = oldNp / LB_TILE, newT = newNp / LB_TILE;
-        double *nX, *nXs, *nY, *nA, *nL, *nI; int* nF;
+        double *nX, *nXs, *nY, *nA, *nL, *nI;
         LB_CUDA(cudaStreamSynchronize(h->stream));
         LB_ALLOC(h, nX, sizeof(double) * D * newNp);
         LB_ALLOC(h, nXs, sizeof(double) * (D + LB_MAX_LAMBDA) * newNp);
@@ -726,7 +713,8 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
         LB_ALLOC(h, nA, sizeof(double) * P * newNp);
         LB_ALLOC(h, nL, sizeof(double) * newNp * newNp);
         LB_ALLOC(h, nI, sizeof(double) * newT * LB_TILE * LB_TILE);
-        LB_ALLOC(h, nF, sizeof(int) * (newT + 8));
+        int rc = h->dFlags.resize(h, sizeof(int) * (newT + 8));
+        if (rc) return rc;
         LB_CUDA(cudaMemsetAsync(nX, 0, sizeof(double) * D * newNp, h->stream));
         LB_CUDA(cudaMemsetAsync(nY, 0, sizeof(double) * P * newNp, h->stream));
         LB_CUDA(cudaMemcpy2DAsync(nX, newNp * 8, h->dX, oldNp * 8, oldNp * 8, D, cudaMemcpyDeviceToDevice, h->stream));
@@ -737,9 +725,8 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
         h->launches += 2;
         LB_CUDA(cudaStreamSynchronize(h->stream));
         lb_pool_free(h->dX); lb_pool_free(h->dXs); lb_pool_free(h->dY); lb_pool_free(h->dAlpha); lb_pool_free(h->dL); lb_pool_free(h->dInvD);
-        lb_pool_free(h->dFlags); lb_pool_free(h->dLinv); lb_pool_free(h->dKinv);
-        h->dX = nX; h->dXs = nXs; h->dY = nY; h->dAlpha = nA; h->dL = nL; h->dInvD = nI; h->dFlags = nF;
-        h->dLinv = h->dKinv = nullptr;
+        h->dX = nX; h->dXs = nXs; h->dY = nY; h->dAlpha = nA; h->dL = nL; h->dInvD = nI;
+        h->dLinv.release(); h->dKinv.release();
         h->Np = newNp;
     }
     const int64_t Np = h->Np;
@@ -755,7 +742,7 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
         if ((rc = make_unique(h, &h->dAlpha, sizeof(double) * P * Np, false))) return rc;
     }
     full(h)->ex.n_append++;
-    double* dYs = h->dScratch;
+    double* dYs = h->dScratch.get();
     double* dx = dYs + (n + 1) * P;
     double* dk = dx + D;
     LB_CUDA(cudaMemcpyAsync(dYs, Yall, sizeof(double) * (n + 1) * P, cudaMemcpyHostToDevice, h->stream));
@@ -772,10 +759,10 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
     h->launches++;
     if ((rc = lb_launch_trsv(h, dk, 1, true))) return rc;
     const double knn = h->kp.sf2 + h->kp.noise + 1e-8; // kernel(x,x) with i == j, kernel.hpp:83
-    append_row_kernel<<<1, 256, 0, h->stream>>>(h->dL, Np, n, dk, knn, h->dInfo);
+    append_row_kernel<<<1, 256, 0, h->stream>>>(h->dL, Np, n, dk, knn, h->dInfo.get());
     h->launches++;
     if ((rc = lb_launch_potf2_block(h, (int)(n / LB_TILE), 0))) return rc;
-    h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    lb_factor_changed(h);
     if ((rc = lb_launch_solve_alpha(h))) return rc;
     return check_info(h);
 }
@@ -804,7 +791,7 @@ extern "C" int lb_debug_set_query_panel_min(long long m)
     return LB_OK;
 }
 
-// Fills h's query workspace, w.dMu (M x P, k^T alpha) and w.dS2 (M), for M candidates on h->stream: the prior, the
+// Fills h's query workspace, w.dMu.get() (M x P, k^T alpha) and w.dS2.get() (M), for M candidates on h->stream: the prior, the
 // reduced-precision path, the panel path for large batches, the fused slab path or the multi-launch path.  Xq is row-major
 // M x D, a device pointer when xq_dev.  The caller holds h->ex.qmutex and has checked the handle's state.  A reduced-precision
 // fill leaves its timeout flag in w.dErr (query_timed_out).
@@ -815,21 +802,21 @@ static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
     const int D = h->D, De = h->kp.D, P = h->P > 0 ? h->P : 1; // raw / staged input dimension
     const int64_t Mp = (M + LB_TILE - 1) / LB_TILE * LB_TILE;
     int rc;
-    if ((rc = ensure(h, &w.dMu, &w.mu_bytes, sizeof(double) * M * P))) return rc;
-    if ((rc = ensure(h, &w.dS2, &w.s2_bytes, sizeof(double) * M))) return rc;
+    if ((rc = ensure(h, w.dMu, sizeof(double) * M * P))) return rc;
+    if ((rc = ensure(h, w.dS2, sizeof(double) * M))) return rc;
     const bool prior = (h->N == 0 || !h->fitted);
     if (prior && h->N != 0) return LB_ERR_STATE;
     if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma2 = k(v,v) + noise
-        LB_CUDA(cudaMemsetAsync(w.dMu, 0, sizeof(double) * M * P, st));
-        fill_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w.dS2, M, h->kp.sf2 + h->kp.noise);
+        LB_CUDA(cudaMemsetAsync(w.dMu.get(), 0, sizeof(double) * M * P, st));
+        fill_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w.dS2.get(), M, h->kp.sf2 + h->kp.noise);
         h->launches++;
     }
     else {
         const double* dQraw = Xq;
         if (!xq_dev) {
-            if ((rc = ensure(h, &w.dQraw, &w.qraw_bytes, sizeof(double) * M * D))) return rc;
-            LB_CUDA(cudaMemcpyAsync(w.dQraw, Xq, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
-            dQraw = w.dQraw;
+            if ((rc = ensure(h, w.dQraw, sizeof(double) * M * D))) return rc;
+            LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
+            dQraw = w.dQraw.get();
         }
         if (h->precision == LB_PREC_TF32 || h->precision == LB_PREC_FP16 || h->precision == LB_PREC_FP16X3) {
             // reduced-precision variance on wgmma (tf32_query.cu); mu is accumulated in fp64 from the fp64 kernel values
@@ -842,22 +829,22 @@ static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
             const int64_t cap = std::max<int64_t>(CH, ((int64_t)4 << 30) / (4 * h->Np) / CH * CH);
             int64_t Mc = (cap >= wave) ? cap / wave * wave : cap;
             Mc = std::min((M + CH - 1) / CH * CH, Mc);
-            if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * Mc))) return rc;
-            if ((rc = ensure(h, &w.dKt, &w.kt_bytes, sizeof(float) * (size_t)Mc * h->Np))) return rc;
-            if ((rc = ensure(h, &w.dNorm2, &w.norm2_bytes, sizeof(double) * (size_t)Mc))) return rc; // Mc floats (split mode: Mc doubles)
-            if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * (size_t)(P + 1) * (h->Np / LB_TILE) * Mc))) return rc; // mean (+ bias) partials per training tile
-            if ((rc = ensure(h, &w.dBias, &w.bias_bytes, sizeof(double) * Mc))) return rc;
-            double* dBiasUse = (h->precision == LB_PREC_FP16X3) ? nullptr : w.dBias; // 22-bit operands: no rounding-bias term
-            if (!w.dErr) LB_ALLOC(h, w.dErr, sizeof(int));
-            LB_CUDA(cudaMemsetAsync(w.dErr, 0, sizeof(int), st));
+            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
+            if ((rc = ensure(h, w.dKt, sizeof(float) * (size_t)Mc * h->Np))) return rc;
+            if ((rc = ensure(h, w.dNorm2, sizeof(double) * (size_t)Mc))) return rc; // Mc floats (split mode: Mc doubles)
+            if ((rc = ensure(h, w.dV, sizeof(double) * (size_t)(P + 1) * (h->Np / LB_TILE) * Mc))) return rc; // mean (+ bias) partials per training tile
+            if ((rc = ensure(h, w.dBias, sizeof(double) * Mc))) return rc;
+            double* dBiasUse = (h->precision == LB_PREC_FP16X3) ? nullptr : w.dBias.get(); // 22-bit operands: no rounding-bias term
+            if ((rc = w.dErr.reserve(h, sizeof(int)))) return rc;
+            LB_CUDA(cudaMemsetAsync(w.dErr.get(), 0, sizeof(int), st));
             for (int64_t m0 = 0; m0 < M; m0 += Mc) {
                 const int64_t mc = std::min(Mc, M - m0);
                 const int64_t mcp = (mc + CH - 1) / CH * CH;
                 dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs, mcp, h->kp, 1);
+                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
                 h->launches++;
-                if ((rc = lb_launch_kstar_tf32(h, st, mc, w.dQs, mcp, w.dKt, w.dV, w.dMu + m0 * P, dBiasUse, &h->launches))) return rc;
-                if ((rc = lb_launch_sigma_tf32(h, st, mc, mcp, w.dKt, w.dNorm2, w.dErr, dBiasUse, w.dS2 + m0, &h->launches))) return rc;
+                if ((rc = lb_launch_kstar_tf32(h, st, mc, w.dQs.get(), mcp, w.dKt.get(), w.dV.get(), w.dMu.get() + m0 * P, dBiasUse, &h->launches))) return rc;
+                if ((rc = lb_launch_sigma_tf32(h, st, mc, mcp, w.dKt.get(), w.dNorm2.get(), w.dErr.get(), dBiasUse, w.dS2.get() + m0, &h->launches))) return rc;
             }
         }
         else if (M >= query_panel_min() && !h->force_unfused) {
@@ -865,15 +852,15 @@ static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
             // candidate chunks bounded so that V (Np x Mc) stays <= ~6 GiB
             const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)6 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
             const int64_t Mc = std::min(Mp, maxcols);
-            if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * Mc))) return rc;
-            if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_query_panel_scratch_doubles(h, Mc)))) return rc;
+            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
+            if ((rc = ensure(h, w.dV, sizeof(double) * lb_query_panel_scratch_doubles(h, Mc)))) return rc;
             for (int64_t m0 = 0; m0 < M; m0 += Mc) {
                 const int64_t mc = std::min(Mc, M - m0);
                 const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
                 dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs, mcp, h->kp, 1);
+                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
                 h->launches++;
-                if ((rc = lb_launch_query_panel(h, st, mc, w.dQs, mcp, w.dV, w.dMu + m0 * P, w.dS2 + m0, &h->launches))) return rc;
+                if ((rc = lb_launch_query_panel(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, &h->launches))) return rc;
             }
         }
         else if (lb_query_fused_supported(h) && !h->force_unfused) {
@@ -882,48 +869,29 @@ static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
             LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
             const int64_t ntiles = (M + 7) / 8;
             const int grid = (int)std::min<int64_t>(sms, ntiles);
-            if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * Mp))) return rc;
-            if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_query_fused_scratch_doubles(h, grid)))) return rc;
+            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mp))) return rc;
+            if ((rc = ensure(h, w.dV, sizeof(double) * lb_query_fused_scratch_doubles(h, grid)))) return rc;
             dim3 g1((unsigned)((Mp + 255) / 256), (unsigned)De);
-            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw, M, D, w.dQs, Mp, h->kp, 1);
+            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw, M, D, w.dQs.get(), Mp, h->kp, 1);
             h->launches++;
-            if ((rc = lb_launch_query_fused(h, st, M, w.dQs, Mp, w.dV, grid, w.dMu, w.dS2, &h->launches))) return rc;
+            if ((rc = lb_launch_query_fused(h, st, M, w.dQs.get(), Mp, w.dV.get(), grid, w.dMu.get(), w.dS2.get(), &h->launches))) return rc;
         }
         else {
         // candidate chunks bounded so that V (Np x Mc) stays <= ~4 GiB
         int64_t Mc = Mp;
         const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)4 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
         if (Mc > maxcols) Mc = maxcols;
-        if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * Mc))) return rc;
-        if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * h->Np * Mc))) return rc;
+        if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
+        if ((rc = ensure(h, w.dV, sizeof(double) * h->Np * Mc))) return rc;
         for (int64_t m0 = 0; m0 < M; m0 += Mc) {
             const int64_t mc = std::min(Mc, M - m0);
             const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
             dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs, mcp, h->kp, 1);
+            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
             h->launches++;
-            if ((rc = lb_launch_query(h, st, mc, w.dQs, mcp, w.dV, w.dMu + m0 * P, w.dS2 + m0, &h->launches))) return rc;
+            if ((rc = lb_launch_query(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, &h->launches))) return rc;
         }
         }
-    }
-    return LB_OK;
-}
-
-// per-block (value, index) records of an M-candidate argmax and the final record, in h's query workspace (caller holds qmutex)
-static int ensure_argmax_bufs(lb_gp_full* h, int64_t M)
-{
-    QueryWs& w = h->ex.ws;
-    const int nblk = (int)((M + 255) / 256);
-    if ((size_t)nblk > w.blk_cap) {
-        lb_dfree_sync(h, w.dBlkVal); lb_dfree_sync(h, w.dBlkIdx);
-        w.dBlkVal = nullptr; w.dBlkIdx = nullptr; w.blk_cap = 0;
-        LB_ALLOC(h, w.dBlkVal, sizeof(double) * nblk);
-        LB_ALLOC(h, w.dBlkIdx, sizeof(long long) * nblk);
-        w.blk_cap = nblk;
-    }
-    if (!w.dBest) {
-        LB_ALLOC(h, w.dBest, sizeof(double));
-        LB_ALLOC(h, w.dBestIdx, sizeof(long long));
     }
     return LB_OK;
 }
@@ -933,11 +901,11 @@ static int mean_on_device(lb_gp_full* h, cudaStream_t st, const double* mean_at_
 {
     *out = mean_at_q;
     if (!mean_at_q || dev) return LB_OK;
-    QueryWs& w = h->ex.ws;
-    int rc = ensure(h, &w.dMean, &w.mean_bytes, sizeof(double) * M);
+    DevBuf<double>& mean = h->ex.ws.am.mean;
+    int rc = ensure(h, mean, sizeof(double) * M);
     if (rc) return rc;
-    LB_CUDA(cudaMemcpyAsync(w.dMean, mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
-    *out = w.dMean;
+    LB_CUDA(cudaMemcpyAsync(mean.get(), mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
+    *out = mean.get();
     return LB_OK;
 }
 
@@ -946,7 +914,7 @@ static int query_timed_out(lb_gp_full* h)
 {
     if (h->precision == LB_PREC_FP64 || h->N == 0 || !h->ex.ws.dErr) return LB_OK; // N == 0: the prior, no flag written
     int herr = 0;
-    LB_CUDA(cudaMemcpyAsync(&herr, h->ex.ws.dErr, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(&herr, h->ex.ws.dErr.get(), sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     return herr ? LB_ERR_TIMEOUT : LB_OK;
 }
@@ -977,9 +945,9 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
             LB_CUDA(cudaHostGetDevicePointer((void**)&ex.dPoint, ex.hPoint, 0));
             ex.point_cap = P + 1 + 7;
         }
-        if ((rc = ensure(h, &w.dQs, &w.qs_bytes, sizeof(double) * De * LB_TILE))) return rc;
-        if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_query_fused_scratch_doubles(h, 1)))) return rc;
-        if ((rc = lb_launch_query_point(h, st, Xq, w.dQs, w.dV, ex.dPoint, &h->launches))) return rc;
+        if ((rc = ensure(h, w.dQs, sizeof(double) * De * LB_TILE))) return rc;
+        if ((rc = ensure(h, w.dV, sizeof(double) * lb_query_fused_scratch_doubles(h, 1)))) return rc;
+        if ((rc = lb_launch_query_point(h, st, Xq, w.dQs.get(), w.dV.get(), ex.dPoint, &h->launches))) return rc;
         LB_CUDA(cudaStreamSynchronize(st));
         if (mu_out) std::memcpy(mu_out, ex.hPoint, sizeof(double) * P);
         if (s2_out) *s2_out = ex.hPoint[P];
@@ -988,38 +956,31 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
     if ((rc = query_fill(h, M, Xq, xq_dev))) return rc;
     if (!out_dev && (rc = query_timed_out(h))) return rc;
     if (with_acq) {
-        if ((rc = ensure_argmax_bufs(h, M))) return rc;
+        if ((rc = w.am.reserve(h->device, st, M))) return rc;
         const double* dMean = nullptr;
         if ((rc = mean_on_device(h, st, mean_at_q, M, out_dev, &dMean))) return rc;
         double* dAcq = nullptr;
         if (acq_out) {
             if (out_dev) dAcq = acq_out;
             else {
-                if ((rc = ensure(h, &w.dAcq, &w.acq_bytes, sizeof(double) * M))) return rc;
-                dAcq = w.dAcq;
+                if ((rc = ensure(h, w.am.vals, sizeof(double) * M))) return rc;
+                dAcq = w.am.vals.get();
             }
         }
-        double* dBV = out_dev ? best_val : w.dBest;
-        long long* dBI = out_dev ? (long long*)best_idx : w.dBestIdx;
+        double* dBV = out_dev ? best_val : w.am.best_val.get();
+        long long* dBI = out_dev ? (long long*)best_idx : w.am.best_idx.get();
         const double p0 = acq_params ? acq_params[0] : 0.0;
         const double p1 = (acq_params && acq_id == LB_ACQ_EI) ? acq_params[1] : 0.0;
-        if ((rc = lb_launch_acq_full(st, acq_id, p0, p1, M, w.dMu, P, dMean, mean_const, w.dS2, dAcq, w.dBlkVal, w.dBlkIdx,
-                 dBV, dBI, &h->launches)))
+        if ((rc = lb_launch_acq_full(st, acq_id, p0, p1, M, w.dMu.get(), P, dMean, mean_const, w.dS2.get(), dAcq, w.am.blk_val.get(),
+                 w.am.blk_idx.get(), dBV, dBI, &h->launches)))
             return rc;
-        if (!out_dev) {
-            if (acq_out) LB_CUDA(cudaMemcpyAsync(acq_out, w.dAcq, sizeof(double) * M, cudaMemcpyDeviceToHost, st));
-            long long bi = 0;
-            LB_CUDA(cudaMemcpyAsync(best_val, w.dBest, sizeof(double), cudaMemcpyDeviceToHost, st));
-            LB_CUDA(cudaMemcpyAsync(&bi, w.dBestIdx, sizeof(long long), cudaMemcpyDeviceToHost, st));
-            LB_CUDA(cudaStreamSynchronize(st));
-            *best_idx = (int64_t)bi;
-        }
+        if (!out_dev && (rc = w.am.read_best(st, best_val, best_idx, acq_out, M))) return rc;
     }
     if (mu_out) {
-        LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu, sizeof(double) * M * P, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu.get(), sizeof(double) * M * P, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     }
     if (s2_out) {
-        LB_CUDA(cudaMemcpyAsync(s2_out, w.dS2, sizeof(double) * M, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(s2_out, w.dS2.get(), sizeof(double) * M, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     }
     if (!out_dev) LB_CUDA(cudaStreamSynchronize(st));
     LB_CUDA(cudaGetLastError());
@@ -1076,9 +1037,9 @@ static int pair_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq
     if (c && (rc = ensure_eci_events(c))) return rc;
     const double* dXq = Xq;
     if (!dev) { // one upload, read by both queries
-        if ((rc = ensure(o, &w.dQraw, &w.qraw_bytes, sizeof(double) * M * o->D))) return rc;
-        LB_CUDA(cudaMemcpyAsync(w.dQraw, Xq, sizeof(double) * M * o->D, cudaMemcpyHostToDevice, st));
-        dXq = w.dQraw;
+        if ((rc = ensure(o, w.dQraw, sizeof(double) * M * o->D))) return rc;
+        LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * o->D, cudaMemcpyHostToDevice, st));
+        dXq = w.dQraw.get();
     }
     if (c) {
         LB_CUDA(cudaEventRecord(o->ex.ev_eci[0], st));
@@ -1096,32 +1057,25 @@ static int pair_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq
         if ((rc = query_timed_out(o))) return rc;
         if (c && (rc = query_timed_out(c))) return rc;
     }
-    if ((rc = ensure_argmax_bufs(o, M))) return rc;
+    if ((rc = w.am.reserve(o->device, st, M))) return rc;
     const double* dMeanO = nullptr;
     const double* dMeanC = nullptr;
     if ((rc = mean_on_device(o, st, o_mean_at_q, M, dev, &dMeanO))) return rc;
     if (c && (rc = mean_on_device(c, st, c_mean_at_q, M, dev, &dMeanC))) return rc;
     double* dAcq = acq_out;
     if ((acq_out && !dev) || (!acq_out && acq_ws)) {
-        if ((rc = ensure(o, &w.dAcq, &w.acq_bytes, sizeof(double) * M))) return rc;
-        dAcq = w.dAcq;
+        if ((rc = ensure(o, w.am.vals, sizeof(double) * M))) return rc;
+        dAcq = w.am.vals.get();
     }
-    double* dBV = dev ? best_val : w.dBest;
-    long long* dBI = dev ? (long long*)best_idx : w.dBestIdx;
+    double* dBV = dev ? best_val : w.am.best_val.get();
+    long long* dBI = dev ? (long long*)best_idx : w.am.best_idx.get();
     rc = epilogue(dMeanO, dMeanC, dAcq, dBV, dBI);
     if (c) { // a later call on c must not overwrite the buffers the epilogue reads before it has run
         LB_CUDA(cudaEventRecord(o->ex.ev_eci[1], st));
         LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[1], 0));
     }
     if (rc) return rc;
-    if (!dev) {
-        if (acq_out) LB_CUDA(cudaMemcpyAsync(acq_out, w.dAcq, sizeof(double) * M, cudaMemcpyDeviceToHost, st));
-        long long bi = 0;
-        LB_CUDA(cudaMemcpyAsync(best_val, w.dBest, sizeof(double), cudaMemcpyDeviceToHost, st));
-        LB_CUDA(cudaMemcpyAsync(&bi, w.dBestIdx, sizeof(long long), cudaMemcpyDeviceToHost, st));
-        LB_CUDA(cudaStreamSynchronize(st));
-        *best_idx = (int64_t)bi;
-    }
+    if (!dev && (rc = w.am.read_best(st, best_val, best_idx, acq_out, M))) return rc;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
 }
@@ -1155,9 +1109,9 @@ static int eci_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double jitter,
     return pair_locked(o, cu, M, Xq, dev, obj_mean_at_q, con_mean_at_q, acq_out, best_val, best_idx, false,
         [&](const double* dMeanObj, const double* dMeanCon, double* dAcq, double* dBV, long long* dBI) {
             const int Po = o->P > 0 ? o->P : 1, Pc = (use_con && c->P > 0) ? c->P : 1;
-            return lb_launch_eci_full(st, f_max, jitter, M, o->ex.ws.dMu, Po, dMeanObj, obj_mean_const, o->ex.ws.dS2,
-                use_con ? c->ex.ws.dMu : nullptr, Pc, dMeanCon, con_mean_const, use_con ? c->ex.ws.dS2 : nullptr, dAcq,
-                o->ex.ws.dBlkVal, o->ex.ws.dBlkIdx, dBV, dBI, &o->launches);
+            return lb_launch_eci_full(st, f_max, jitter, M, o->ex.ws.dMu.get(), Po, dMeanObj, obj_mean_const, o->ex.ws.dS2.get(),
+                use_con ? c->ex.ws.dMu.get() : nullptr, Pc, dMeanCon, con_mean_const, use_con ? c->ex.ws.dS2.get() : nullptr, dAcq,
+                o->ex.ws.am.blk_val.get(), o->ex.ws.am.blk_idx.get(), dBV, dBI, &o->launches);
         });
 }
 
@@ -1228,14 +1182,14 @@ static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point
             QueryWs& w = a->ex.ws;
             int rc;
             if (k > 0) {
-                if ((rc = ensure(a, &w.dFront, &w.front_bytes, sizeof(double) * 2 * k))) return rc;
-                LB_CUDA(cudaMemcpyAsync(w.dFront, sorted.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
+                if ((rc = ensure(a, w.dFront, sizeof(double) * 2 * k))) return rc;
+                LB_CUDA(cudaMemcpyAsync(w.dFront.get(), sorted.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
             }
             const int Pa = a->P > 0 ? a->P : 1, Pb = b->P > 0 ? b->P : 1;
-            if ((rc = lb_launch_ehvi(st, ref_point[0], ref_point[1], k, w.dFront, M, w.dMu, Pa, dMean0, mean0_const, w.dS2, b->ex.ws.dMu, Pb,
-                     dMean1, mean1_const, b->ex.ws.dS2, dAcq, &a->launches)))
+            if ((rc = lb_launch_ehvi(st, ref_point[0], ref_point[1], k, w.dFront.get(), M, w.dMu.get(), Pa, dMean0, mean0_const, w.dS2.get(), b->ex.ws.dMu.get(), Pb,
+                     dMean1, mean1_const, b->ex.ws.dS2.get(), dAcq, &a->launches)))
                 return rc;
-            return lb_launch_values_argmax(st, M, dAcq, w.dBlkVal, w.dBlkIdx, dBV, dBI, &a->launches);
+            return lb_launch_values_argmax(st, M, dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &a->launches);
         });
 }
 
@@ -1270,26 +1224,28 @@ static int pareto_common(const lb_gp* hc, int64_t n, int K, const double* objs, 
     std::vector<double> hobj;
     std::vector<int> keep((size_t)n);
     int herr = 0;
-    double* dObj = nullptr;
-    int* dKeep = nullptr;
-    int rc = LB_OK;
-    cudaError_t e = cudaSuccess;
-    if (dev) hobj.resize((size_t)(n * K));
-    if (!(rc = lb_dalloc(h, &dKeep, sizeof(int) * (n + 1))) && (dev || !(rc = lb_dalloc(h, &dObj, sizeof(double) * n * K)))) {
-        const double* dO = dev ? objs : dObj;
-        if (!dev) e = cudaMemcpyAsync(dObj, objs, sizeof(double) * n * K, cudaMemcpyHostToDevice, st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(dKeep + n, 0, sizeof(int), st);
-        if (e == cudaSuccess) rc = lb_launch_pareto(st, n, K, dO, dKeep, dKeep + n, &h->launches);
-        if (e == cudaSuccess && !rc) e = cudaMemcpyAsync(keep.data(), dKeep, sizeof(int) * n, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && !rc) e = cudaMemcpyAsync(&herr, dKeep + n, sizeof(int), cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess && !rc && dev) e = cudaMemcpyAsync(hobj.data(), objs, sizeof(double) * n * K, cudaMemcpyDeviceToHost, st);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (!rc && e != cudaSuccess) { lb_set_last_cuda_error(e, __FILE__, __LINE__); rc = LB_ERR_CUDA; }
+    int rc;
+    {
+        StreamTemps tmp(h->device, st);
+        int* dKeep = nullptr;
+        const double* dO = objs;
+        if ((rc = tmp.alloc(sizeof(int) * (n + 1), &dKeep))) return rc;
+        if (!dev) {
+            double* dObj = nullptr;
+            if ((rc = tmp.alloc(sizeof(double) * n * K, &dObj))) return rc;
+            LB_CUDA(cudaMemcpyAsync(dObj, objs, sizeof(double) * n * K, cudaMemcpyHostToDevice, st));
+            dO = dObj;
+        }
+        LB_CUDA(cudaMemsetAsync(dKeep + n, 0, sizeof(int), st));
+        if ((rc = lb_launch_pareto(st, n, K, dO, dKeep, dKeep + n, &h->launches))) return rc;
+        LB_CUDA(cudaMemcpyAsync(keep.data(), dKeep, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(&herr, dKeep + n, sizeof(int), cudaMemcpyDeviceToHost, st));
+        if (dev) {
+            hobj.resize((size_t)(n * K));
+            LB_CUDA(cudaMemcpyAsync(hobj.data(), objs, sizeof(double) * n * K, cudaMemcpyDeviceToHost, st));
+        }
+        LB_CUDA(cudaStreamSynchronize(st));
     }
-    cudaStreamSynchronize(st);
-    lb_pool_free(dObj);
-    lb_pool_free(dKeep);
-    if (rc) return rc;
     if (herr) return LB_ERR_ARG;
     const double* O = dev ? hobj.data() : objs;
     std::vector<int64_t> front;
@@ -1344,26 +1300,22 @@ static int sparsify_common(const lb_gp* hc, int64_t N, int D, const double* X, i
         return LB_OK;
     }
     if (dev) return lb_run_sparsify(h, st, N, D, X, max_points, (long long*)kept, n_kept, (long long*)removed, removed_score, &h->launches);
+    StreamTemps tmp(h->device, st);
     double* dX = nullptr;
     long long *dKept = nullptr, *dRm = nullptr;
     double* dRs = nullptr;
-    int rc = LB_OK;
-    if (!(rc = lb_dalloc(h, &dX, sizeof(double) * N * D)) && !(rc = lb_dalloc(h, &dKept, sizeof(long long) * N)) &&
-        (!removed || !(rc = lb_dalloc(h, &dRm, sizeof(long long) * N))) && (!removed_score || !(rc = lb_dalloc(h, &dRs, sizeof(double) * N)))) {
-        cudaError_t e = cudaMemcpyAsync(dX, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { lb_set_last_cuda_error(e, __FILE__, __LINE__); rc = LB_ERR_CUDA; }
-        if (!rc) rc = lb_run_sparsify(h, st, N, D, dX, max_points, dKept, n_kept, dRm, dRs, &h->launches);
-        const int64_t nr = rc ? 0 : N - *n_kept;
-        if (!rc && (e = cudaMemcpyAsync(kept, dKept, sizeof(int64_t) * *n_kept, cudaMemcpyDeviceToHost, st)) == cudaSuccess && nr > 0) {
-            if (removed) e = cudaMemcpyAsync(removed, dRm, sizeof(int64_t) * nr, cudaMemcpyDeviceToHost, st);
-            if (e == cudaSuccess && removed_score) e = cudaMemcpyAsync(removed_score, dRs, sizeof(double) * nr, cudaMemcpyDeviceToHost, st);
-        }
-        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-        if (!rc && e != cudaSuccess) { lb_set_last_cuda_error(e, __FILE__, __LINE__); rc = LB_ERR_CUDA; }
-    }
-    cudaStreamSynchronize(st);
-    for (void* q : {(void*)dX, (void*)dKept, (void*)dRm, (void*)dRs}) lb_pool_free(q);
-    return rc;
+    int rc;
+    if ((rc = tmp.alloc(sizeof(double) * N * D, &dX)) || (rc = tmp.alloc(sizeof(long long) * N, &dKept))
+        || (removed && (rc = tmp.alloc(sizeof(long long) * N, &dRm))) || (removed_score && (rc = tmp.alloc(sizeof(double) * N, &dRs))))
+        return rc;
+    LB_CUDA(cudaMemcpyAsync(dX, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
+    if ((rc = lb_run_sparsify(h, st, N, D, dX, max_points, dKept, n_kept, dRm, dRs, &h->launches))) return rc;
+    const int64_t nr = N - *n_kept;
+    LB_CUDA(cudaMemcpyAsync(kept, dKept, sizeof(int64_t) * *n_kept, cudaMemcpyDeviceToHost, st));
+    if (removed && nr > 0) LB_CUDA(cudaMemcpyAsync(removed, dRm, sizeof(int64_t) * nr, cudaMemcpyDeviceToHost, st));
+    if (removed_score && nr > 0) LB_CUDA(cudaMemcpyAsync(removed_score, dRs, sizeof(double) * nr, cudaMemcpyDeviceToHost, st));
+    LB_CUDA(cudaStreamSynchronize(st));
+    return LB_OK;
 }
 
 int lb_sparsify(const lb_gp* h, int64_t N, int D, const double* X_rowmajor, int64_t max_points, int64_t* kept, int64_t* n_kept,
@@ -1383,10 +1335,10 @@ int lb_log_lik(lb_gp* hh, double* out)
     if (!hh->fitted) return LB_ERR_STATE;
     LB_DEVICE(hh);
     lb_gp_full* h = full(hh);
-    int rc = lb_launch_loglik(h, h->ex.dMisc);
+    int rc = lb_launch_loglik(h, h->ex.dMisc.get());
     if (rc) return rc;
     double v[3];
-    LB_CUDA(cudaMemcpyAsync(v, h->ex.dMisc, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(v, h->ex.dMisc.get(), sizeof(v), cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     *out = v[2];
     return LB_OK;
@@ -1411,8 +1363,8 @@ int lb_kernel_grad_log_lik(lb_gp* hh, int optimize_noise, double* grad)
     if (!h->kinv_valid && (rc = lb_launch_kinv(h))) return rc;
     const int nh = h->n_hparams + (optimize_noise ? 1 : 0);
     if (nh > LB_MAX_HPARAMS) return LB_ERR_ARG;
-    if ((rc = lb_launch_grad(h, optimize_noise, h->ex.dMisc + 8))) return rc;
-    LB_CUDA(cudaMemcpyAsync(grad, h->ex.dMisc + 8, sizeof(double) * nh, cudaMemcpyDeviceToHost, h->stream));
+    if ((rc = lb_launch_grad(h, optimize_noise, h->ex.dMisc.get() + 8))) return rc;
+    LB_CUDA(cudaMemcpyAsync(grad, h->ex.dMisc.get() + 8, sizeof(double) * nh, cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     return LB_OK;
 }
@@ -1423,9 +1375,9 @@ int lb_log_loo_cv(lb_gp* hh, double* out)
     if (!hh->fitted) return LB_ERR_STATE;
     LB_DEVICE(hh);
     lb_gp_full* h = full(hh);
-    int rc = lb_launch_loo_value(h, h->ex.dMisc + 4);
+    int rc = lb_launch_loo_value(h, h->ex.dMisc.get() + 4);
     if (rc) return rc;
-    LB_CUDA(cudaMemcpyAsync(out, h->ex.dMisc + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(out, h->ex.dMisc.get() + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     return LB_OK;
 }
@@ -1438,9 +1390,9 @@ int lb_kernel_grad_log_loo_cv(lb_gp* hh, int optimize_noise, double* grad)
     lb_gp_full* h = full(hh);
     const int nh = h->n_hparams + (optimize_noise ? 1 : 0);
     if (nh > LB_MAX_HPARAMS) return LB_ERR_ARG;
-    int rc = lb_launch_loo_grad(h, optimize_noise, h->ex.dMisc + 8);
+    int rc = lb_launch_loo_grad(h, optimize_noise, h->ex.dMisc.get() + 8);
     if (rc) return rc;
-    LB_CUDA(cudaMemcpyAsync(grad, h->ex.dMisc + 8, sizeof(double) * nh, cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(grad, h->ex.dMisc.get() + 8, sizeof(double) * nh, cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     return LB_OK;
 }
@@ -1450,16 +1402,13 @@ int lb_kinv_obs_mean(lb_gp* h, double* out)
     if (!h || !out) return LB_ERR_ARG;
     if (!h->fitted) return LB_ERR_STATE;
     LB_DEVICE(h);
+    StreamTemps tmp(h->device, h->stream);
     double* dOut = nullptr;
-    LB_ALLOC(h, dOut, sizeof(double) * h->N * h->P);
-    int rc = lb_launch_kinv_obs(h, dOut);
-    if (!rc) {
-        if (cudaMemcpyAsync(out, dOut, sizeof(double) * h->N * h->P, cudaMemcpyDeviceToHost, h->stream) != cudaSuccess
-            || cudaStreamSynchronize(h->stream) != cudaSuccess)
-            rc = LB_ERR_CUDA;
-    }
-    lb_dfree_sync(h, dOut);
-    return rc;
+    int rc;
+    if ((rc = tmp.alloc(sizeof(double) * h->N * h->P, &dOut)) || (rc = lb_launch_kinv_obs(h, dOut))) return rc;
+    LB_CUDA(cudaMemcpyAsync(out, dOut, sizeof(double) * h->N * h->P, cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaStreamSynchronize(h->stream));
+    return LB_OK;
 }
 
 int lb_get(lb_gp* h, int what, double* dst)
@@ -1476,8 +1425,8 @@ int lb_get(lb_gp* h, int what, double* dst)
         return LB_OK;
     }
     if ((rc = lb_ensure_scratch(h, sizeof(double) * (size_t)(Np * Np + N * N)))) return rc;
-    double* dTmp = h->dScratch;
-    double* dOut = h->dScratch + Np * Np;
+    double* dTmp = h->dScratch.get();
+    double* dOut = h->dScratch.get() + Np * Np;
     const double* src = nullptr;
     int lower = 0;
     if (what == LB_GET_K) {
@@ -1496,10 +1445,10 @@ int lb_get(lb_gp* h, int what, double* dst)
         if (!h->fitted) return LB_ERR_STATE;
         if (!h->kinv_valid && (rc = lb_launch_kinv(h))) return rc;
         if (!h->kinv_sym) {
-            if ((rc = lb_launch_symmetrize(h, h->dKinv))) return rc;
+            if ((rc = lb_launch_symmetrize(h, h->dKinv.get()))) return rc;
             h->kinv_sym = true;
         }
-        src = h->dKinv;
+        src = h->dKinv.get();
     }
     else
         return LB_ERR_ARG;
@@ -1529,12 +1478,12 @@ int lb_clone(const lb_gp* src, lb_gp** out)
     h->kp.lambda = nullptr;
     std::memcpy(full(h)->ex.lambda_host, full(src)->ex.lambda_host, sizeof(full(h)->ex.lambda_host));
     if (src->kp.klam > 0) { // own copy of the Lambda matrix (rewritten by every lb_set_kernel)
-        if (lb_dalloc(h, &h->dLambda, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA)
-            || cudaMemcpyAsync(h->dLambda, src->dLambda, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) {
+        if (h->dLambda.resize(h, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA)
+            || cudaMemcpyAsync(h->dLambda.get(), src->dLambda.get(), sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA, cudaMemcpyDeviceToDevice, h->stream) != cudaSuccess) {
             lb_destroy(h);
             return LB_ERR_CUDA;
         }
-        h->kp.lambda = h->dLambda;
+        h->kp.lambda = h->dLambda.get();
     }
     if (src->Np > 0) {
         h->Np = src->Np;
@@ -1548,7 +1497,7 @@ int lb_clone(const lb_gp* src, lb_gp** out)
             h->dInvD = share(src->dInvD);
             h->fitted = true;
         }
-        if (src->dFlags && lb_dalloc(h, &h->dFlags, sizeof(int) * (src->Np / LB_TILE + 8))) { lb_destroy(h); return LB_ERR_ALLOC; }
+        if (src->dFlags && h->dFlags.resize(h, sizeof(int) * (src->Np / LB_TILE + 8))) { lb_destroy(h); return LB_ERR_ALLOC; }
     }
     *out = h;
     return LB_OK;
@@ -1616,8 +1565,9 @@ int lb_dchol_adopt_begin(lb_gp* h, int64_t Nd)
     int rc;
     if ((rc = ensure_fit_buffers(h))) return rc;
     if ((rc = lb_launch_scale_x(h))) return rc;
-    LB_CUDA(cudaMemsetAsync(h->dInfo, 0, 2 * sizeof(int), h->stream));
-    h->fitted = false; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), h->stream));
+    h->fitted = false;
+    lb_factor_changed(h);
     return LB_OK;
 }
 // one received (or own) panel message into the handle's L / invD, on `stream` (cudaStream_t as void*; NULL = the handle's)
@@ -1639,7 +1589,8 @@ int lb_dchol_adopt_end(lb_gp* h, int info)
     if (!h) return LB_ERR_ARG;
     LB_DEVICE(h);
     if (info > 0) return info;
-    h->fitted = true; h->linv_valid = false; h->linv_levels = 0; h->kinv_valid = false; h->linv32_valid = false;
+    h->fitted = true;
+    lb_factor_changed(h);
     int rc = lb_launch_solve_alpha(h);
     if (rc) return rc;
     return check_info(h);
@@ -1670,9 +1621,9 @@ int lb_dinv_columns(lb_gp* hc, int rank, int G, double* absmax_host)
     LB_DEVICE(h);
     std::lock_guard<std::mutex> lock(h->ex.qmutex);
     QueryWs& w = h->ex.ws;
-    if ((rc = ensure(h, &w.dV, &w.v_bytes, sizeof(double) * lb_linv_columns_scratch_doubles(h, G)))) return rc;
-    if ((rc = lb_launch_linv_columns(h, h->stream, rank, G, w.dV, &h->launches))) return rc;
-    return lb_dinv_absmax(h, w.dV, G, absmax_host);
+    if ((rc = ensure(h, w.dV, sizeof(double) * lb_linv_columns_scratch_doubles(h, G)))) return rc;
+    if ((rc = lb_launch_linv_columns(h, h->stream, rank, G, w.dV.get(), &h->launches))) return rc;
+    return lb_dinv_absmax(h, w.dV.get(), G, absmax_host);
 }
 
 int lb_dinv_pack(lb_gp* hc, int rank, int G, double absmax_all, void* dChunk)
@@ -1684,8 +1635,8 @@ int lb_dinv_pack(lb_gp* hc, int rank, int G, double absmax_all, void* dChunk)
     LB_DEVICE(h);
     std::lock_guard<std::mutex> lock(h->ex.qmutex);
     QueryWs& w = h->ex.ws;
-    if (!w.dV || w.v_bytes < sizeof(double) * lb_linv_columns_scratch_doubles(h, G)) return LB_ERR_STATE; // lb_dinv_columns first
-    return lb_dinv_pack_impl(h, w.dV, rank, G, absmax_all, dChunk);
+    if (!w.dV || w.dV.bytes() < sizeof(double) * lb_linv_columns_scratch_doubles(h, G)) return LB_ERR_STATE; // lb_dinv_columns first
+    return lb_dinv_pack_impl(h, w.dV.get(), rank, G, absmax_all, dChunk);
 }
 
 int lb_dinv_adopt(lb_gp* hc, int G, const void* dAll, double absmax_all)

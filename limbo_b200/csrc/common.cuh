@@ -16,6 +16,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <vector>
 
 #define LB_TILE 128
 #define LB_NEV 8 // events per handle: fork / panel x2 / a-update x2 / join / second-group fork + join
@@ -291,6 +292,125 @@ __device__ __forceinline__ double lb_warp_sum(double v)
 }
 
 // ---------------------------------------------------------------------------
+// Device buffers
+// ---------------------------------------------------------------------------
+// pooled, reference-counted device buffers (pool.cu): every buffer a handle owns comes from here
+void* lb_pool_alloc(int device, size_t bytes);
+void lb_pool_free(void* p);     // drops one reference; the buffer returns to the pool with the last one
+void lb_pool_retain(void* p);
+bool lb_pool_shared(void* p);   // more than one handle references the buffer
+
+struct lb_gp;
+
+// Sole owner of one pool lease: the buffers of a handle that lb_clone never shares.  No implicit conversion to T*, so a
+// DevBuf cannot be handed to lb_pool_free or overwritten with a raw pointer.  cudaFree synchronises implicitly, the pool
+// does not: a reallocation waits for `stream` before the old buffer goes back, release() does not wait (the owner
+// guarantees that no work on the buffer is pending).
+template <typename T>
+class DevBuf {
+public:
+    DevBuf() = default;
+    DevBuf(DevBuf&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; o.bytes_ = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept
+    {
+        if (this != &o) {
+            release();
+            p_ = o.p_; bytes_ = o.bytes_;
+            o.p_ = nullptr; o.bytes_ = 0;
+        }
+        return *this;
+    }
+    ~DevBuf() { release(); }
+    T* get() const { return p_; }
+    explicit operator bool() const { return p_ != nullptr; }
+    size_t bytes() const { return bytes_; }
+    // grow-only: at least `bytes`; a reallocation takes `slack` bytes more
+    int reserve(int device, cudaStream_t stream, size_t bytes, size_t slack = 0)
+    {
+        return (p_ && bytes_ >= bytes) ? LB_OK : take(device, stream, bytes + slack);
+    }
+    // exactly `bytes`
+    int resize(int device, cudaStream_t stream, size_t bytes) { return (p_ && bytes_ == bytes) ? LB_OK : take(device, stream, bytes); }
+    int reserve(const lb_gp* h, size_t bytes, size_t slack = 0);
+    int resize(const lb_gp* h, size_t bytes);
+    void release()
+    {
+        lb_pool_free(p_);
+        p_ = nullptr;
+        bytes_ = 0;
+    }
+
+private:
+    int take(int device, cudaStream_t stream, size_t bytes)
+    {
+        if (p_) {
+            cudaStreamSynchronize(stream); // kernels in flight may still use the old buffer
+            release();
+        }
+        p_ = static_cast<T*>(lb_pool_alloc(device, bytes));
+        if (!p_) return LB_ERR_ALLOC;
+        bytes_ = bytes;
+        return LB_OK;
+    }
+    T* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+
+// Buffers that live for one call on one stream: the destructor synchronises the stream once and returns every lease.
+class StreamTemps {
+public:
+    StreamTemps(int device, cudaStream_t stream) : device_(device), stream_(stream) {}
+    StreamTemps(const StreamTemps&) = delete;
+    StreamTemps& operator=(const StreamTemps&) = delete;
+    ~StreamTemps()
+    {
+        if (leases_.empty()) return;
+        cudaStreamSynchronize(stream_);
+        for (void* p : leases_) lb_pool_free(p);
+    }
+    template <typename T>
+    int alloc(size_t bytes, T** out)
+    {
+        *out = static_cast<T*>(lb_pool_alloc(device_, bytes));
+        if (!*out) return LB_ERR_ALLOC;
+        leases_.push_back(*out);
+        return LB_OK;
+    }
+
+private:
+    int device_;
+    cudaStream_t stream_;
+    std::vector<void*> leases_;
+};
+
+// The values, means and argmax records of an M-candidate acquisition.  Callers size vals / mean; reserve() sizes the
+// per-block (256 candidates) records and the final record.
+struct ArgmaxWs {
+    DevBuf<double> vals, mean, blk_val, best_val;
+    DevBuf<long long> blk_idx, best_idx;
+    int reserve(int device, cudaStream_t stream, int64_t M)
+    {
+        const size_t nblk = (size_t)((M + 255) / 256);
+        int rc;
+        if ((rc = blk_val.reserve(device, stream, sizeof(double) * nblk)) || (rc = blk_idx.reserve(device, stream, sizeof(long long) * nblk))
+            || (rc = best_val.reserve(device, stream, sizeof(double))) || (rc = best_idx.reserve(device, stream, sizeof(long long))))
+            return rc;
+        return LB_OK;
+    }
+    // the final record, and the M values when vals_out, to the host; synchronises the stream
+    int read_best(cudaStream_t stream, double* best, int64_t* idx, double* vals_out, int64_t M) const
+    {
+        long long bi = 0;
+        if (vals_out) LB_CUDA(cudaMemcpyAsync(vals_out, vals.get(), sizeof(double) * M, cudaMemcpyDeviceToHost, stream));
+        LB_CUDA(cudaMemcpyAsync(best, best_val.get(), sizeof(double), cudaMemcpyDeviceToHost, stream));
+        LB_CUDA(cudaMemcpyAsync(&bi, best_idx.get(), sizeof(long long), cudaMemcpyDeviceToHost, stream));
+        LB_CUDA(cudaStreamSynchronize(stream));
+        *idx = (int64_t)bi;
+        return LB_OK;
+    }
+};
+
+// ---------------------------------------------------------------------------
 // Host-side handle
 // ---------------------------------------------------------------------------
 struct lb_gp {
@@ -313,26 +433,26 @@ struct lb_gp {
 
     double* dX = nullptr;    // D x Np raw samples (SoA)
     double* dXs = nullptr;   // (D + LB_MAX_LAMBDA) x Np samples staged for the kernel (SE-ARD: x/ell, then A^T x)
-    double* dLambda = nullptr; // D x LB_MAX_LAMBDA (SE-ARD A matrix)
-    double* dLinvW = nullptr; int64_t linvw_np = 0; // reduced-precision path: |L^-1 e_k|^2 per column (rounding-bias weights)
+    DevBuf<double> dLambda;  // D x LB_MAX_LAMBDA (SE-ARD A matrix)
+    DevBuf<double> dLinvW;   // reduced-precision path: |L^-1 e_k|^2 per column (rounding-bias weights)
     double* dY = nullptr;    // Np x P  obs_mean (col-major), zero padded
     double* dL = nullptr;    // Np x Np K then L (col-major)
     double* dInvD = nullptr; // T x 128 x 128
     double* dAlpha = nullptr; // Np x P
-    double* dLinv = nullptr; // Np x Np (lazy: L^-1)
-    double* dKinv = nullptr; // Np x Np (lazy: K^-1, lower valid + mirrored)
-    float* dLinv32 = nullptr; int64_t linv32_rows = 0; bool linv32_valid = false; double linv32_scale = 1.0; // reduced-precision path: row-major fp32 / fp16 L^-1
-    int* dInfo = nullptr;    // [0] first failing pivot (1-based) or 0; [1] solver error
-    int* dFlags = nullptr;   // T+8 ints: ticket counters of the persistent solves
-    double* dTrsvX = nullptr; int64_t trsvx_np = 0; // trsv: published solution blocks (sentinel-filled per launch)
-    double* dScratch = nullptr; size_t scratch_bytes = 0;
+    DevBuf<double> dLinv;    // Np x Np (lazy: L^-1)
+    DevBuf<double> dKinv;    // Np x Np (lazy: K^-1, lower valid + mirrored)
+    DevBuf<float> dLinv32; bool linv32_valid = false; double linv32_scale = 1.0; // reduced-precision path: row-major fp32 / fp16 L^-1
+    DevBuf<int> dInfo;       // [0] first failing pivot (1-based) or 0; [1] solver error
+    DevBuf<int> dFlags;      // T+8 ints: ticket counters of the persistent solves
+    DevBuf<double> dTrsvX;   // trsv: published solution blocks (sentinel-filled per launch)
+    DevBuf<double> dScratch;
 
     bool fitted = false;
     bool linv_valid = false;
     int linv_levels = 0;     // diagonal blocks of this many 128-tiles of dLinv hold the inverse (0: nothing, >= T: all of L^-1)
     bool kinv_valid = false;
     bool kinv_sym = false;   // upper triangle of dKinv mirrored (needed by the LOO products and lb_get)
-    double* dWork = nullptr; int64_t work_np = 0; // Np x Np workspace (dK/dtheta of the LOO gradient)
+    DevBuf<double> dWork;    // Np x Np workspace (dK/dtheta of the LOO gradient)
     bool force_unfused = false; // tests: use the multi-launch query path
 
     // counters for bench.py ("gpu_launches")
@@ -340,16 +460,30 @@ struct lb_gp {
     void* prof = nullptr; // Profiler* when per-kernel-class event timing is enabled (abi.cu)
 };
 
+template <typename T>
+inline int DevBuf<T>::reserve(const lb_gp* h, size_t bytes, size_t slack) { return reserve(h->device, h->stream, bytes, slack); }
+template <typename T>
+inline int DevBuf<T>::resize(const lb_gp* h, size_t bytes) { return resize(h->device, h->stream, bytes); }
+
+// The factor changed: every cache derived from it (L^-1 and its diagonal-block levels, K^-1, the reduced-precision copy)
+// is stale.
+inline void lb_factor_changed(lb_gp* h)
+{
+    h->linv_valid = false;
+    h->linv_levels = 0;
+    h->kinv_valid = false;
+    h->linv32_valid = false;
+}
+
 // Every extern "C" entry that takes a handle runs on the handle's device and restores the caller's current device on
 // return (one process may hold handles on several GPUs, e.g. one MultiGP output per device).
 struct DeviceGuard {
     int prev = -1;
     bool ok = true;
-    explicit DeviceGuard(const lb_gp* h)
+    explicit DeviceGuard(int device)
     {
-        if (!h) return;
         if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-        if (prev != h->device && cudaSetDevice(h->device) != cudaSuccess) ok = false;
+        if (prev != device && cudaSetDevice(device) != cudaSuccess) ok = false;
     }
     ~DeviceGuard()
     {
@@ -360,7 +494,7 @@ struct DeviceGuard {
     }
 };
 #define LB_DEVICE(h)                        \
-    DeviceGuard lb_dev_guard__(h);          \
+    DeviceGuard lb_dev_guard__((h)->device); \
     if (!lb_dev_guard__.ok) return LB_ERR_CUDA
 
 // cudaFuncSetAttribute applies to the CURRENT device: once-only flags must be per device (one process may hold handles on
@@ -377,25 +511,12 @@ struct LbOncePerDevice {
     }
 };
 
-// pooled, reference-counted device buffers (pool.cu): every buffer a handle owns comes from here
-void* lb_pool_alloc(int device, size_t bytes);
-void lb_pool_free(void* p);     // drops one reference; the buffer returns to the pool with the last one
-void lb_pool_retain(void* p);
-bool lb_pool_shared(void* p);   // more than one handle references the buffer
+// the buffers lb_clone shares copy-on-write (ref-counted raw pointers)
 template <typename T>
 inline int lb_dalloc(const lb_gp* h, T** p, size_t bytes)
 {
     *p = static_cast<T*>(lb_pool_alloc(h->device, bytes));
     return *p ? LB_OK : LB_ERR_ALLOC;
-}
-// cudaFree synchronises implicitly, the pool does not: wait for the handle's pending work before a buffer that
-// kernels in flight may still use goes back to the pool
-template <typename H>
-inline void lb_dfree_sync(H* h, void* p)
-{
-    if (!p) return;
-    cudaStreamSynchronize(h->stream);
-    lb_pool_free(p);
 }
 #define LB_ALLOC(h, ptr, bytes)                      \
     do {                                             \

@@ -432,14 +432,14 @@ int lb_launch_linv_levels(lb_gp* h, int want_tiles)
     const int T = (int)(h->Np / LB_TILE);
     const size_t bytes = sizeof(double) * h->Np * h->Np;
     if (!h->dLinv) {
-        LB_ALLOC(h, h->dLinv, bytes);
-        LB_CUDA(cudaMemsetAsync(h->dLinv, 0, bytes, h->stream)); // strict upper part stays zero
+        if ((rc = h->dLinv.reserve(h, bytes))) return rc;
+        LB_CUDA(cudaMemsetAsync(h->dLinv.get(), 0, bytes, h->stream)); // strict upper part stays zero
         h->linv_levels = 0;
     }
-    if (!h->dKinv) LB_ALLOC(h, h->dKinv, bytes); // doubles as the W workspace of the recursion
+    if ((rc = h->dKinv.reserve(h, bytes))) return rc; // doubles as the W workspace of the recursion
     LbProfScope ps(h, h->stream, LB_PC_TRTRI);
     if (h->linv_levels == 0) {
-        trtri_diag_copy_kernel<<<T, 256, 0, h->stream>>>(h->dInvD, h->dLinv, h->Np);
+        trtri_diag_copy_kernel<<<T, 256, 0, h->stream>>>(h->dInvD, h->dLinv.get(), h->Np);
         h->launches++;
         h->linv_levels = 1;
     }
@@ -447,7 +447,7 @@ int lb_launch_linv_levels(lb_gp* h, int want_tiles)
         const int nprob = (T + 2 * sb - 1) / (2 * sb);
         h->kinv_valid = false; // W overwrites dKinv
         for (int step = 1; step <= 2; ++step) {
-            trtri_level_kernel<<<nprob * sb * sb, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, h->stream>>>(h->dL, h->dLinv, h->dKinv, h->Np, sb,
+            trtri_level_kernel<<<nprob * sb * sb, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, h->stream>>>(h->dL, h->dLinv.get(), h->dKinv.get(), h->Np, sb,
                 step, T);
             h->launches++;
         }
@@ -475,9 +475,9 @@ int lb_launch_kinv(lb_gp* h)
         if (rc) return rc;
     }
     const int T = (int)(h->Np / LB_TILE);
-    if (!h->dKinv) LB_ALLOC(h, h->dKinv, sizeof(double) * h->Np * h->Np);
+    if ((rc = h->dKinv.reserve(h, sizeof(double) * h->Np * h->Np))) return rc;
     LbProfScope ps(h, h->stream, LB_PC_LAUUM);
-    lauum_kernel<<<T * (T + 1) / 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, h->stream>>>(h->dLinv, h->Np, h->dKinv, T);
+    lauum_kernel<<<T * (T + 1) / 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, h->stream>>>(h->dLinv.get(), h->Np, h->dKinv.get(), T);
     h->launches++;
     LB_CUDA(cudaGetLastError());
     h->kinv_valid = true;
@@ -503,12 +503,12 @@ int lb_launch_grad(lb_gp* h, int optimize_noise, double* dGrad)
     if (rc) return rc;
     LbProfScope ps(h, h->stream, LB_PC_GRAD);
     switch (h->kp.id) {
-    case LB_K_SE_ARD: grad_kernel<LB_K_SE_ARD><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv, h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch); break;
-    case LB_K_MATERN52: grad_kernel<LB_K_MATERN52><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv, h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch); break;
-    case LB_K_MATERN32: grad_kernel<LB_K_MATERN32><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv, h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch); break;
-    default: grad_kernel<LB_K_EXP><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv, h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch); break;
+    case LB_K_SE_ARD: grad_kernel<LB_K_SE_ARD><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv.get(), h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch.get()); break;
+    case LB_K_MATERN52: grad_kernel<LB_K_MATERN52><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv.get(), h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch.get()); break;
+    case LB_K_MATERN32: grad_kernel<LB_K_MATERN32><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv.get(), h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch.get()); break;
+    default: grad_kernel<LB_K_EXP><<<ntiles, 256, 0, h->stream>>>(h->dXs, h->dKinv.get(), h->dAlpha, h->P, h->N, h->Np, h->kp, optimize_noise, nh, h->dScratch.get()); break;
     }
-    grad_reduce_kernel<<<nh, 256, 0, h->stream>>>(h->dScratch, ntiles, nh, dGrad);
+    grad_reduce_kernel<<<nh, 256, 0, h->stream>>>(h->dScratch.get(), ntiles, nh, dGrad);
     h->launches += 2;
     LB_CUDA(cudaGetLastError());
     if (h->kp.id == LB_K_SE_ARD && h->kp.klam > 0) return lb_launch_grad_lambda(h, dGrad);

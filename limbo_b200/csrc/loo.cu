@@ -256,7 +256,7 @@ int ensure_sym_kinv(lb_gp* h)
     int rc;
     if (!h->kinv_valid && (rc = lb_launch_kinv(h))) return rc;
     if (!h->kinv_sym) {
-        if ((rc = lb_launch_symmetrize(h, h->dKinv))) return rc;
+        if ((rc = lb_launch_symmetrize(h, h->dKinv.get()))) return rc;
         h->kinv_sym = true;
     }
     return LB_OK;
@@ -268,7 +268,7 @@ int lb_launch_loo_value(lb_gp* h, double* dOut)
 {
     int rc;
     if (!h->kinv_valid && (rc = lb_launch_kinv(h))) return rc;
-    loo_value_kernel<<<1, 1024, 0, h->stream>>>(h->dKinv, h->Np, h->N, h->dAlpha, h->P, dOut);
+    loo_value_kernel<<<1, 1024, 0, h->stream>>>(h->dKinv.get(), h->Np, h->N, h->dAlpha, h->P, dOut);
     h->launches++;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
@@ -281,22 +281,18 @@ int lb_launch_loo_grad(lb_gp* h, int optimize_noise, double* dGrad)
     const int64_t Np = h->Np;
     const int T = (int)(Np / LB_TILE);
     const int nh = h->n_hparams + (optimize_noise ? 1 : 0);
-    if (!h->dWork || h->work_np != Np) {
-        lb_dfree_sync(h, h->dWork);
-        h->dWork = nullptr;
-        LB_ALLOC(h, h->dWork, sizeof(double) * Np * Np);
-        h->work_np = Np;
-    }
+    if ((rc = h->dWork.resize(h, sizeof(double) * Np * Np))) return rc;
     if ((rc = lb_ensure_scratch(h, sizeof(double) * (size_t)(h->P + 1) * T * Np))) return rc;
     LB_CUDA(cudaFuncSetAttribute(loo_zeta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::PIPE_BYTES));
-    double* part_zk = h->dScratch;
-    double* part_za = h->dScratch + (int64_t)T * Np;
+    double* part_zk = h->dScratch.get();
+    double* part_za = h->dScratch.get() + (int64_t)T * Np;
     LbProfScope ps(h, h->stream, LB_PC_GRAD);
     for (int q = 0; q < nh; ++q) {
         dim3 g1((unsigned)Np, (unsigned)((Np + 255) / 256));
-        dk_build_kernel<<<g1, 256, 0, h->stream>>>(h->dXs, Np, h->N, h->kp, q, h->n_hparams, h->dWork);
-        loo_zeta_kernel<<<T * T, Cfg::THREADS, Cfg::PIPE_BYTES, h->stream>>>(h->dKinv, h->dWork, Np, h->dAlpha, h->P, T, part_zk, part_za);
-        loo_grad_reduce_kernel<<<1, 1024, 0, h->stream>>>(h->dKinv, Np, h->N, h->dAlpha, h->P, T, part_zk, part_za, dGrad + q);
+        dk_build_kernel<<<g1, 256, 0, h->stream>>>(h->dXs, Np, h->N, h->kp, q, h->n_hparams, h->dWork.get());
+        loo_zeta_kernel<<<T * T, Cfg::THREADS, Cfg::PIPE_BYTES, h->stream>>>(h->dKinv.get(), h->dWork.get(), Np, h->dAlpha, h->P, T, part_zk,
+            part_za);
+        loo_grad_reduce_kernel<<<1, 1024, 0, h->stream>>>(h->dKinv.get(), Np, h->N, h->dAlpha, h->P, T, part_zk, part_za, dGrad + q);
         h->launches += 3;
     }
     LB_CUDA(cudaGetLastError());
@@ -312,19 +308,14 @@ int lb_launch_grad_lambda(lb_gp* h, double* dGrad)
     int rc = ensure_sym_kinv(h);
     if (rc) return rc;
     const int64_t Np = h->Np;
-    if (!h->dWork || h->work_np != Np) {
-        lb_dfree_sync(h, h->dWork);
-        h->dWork = nullptr;
-        LB_ALLOC(h, h->dWork, sizeof(double) * Np * Np);
-        h->work_np = Np;
-    }
+    if ((rc = h->dWork.resize(h, sizeof(double) * Np * Np))) return rc;
     if ((rc = lb_ensure_scratch(h, sizeof(double) * WDOT_BLOCKS))) return rc;
     const int Dr = h->kp.Draw;
     for (int q = Dr; q < Dr + Dr * h->kp.klam; ++q) {
         dim3 g1((unsigned)Np, (unsigned)((Np + 255) / 256));
-        dk_build_kernel<<<g1, 256, 0, h->stream>>>(h->dXs, Np, h->N, h->kp, q, h->n_hparams, h->dWork);
-        wdot_kernel<<<WDOT_BLOCKS, 256, 0, h->stream>>>(h->dKinv, h->dWork, Np, h->N, h->dAlpha, h->P, h->dScratch);
-        wdot_reduce_kernel<<<1, 256, 0, h->stream>>>(h->dScratch, dGrad + q);
+        dk_build_kernel<<<g1, 256, 0, h->stream>>>(h->dXs, Np, h->N, h->kp, q, h->n_hparams, h->dWork.get());
+        wdot_kernel<<<WDOT_BLOCKS, 256, 0, h->stream>>>(h->dKinv.get(), h->dWork.get(), Np, h->N, h->dAlpha, h->P, h->dScratch.get());
+        wdot_reduce_kernel<<<1, 256, 0, h->stream>>>(h->dScratch.get(), dGrad + q);
         h->launches += 3;
     }
     LB_CUDA(cudaGetLastError());
@@ -338,8 +329,8 @@ int lb_launch_kinv_obs(lb_gp* h, double* dOut)
     if (rc) return rc;
     if ((rc = lb_ensure_scratch(h, sizeof(double) * (size_t)KSLICES * h->P * h->Np))) return rc;
     dim3 g((unsigned)((h->N + 255) / 256), KSLICES);
-    kinv_obs_kernel<<<g, 256, 0, h->stream>>>(h->dKinv, h->Np, h->N, h->dY, h->P, h->dScratch);
-    kinv_obs_reduce_kernel<<<(unsigned)((h->N + 255) / 256), 256, 0, h->stream>>>(h->dScratch, h->Np, h->N, h->P, dOut);
+    kinv_obs_kernel<<<g, 256, 0, h->stream>>>(h->dKinv.get(), h->Np, h->N, h->dY, h->P, h->dScratch.get());
+    kinv_obs_reduce_kernel<<<(unsigned)((h->N + 255) / 256), 256, 0, h->stream>>>(h->dScratch.get(), h->Np, h->N, h->P, dOut);
     h->launches += 2;
     LB_CUDA(cudaGetLastError());
     return LB_OK;

@@ -149,6 +149,8 @@ extern "C" {
 // cudaMalloc calls / pool hits so far (tests: a likelihood evaluation on a warm pool allocates nothing)
 long long lb_debug_pool_mallocs(void) { Pool& P = pool(); std::lock_guard<std::mutex> lk(P.mu); return P.n_malloc; }
 long long lb_debug_pool_hits(void) { Pool& P = pool(); std::lock_guard<std::mutex> lk(P.mu); return P.n_hit; }
+// buffers currently leased (tests: a balanced round of calls returns every lease it took)
+long long lb_debug_pool_live(void) { Pool& P = pool(); std::lock_guard<std::mutex> lk(P.mu); return (long long)P.live.size(); }
 // release every idle buffer of every device back to the driver
 int lb_pool_trim(void)
 {

@@ -299,7 +299,7 @@ int lb_debug_potf2_clocks(lb_gp* h, int k, long long* out_host, int n)
     long long* d = nullptr;
     LB_CUDA(cudaMalloc(&d, sizeof(long long) * 16));
     LB_CUDA(cudaMemset(d, 0, sizeof(long long) * 16));
-    potf2_inv_kernel<<<1, 256, POTF2_SMEM, h->stream>>>(h->dL, h->Np, k, h->dInvD, h->dInfo, 1, d);
+    potf2_inv_kernel<<<1, 256, POTF2_SMEM, h->stream>>>(h->dL, h->Np, k, h->dInvD, h->dInfo.get(), 1, d);
     LB_CUDA(cudaStreamSynchronize(h->stream));
     LB_CUDA(cudaMemcpy(out_host, d, sizeof(long long) * (n < 16 ? n : 16), cudaMemcpyDeviceToHost));
     cudaFree(d);
@@ -310,7 +310,7 @@ int lb_launch_potf2_block(lb_gp* h, int k, int do_factor)
 {
     int rc = set_attrs();
     if (rc) return rc;
-    potf2_inv_kernel<<<1, 256, POTF2_SMEM, h->stream>>>(h->dL, h->Np, k, h->dInvD, h->dInfo, do_factor);
+    potf2_inv_kernel<<<1, 256, POTF2_SMEM, h->stream>>>(h->dL, h->Np, k, h->dInvD, h->dInfo.get(), do_factor);
     h->launches++;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
@@ -339,7 +339,7 @@ static int launch_pair_panel(lb_gp* h, cudaStream_t side, int k, int T, int64_t 
 {
     {
         LbProfScope ps(h, side, LB_PC_POTF2);
-        potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo, 1);
+        potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo.get(), 1);
     }
     h->launches++;
     if (k + 1 < T) {
@@ -353,7 +353,7 @@ static int launch_pair_panel(lb_gp* h, cudaStream_t side, int k, int T, int64_t 
         }
         {
             LbProfScope ps(h, side, LB_PC_POTF2);
-            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo, 1);
+            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo.get(), 1);
         }
         h->launches += 3;
         if (k + 2 < T) {
@@ -371,7 +371,7 @@ static int launch_potrf_quads(lb_gp* h)
     const int T = (int)(h->Np / LB_TILE);
     const int64_t ld = h->Np;
     cudaStream_t main = h->stream, side = h->side ? h->side : h->stream;
-    LB_CUDA(cudaMemsetAsync(h->dInfo, 0, 2 * sizeof(int), main));
+    LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), main));
     if (side != main) {
         LB_CUDA(cudaEventRecord(h->ev[0], main)); // inputs (K) ready
         LB_CUDA(cudaStreamWaitEvent(side, h->ev[0], 0));
@@ -450,7 +450,7 @@ int lb_launch_potrf(lb_gp* h)
         if (h->aux) second = h->aux;
     }
     const int cstar = (second != main) ? (((int)(0.38 * T)) & ~1) : T; // even: a pair (k, k + 1) never straddles the boundary // left group: columns < cstar (long columns), right: >= cstar; ~equal tile counts at the start
-    LB_CUDA(cudaMemsetAsync(h->dInfo, 0, 2 * sizeof(int), main));
+    LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), main));
     if (side != main) {
         LB_CUDA(cudaEventRecord(h->ev[0], main)); // inputs (K) ready
         LB_CUDA(cudaStreamWaitEvent(side, h->ev[0], 0));
@@ -462,7 +462,7 @@ int lb_launch_potrf(lb_gp* h)
         // ---- panel(p) on the side stream ----
         {
             LbProfScope ps(h, side, LB_PC_POTF2);
-            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo, 1);
+            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo.get(), 1);
         }
         h->launches++;
         if (pair) {
@@ -476,7 +476,7 @@ int lb_launch_potrf(lb_gp* h)
             }
             {
                 LbProfScope ps(h, side, LB_PC_POTF2);
-                potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo, 1);
+                potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo.get(), 1);
             }
             h->launches += 3;
             if (k + 2 < T) {
@@ -728,8 +728,8 @@ int lb_dchol_finish(lb_gp* h, double* dLoc, int64_t Nd, int64_t N, int rank, int
     if (!h || !dLoc || !dLogdetPart) return LB_ERR_ARG;
     int rc = lb_ensure_scratch(h, sizeof(double) * 1024);
     if (rc) return rc;
-    dchol_finish_kernel<<<1024, 256, 0, h->stream>>>(dLoc, Nd, N, rank, G, ncols_local, h->dScratch);
-    dchol_sum_kernel<<<1, 1, 0, h->stream>>>(h->dScratch, 1024, dLogdetPart);
+    dchol_finish_kernel<<<1024, 256, 0, h->stream>>>(dLoc, Nd, N, rank, G, ncols_local, h->dScratch.get());
+    dchol_sum_kernel<<<1, 1, 0, h->stream>>>(h->dScratch.get(), 1024, dLogdetPart);
     h->launches += 2;
     LB_CUDA(cudaGetLastError());
     return LB_OK;

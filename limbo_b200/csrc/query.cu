@@ -1010,7 +1010,7 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
                 const int c0 = gbeg[g] * wmul, nc = (gbeg[g + 1] - gbeg[g]) * wmul;
                 if (nc <= 0) continue;
                 panel_update_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dL, ld, dV, dT, ldt, s0, nrows, c0, 0, 1);
-                panel_solve_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dLinv, ld, dT, ldt, dV, s0, nrows, dNorm, Mp, c0, 0, 1);
+                panel_solve_kernel<CD, false><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, sts[g]>>>(h->dLinv.get(), ld, dT, ldt, dV, s0, nrows, dNorm, Mp, c0, 0, 1);
                 if (launches) *launches += 2;
             }
         }
@@ -1074,7 +1074,7 @@ int lb_launch_linv_columns(lb_gp* h, cudaStream_t st, int rank, int G, double* d
     for (int s0 = 0; s0 < T; s0 += SB) {
         const int nrows = (T - s0 < SB) ? (T - s0) : SB;
         panel_update_kernel<CD, true><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, st>>>(h->dL, ld, dV, dT, ldt, s0, nrows, 0, rank, G);
-        panel_solve_kernel<CD, true><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, st>>>(h->dLinv, ld, dT, ldt, dV, s0, nrows, nullptr, Mp, 0, rank, G);
+        panel_solve_kernel<CD, true><<<nrows * nc, CD::THREADS, CD::PIPE_BYTES, st>>>(h->dLinv.get(), ld, dT, ldt, dV, s0, nrows, nullptr, Mp, 0, rank, G);
         if (launches) *launches += 2;
     }
     if (launches) *launches += 1;

@@ -354,80 +354,58 @@ int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const dou
     LB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sparsify_greedy_kernel, LOOP_THREADS, 0));
     if (per_sm < 1) return LB_ERR_UNSUPPORTED;
     const int G = nsm;
-    double *Xs = nullptr, *nbr_s = nullptr, *score = nullptr, *part_s = nullptr, *rs = nullptr;
+    StreamTemps tmp(h->device, st);
+    double *Xs = nullptr, *nbr_s = nullptr, *score = nullptr, *part_s = nullptr, *rs = dRemovedScore;
     int *nbr_j = nullptr, *alive = nullptr, *aff = nullptr, *aff_best = nullptr, *part_i = nullptr;
     unsigned* ctl = nullptr;
-    long long *cnt = nullptr, *rm = nullptr;
-    int rc = LB_OK;
-    auto release = [&]() {
-        cudaStreamSynchronize(st);
-        void* all[] = {Xs, nbr_s, score, part_s, nbr_j, alive, aff, aff_best, part_i, ctl, cnt, dRemoved ? nullptr : rm,
-            dRemovedScore ? nullptr : rs};
-        for (void* q : all) lb_pool_free(q);
-    };
-#define SP_ALLOC(ptr, bytes)                                 \
-    if ((rc = lb_dalloc(h, &(ptr), (bytes)))) { release(); return rc; }
-    SP_ALLOC(Xs, sizeof(double) * D * N);
-    SP_ALLOC(nbr_s, sizeof(double) * k * N);
-    SP_ALLOC(nbr_j, sizeof(int) * k * N);
-    SP_ALLOC(score, sizeof(double) * N);
-    SP_ALLOC(alive, sizeof(int) * N);
-    SP_ALLOC(aff, sizeof(int) * N);
-    SP_ALLOC(aff_best, sizeof(int) * N);
-    SP_ALLOC(part_s, sizeof(double) * G);
-    SP_ALLOC(part_i, sizeof(int) * G);
-    SP_ALLOC(ctl, sizeof(unsigned) * CTL_WORDS);
-    SP_ALLOC(cnt, sizeof(long long) * 2); // n_removed, n_kept
-    rm = dRemoved;
-    rs = dRemovedScore;
-    if (!rm) SP_ALLOC(rm, sizeof(long long) * N);
-    if (!rs) SP_ALLOC(rs, sizeof(double) * N);
-#undef SP_ALLOC
-    auto fail = [&](cudaError_t e, int line) {
-        lb_set_last_cuda_error(e, __FILE__, line);
-        release();
-        return LB_ERR_CUDA;
-    };
-    cudaError_t e;
-    if ((e = cudaMemsetAsync(ctl, 0, sizeof(unsigned) * CTL_WORDS, st)) != cudaSuccess) return fail(e, __LINE__);
-    if ((e = cudaMemsetAsync(cnt, 0, sizeof(long long) * 2, st)) != cudaSuccess) return fail(e, __LINE__);
-    cudaEvent_t ev[3] = {};
+    long long *cnt = nullptr, *rm = dRemoved;
+    int rc;
+    if ((rc = tmp.alloc(sizeof(double) * D * N, &Xs)) || (rc = tmp.alloc(sizeof(double) * k * N, &nbr_s))
+        || (rc = tmp.alloc(sizeof(int) * k * N, &nbr_j)) || (rc = tmp.alloc(sizeof(double) * N, &score))
+        || (rc = tmp.alloc(sizeof(int) * N, &alive)) || (rc = tmp.alloc(sizeof(int) * N, &aff)) || (rc = tmp.alloc(sizeof(int) * N, &aff_best))
+        || (rc = tmp.alloc(sizeof(double) * G, &part_s)) || (rc = tmp.alloc(sizeof(int) * G, &part_i))
+        || (rc = tmp.alloc(sizeof(unsigned) * CTL_WORDS, &ctl)) || (rc = tmp.alloc(sizeof(long long) * 2, &cnt)) // n_removed, n_kept
+        || (!rm && (rc = tmp.alloc(sizeof(long long) * N, &rm))) || (!rs && (rc = tmp.alloc(sizeof(double) * N, &rs))))
+        return rc;
+    LB_CUDA(cudaMemsetAsync(ctl, 0, sizeof(unsigned) * CTL_WORDS, st));
+    LB_CUDA(cudaMemsetAsync(cnt, 0, sizeof(long long) * 2, st));
+    struct Events { // debug timing (lb_debug_sparsify_timing)
+        cudaEvent_t ev[3] = {};
+        ~Events() { for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x); }
+    } t;
+    cudaEvent_t* ev = t.ev;
     if (g_timing.on)
-        for (cudaEvent_t& x : ev) cudaEventCreate(&x);
+        for (cudaEvent_t& x : t.ev) cudaEventCreate(&x);
     sparsify_soa_kernel<<<(unsigned)((N + 255) / 256), 256, 0, st>>>(dX, N, D, Xs);
     if (ev[0]) cudaEventRecord(ev[0], st);
     const size_t init_smem = sizeof(double) * 2 * D * INIT_THREADS;
     static LbOncePerDevice attr_once;
-    if (attr_once.need() &&
-        (e = cudaFuncSetAttribute(sparsify_knn_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-             (int)(sizeof(double) * 2 * LB_MAX_D * INIT_THREADS))) != cudaSuccess)
-        return fail(e, __LINE__);
+    if (attr_once.need())
+        LB_CUDA(cudaFuncSetAttribute(sparsify_knn_init_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+            (int)(sizeof(double) * 2 * LB_MAX_D * INIT_THREADS)));
     sparsify_knn_init_kernel<<<(unsigned)((N + INIT_THREADS - 1) / INIT_THREADS), INIT_THREADS, init_smem, st>>>(Xs, N, D, k, nbr_s,
         nbr_j, score, alive, ctl);
-    if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, __LINE__);
+    LB_CUDA(cudaGetLastError());
     if (ev[1]) cudaEventRecord(ev[1], st);
     const double* cXs = Xs;
     int64_t cN = N, cmax = max_points;
     int cD = D, ck = k;
     void* args[] = {(void*)&cXs, &cN, &cD, &ck, &cmax, &nbr_s, &nbr_j, &score, &alive, &aff, &aff_best, &part_s, &part_i, &ctl, &rm, &rs,
         &cnt};
-    if ((e = cudaLaunchCooperativeKernel((const void*)sparsify_greedy_kernel, dim3(G), dim3(LOOP_THREADS), args, 0, st)) != cudaSuccess)
-        return fail(e, __LINE__);
+    LB_CUDA(cudaLaunchCooperativeKernel((const void*)sparsify_greedy_kernel, dim3(G), dim3(LOOP_THREADS), args, 0, st));
     if (ev[2]) cudaEventRecord(ev[2], st);
     sparsify_compact_kernel<<<1, 1024, 0, st>>>(alive, N, dKept, cnt + 1);
-    if ((e = cudaGetLastError()) != cudaSuccess) return fail(e, __LINE__);
+    LB_CUDA(cudaGetLastError());
     *launches += 4;
     long long hc[2] = {0, 0};
     int herr = 0;
-    if ((e = cudaMemcpyAsync(hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return fail(e, __LINE__);
-    if ((e = cudaMemcpyAsync(&herr, ctl + CTL_ERR, sizeof(int), cudaMemcpyDeviceToHost, st)) != cudaSuccess) return fail(e, __LINE__);
-    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return fail(e, __LINE__);
+    LB_CUDA(cudaMemcpyAsync(hc, cnt, sizeof(hc), cudaMemcpyDeviceToHost, st));
+    LB_CUDA(cudaMemcpyAsync(&herr, ctl + CTL_ERR, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LB_CUDA(cudaStreamSynchronize(st));
     if (ev[0]) {
         cudaEventElapsedTime(&g_timing.ms[0], ev[0], ev[1]);
         cudaEventElapsedTime(&g_timing.ms[1], ev[1], ev[2]);
-        for (cudaEvent_t x : ev) cudaEventDestroy(x);
     }
-    release();
     if (herr & SP_ERR_NONFINITE) return LB_ERR_ARG;
     if (herr & SP_ERR_TIMEOUT) return LB_ERR_TIMEOUT;
     *n_kept = hc[1];

@@ -461,85 +461,56 @@ struct lb_spgp {
 
     int64_t N = 0, Np = 0;
     int D = 0;
-    double* dX = nullptr; // N x D row-major
-    double* dY = nullptr; // Np, zero padded
+    DevBuf<double> dX; // N x D row-major
+    DevBuf<double> dY; // Np, zero padded
 
     int M = 0;
-    int64_t Mp = 0, mp_alloc = 0, np_alloc = 0;
-    double *dXt = nullptr, *dXbt = nullptr, *dSb = nullptr;
-    double* dW = nullptr; size_t w_cap = 0; // w
-    double *dK = nullptr, *dV = nullptr, *dP1 = nullptr, *dP2 = nullptr, *dP3 = nullptr; // Mp x Np
-    double *dQ = nullptr, *dZ = nullptr, *dInvA = nullptr, *dTT = nullptr;               // Mp x Mp
-    double* dNv = nullptr;  // N-vectors, 12 x Np
-    double* dMv = nullptr;  // M-vectors, 8 x Mp
-    double* dS = nullptr;   // scalars
-    double* dOut = nullptr; size_t out_cap = 0; // f, grad
-    double* dWork = nullptr; size_t work_cap = 0; // split-K slices, row / block partials
+    int64_t Mp = 0;
+    DevBuf<double> dXt, dXbt, dSb;
+    DevBuf<double> dW;                    // w
+    DevBuf<double> dK, dV, dP1, dP2, dP3; // Mp x Np
+    DevBuf<double> dQ, dZ, dInvA, dTT;    // Mp x Mp
+    DevBuf<double> dNv;   // N-vectors, 12 x Np
+    DevBuf<double> dMv;   // M-vectors, 8 x Mp
+    DevBuf<double> dS;    // scalars
+    DevBuf<double> dOut;  // f, grad
+    DevBuf<double> dWork; // split-K slices, row / block partials
     // prediction state (lb_spgp_compute)
     bool computed = false;
     double c = 0, sig = 0;
     // query workspace
-    double *dQx = nullptr, *dQxt = nullptr, *dKs = nullptr, *dLst = nullptr, *dLmst = nullptr, *dQv = nullptr; size_t q_cap = 0;
-    double *dMu = nullptr, *dS2 = nullptr, *dAcq = nullptr, *dMeanQ = nullptr, *dBlk = nullptr; long long *dBlkIdx = nullptr, *dBestIdx = nullptr;
-    double* dBest = nullptr;
-    int64_t mq_cap = 0;
+    DevBuf<double> dQx, dQxt, dMu, dS2;
+    ArgmaxWs am; // acquisition values, means, argmax records
 };
 
 namespace {
 
-void spfree(void*& p)
-{
-    lb_pool_free(p);
-    p = nullptr;
-}
-#define SP_FREE(p) spfree(reinterpret_cast<void*&>(p))
-
-template <typename T>
-int spalloc(lb_spgp* s, T** p, size_t bytes)
-{
-    *p = static_cast<T*>(lb_pool_alloc(s->device, bytes));
-    return *p ? LB_OK : LB_ERR_ALLOC;
-}
-#define SP_ALLOC(s, p, bytes)                           \
-    do {                                                \
-        int rc_ = spalloc((s), &(p), (bytes));          \
-        if (rc_) return rc_;                            \
-    } while (0)
-
+// the inner handles' factor storage (raw: lb_gp's copy-on-write buffers, never shared here) and its inverses
 void free_inner(lb_gp* h)
 {
-    void* all[] = {h->dL, h->dInvD, h->dLinv, h->dKinv};
-    for (void* p : all) lb_pool_free(p);
-    h->dL = h->dInvD = h->dLinv = h->dKinv = nullptr;
-    h->linv_valid = h->kinv_valid = false;
-    h->linv_levels = 0;
+    lb_pool_free(h->dL);
+    lb_pool_free(h->dInvD);
+    h->dL = h->dInvD = nullptr;
+    h->dLinv.release();
+    h->dKinv.release();
+    lb_factor_changed(h);
     h->Np = 0;
 }
 
+// callers synchronise s->st before Mp changes (ensure_state: the Mp-sized buffers are reallocated first)
 int ensure_inner(lb_spgp* s, lb_gp* h, int64_t Mp, int M)
 {
     if (h->Np != Mp) {
         free_inner(h);
         const int64_t T = Mp / LB_TILE;
-        SP_ALLOC(s, h->dL, sizeof(double) * Mp * Mp);
-        SP_ALLOC(s, h->dInvD, sizeof(double) * T * LB_TILE * LB_TILE);
+        LB_ALLOC(h, h->dL, sizeof(double) * Mp * Mp);
+        LB_ALLOC(h, h->dInvD, sizeof(double) * T * LB_TILE * LB_TILE);
         LB_CUDA(cudaMemsetAsync(h->dInvD, 0, sizeof(double) * T * LB_TILE * LB_TILE, s->st));
         h->Np = Mp;
     }
     h->N = M;
-    h->linv_valid = h->kinv_valid = false; // a new factor invalidates the inverses
-    h->linv_levels = 0;
+    lb_factor_changed(h); // a new factor invalidates the inverses
     return LB_OK;
-}
-
-void free_state(lb_spgp* s)
-{
-    SP_FREE(s->dXt); SP_FREE(s->dXbt); SP_FREE(s->dSb);
-    SP_FREE(s->dK); SP_FREE(s->dV); SP_FREE(s->dP1); SP_FREE(s->dP2); SP_FREE(s->dP3);
-    SP_FREE(s->dQ); SP_FREE(s->dZ); SP_FREE(s->dInvA); SP_FREE(s->dTT);
-    SP_FREE(s->dNv); SP_FREE(s->dMv);
-    s->mp_alloc = s->np_alloc = 0;
-    s->computed = false;
 }
 
 int ensure_state(lb_spgp* s, int M)
@@ -547,34 +518,15 @@ int ensure_state(lb_spgp* s, int M)
     const int64_t Mp = round_up(M, LB_TILE), Np = s->Np;
     s->M = M;
     s->Mp = Mp;
-    if (s->mp_alloc != Mp || s->np_alloc != Np) {
-        cudaStreamSynchronize(s->st);
-        free_state(s);
-        const size_t mn = sizeof(double) * Mp * Np, mm = sizeof(double) * Mp * Mp;
-        SP_ALLOC(s, s->dXt, sizeof(double) * s->D * Np);
-        SP_ALLOC(s, s->dXbt, sizeof(double) * s->D * Mp);
-        SP_ALLOC(s, s->dSb, sizeof(double) * LB_MAX_D);
-        SP_ALLOC(s, s->dK, mn); SP_ALLOC(s, s->dV, mn); SP_ALLOC(s, s->dP1, mn); SP_ALLOC(s, s->dP2, mn); SP_ALLOC(s, s->dP3, mn);
-        SP_ALLOC(s, s->dQ, mm); SP_ALLOC(s, s->dZ, mm); SP_ALLOC(s, s->dInvA, mm); SP_ALLOC(s, s->dTT, mm);
-        SP_ALLOC(s, s->dNv, sizeof(double) * 12 * Np);
-        SP_ALLOC(s, s->dMv, sizeof(double) * 8 * Mp);
-        s->mp_alloc = Mp;
-        s->np_alloc = Np;
-    }
+    const size_t mn = sizeof(double) * Mp * Np, mm = sizeof(double) * Mp * Mp;
+    const std::pair<DevBuf<double>*, size_t> bufs[] = {{&s->dXt, sizeof(double) * s->D * Np}, {&s->dXbt, sizeof(double) * s->D * Mp},
+        {&s->dSb, sizeof(double) * LB_MAX_D}, {&s->dK, mn}, {&s->dV, mn}, {&s->dP1, mn}, {&s->dP2, mn}, {&s->dP3, mn}, {&s->dQ, mm},
+        {&s->dZ, mm}, {&s->dInvA, mm}, {&s->dTT, mm}, {&s->dNv, sizeof(double) * 12 * Np}, {&s->dMv, sizeof(double) * 8 * Mp}};
     int rc;
+    for (const auto& b : bufs)
+        if ((rc = b.first->resize(s->device, s->st, b.second))) return rc;
     if ((rc = ensure_inner(s, s->q, Mp, M))) return rc;
     if ((rc = ensure_inner(s, s->a, Mp, M))) return rc;
-    return LB_OK;
-}
-
-int ensure_buf(lb_spgp* s, double** p, size_t* cap, size_t bytes)
-{
-    if (*cap >= bytes && *p) return LB_OK;
-    cudaStreamSynchronize(s->st);
-    SP_FREE(*p);
-    *cap = 0;
-    SP_ALLOC(s, *p, bytes);
-    *cap = bytes;
     return LB_OK;
 }
 
@@ -596,15 +548,15 @@ int gemm(lb_spgp* s, const double* A, int64_t lda, const double* B, int64_t ldb,
     }
     double* out = C;
     if (splits > 1) {
-        int rc = ensure_buf(s, &s->dWork, &s->work_cap, sizeof(double) * splits * rows * cols);
+        int rc = s->dWork.reserve(s->device, s->st, sizeof(double) * splits * rows * cols);
         if (rc) return rc;
-        out = s->dWork;
+        out = s->dWork.get();
     }
     spgp_gemm_kernel<A_KC, B_KC><<<dim3(tiles, splits), GC::THREADS, GC::PIPE_BYTES, s->st>>>(A, lda, B, ldb, out, splits > 1 ? rows : ldc,
         rows * cols, mtiles, (int)K, tri, (int)kchunk, diag);
     s->launches++;
     if (splits > 1) {
-        spgp_split_reduce_kernel<<<nblocks(rows * cols, 256), 256, 0, s->st>>>(s->dWork, splits, rows, ldc, C, diag);
+        spgp_split_reduce_kernel<<<nblocks(rows * cols, 256), 256, 0, s->st>>>(s->dWork.get(), splits, rows, ldc, C, diag);
         s->launches++;
     }
     LB_CUDA(cudaGetLastError());
@@ -634,8 +586,8 @@ int check_w(const lb_spgp* s, int64_t M, int64_t n_w, const double* w)
 int read_info(lb_spgp* s)
 {
     int iq[2] = {0, 0}, ia[2] = {0, 0};
-    LB_CUDA(cudaMemcpyAsync(iq, s->q->dInfo, sizeof(iq), cudaMemcpyDeviceToHost, s->st));
-    LB_CUDA(cudaMemcpyAsync(ia, s->a->dInfo, sizeof(ia), cudaMemcpyDeviceToHost, s->st));
+    LB_CUDA(cudaMemcpyAsync(iq, s->q->dInfo.get(), sizeof(iq), cudaMemcpyDeviceToHost, s->st));
+    LB_CUDA(cudaMemcpyAsync(ia, s->a->dInfo.get(), sizeof(ia), cudaMemcpyDeviceToHost, s->st));
     LB_CUDA(cudaStreamSynchronize(s->st));
     if (iq[1] || ia[1]) return LB_ERR_TIMEOUT;
     if (iq[0] > 0) return iq[0];
@@ -657,37 +609,37 @@ int forward(lb_spgp* s, int M, const double* w, double jitter, double* c_out, do
     const double c = exp(w[(int64_t)(M + 1) * D]), sig = exp(w[(int64_t)(M + 1) * D + 1]);
     *c_out = c;
     *sig_out = sig;
-    if ((rc = ensure_buf(s, &s->dW, &s->w_cap, sizeof(double) * ((M + 1) * D + 2)))) return rc;
-    LB_CUDA(cudaMemcpyAsync(s->dSb, sb, sizeof(double) * D, cudaMemcpyHostToDevice, s->st));
-    LB_CUDA(cudaMemcpyAsync(s->dW, w, sizeof(double) * ((M + 1) * D + 2), cudaMemcpyHostToDevice, s->st));
-    double* ep = s->dNv;
-    double* yt = s->dNv + Np;
-    double* sumvsq = s->dNv + 2 * Np;
-    double* bet = s->dMv;
-    spgp_stage_kernel<<<dim3(nblocks(Np, 256), D), 256, 0, s->st>>>(s->dX, N, D, s->dSb, s->dXt, Np);
-    spgp_stage_xb_kernel<<<dim3(nblocks(Mp, 256), D), 256, 0, s->st>>>(s->dW, M, s->dSb, s->dXbt, Mp);
-    spgp_kmat_kernel<<<nblocks(Mp * Mp, 256), 256, 0, s->st>>>(s->dXbt, Mp, M, s->dXbt, Mp, M, D, c, s->dQ, Mp, Mp, 1, jitter, s->q->dL);
-    spgp_kmat_kernel<<<nblocks(Mp * Np, 256), 256, 0, s->st>>>(s->dXbt, Mp, M, s->dXt, Np, N, D, c, s->dK, Mp, Np, 0, 0.0, nullptr);
+    if ((rc = s->dW.reserve(s->device, s->st, sizeof(double) * ((M + 1) * D + 2)))) return rc;
+    LB_CUDA(cudaMemcpyAsync(s->dSb.get(), sb, sizeof(double) * D, cudaMemcpyHostToDevice, s->st));
+    LB_CUDA(cudaMemcpyAsync(s->dW.get(), w, sizeof(double) * ((M + 1) * D + 2), cudaMemcpyHostToDevice, s->st));
+    double* ep = s->dNv.get();
+    double* yt = s->dNv.get() + Np;
+    double* sumvsq = s->dNv.get() + 2 * Np;
+    double* bet = s->dMv.get();
+    spgp_stage_kernel<<<dim3(nblocks(Np, 256), D), 256, 0, s->st>>>(s->dX.get(), N, D, s->dSb.get(), s->dXt.get(), Np);
+    spgp_stage_xb_kernel<<<dim3(nblocks(Mp, 256), D), 256, 0, s->st>>>(s->dW.get(), M, s->dSb.get(), s->dXbt.get(), Mp);
+    spgp_kmat_kernel<<<nblocks(Mp * Mp, 256), 256, 0, s->st>>>(s->dXbt.get(), Mp, M, s->dXbt.get(), Mp, M, D, c, s->dQ.get(), Mp, Mp, 1, jitter, s->q->dL);
+    spgp_kmat_kernel<<<nblocks(Mp * Np, 256), 256, 0, s->st>>>(s->dXbt.get(), Mp, M, s->dXt.get(), Np, N, D, c, s->dK.get(), Mp, Np, 0, 0.0, nullptr);
     s->launches += 4;
     LB_CUDA(cudaGetLastError());
     // L = chol(Q), L^-1
     if ((rc = lb_launch_potrf(s->q))) return rc;
     if ((rc = lb_launch_linv(s->q))) return rc;
     // V = L^-1 K; ep; K~, V~, y~
-    if ((rc = gemm<false, true>(s, s->q->dLinv, Mp, s->dK, Mp, s->dV, Mp, Mp, Np, Mp, 1, 0.0))) return rc;
-    spgp_ep_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dK, s->dV, Mp, N, Np, s->dY, c, sig, ep, yt, sumvsq);
+    if ((rc = gemm<false, true>(s, s->q->dLinv.get(), Mp, s->dK.get(), Mp, s->dV.get(), Mp, Mp, Np, Mp, 1, 0.0))) return rc;
+    spgp_ep_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dK.get(), s->dV.get(), Mp, N, Np, s->dY.get(), c, sig, ep, yt, sumvsq);
     s->launches++;
     // Lm = chol(sig I + V~ V~^T), Lm^-1
-    if ((rc = gemm<false, false>(s, s->dV, Mp, s->dV, Mp, s->a->dL, Mp, Mp, Mp, Np, 0, sig))) return rc;
+    if ((rc = gemm<false, false>(s, s->dV.get(), Mp, s->dV.get(), Mp, s->a->dL, Mp, Mp, Mp, Np, 0, sig))) return rc;
     if ((rc = lb_launch_potrf(s->a))) return rc;
     if ((rc = lb_launch_linv(s->a))) return rc;
     // invLmV = Lm^-1 V~, bet = invLmV y~
-    if ((rc = gemm<false, true>(s, s->a->dLinv, Mp, s->dV, Mp, s->dP1, Mp, Mp, Np, Mp, 1, 0.0))) return rc;
+    if ((rc = gemm<false, true>(s, s->a->dLinv.get(), Mp, s->dV.get(), Mp, s->dP1.get(), Mp, Mp, Np, Mp, 1, 0.0))) return rc;
     int ns;
     const int64_t strip = pick_strip(s, Mp, N, &ns);
-    if ((rc = ensure_buf(s, &s->dWork, &s->work_cap, sizeof(double) * ns * Mp))) return rc;
-    spgp_rowdot_kernel<<<dim3((unsigned)(Mp / 128), ns), 128, 0, s->st>>>(s->dP1, Mp, N, strip, yt, s->dWork);
-    spgp_sum_parts_kernel<<<nblocks(Mp, 256), 256, 0, s->st>>>(s->dWork, ns, Mp, bet);
+    if ((rc = s->dWork.reserve(s->device, s->st, sizeof(double) * ns * Mp))) return rc;
+    spgp_rowdot_kernel<<<dim3((unsigned)(Mp / 128), ns), 128, 0, s->st>>>(s->dP1.get(), Mp, N, strip, yt, s->dWork.get());
+    spgp_sum_parts_kernel<<<nblocks(Mp, 256), 256, 0, s->st>>>(s->dWork.get(), ns, Mp, bet);
     s->launches += 3;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
@@ -701,53 +653,53 @@ int likelihood(lb_spgp* s, int M, const double* w, double jitter, double* f, dou
     const int D = s->D;
     const int64_t Mp = s->Mp, Np = s->Np, N = s->N;
     const int nw = (M + 1) * D + 2;
-    if ((rc = ensure_buf(s, &s->dOut, &s->out_cap, sizeof(double) * (nw + 1)))) return rc;
-    if (!s->dS) SP_ALLOC(s, s->dS, sizeof(double) * 64);
-    double* ep = s->dNv;
-    double* yt = s->dNv + Np;
-    double* sumvsq = s->dNv + 2 * Np;
-    double* mu = s->dNv + 3 * Np;
-    double* bv = s->dNv + 4 * Np;
-    double* sq_lmv = s->dNv + 5 * Np;
-    double* sq_lv = s->dNv + 6 * Np;
-    double* r = s->dNv + 7 * Np;
-    double* big = s->dNv + 8 * Np;
-    double* bet = s->dMv;
-    double* u = s->dMv + Mp;
-    double* b1 = s->dMv + 2 * Mp;
+    if ((rc = s->dOut.reserve(s->device, s->st, sizeof(double) * (nw + 1))) || (rc = s->dS.reserve(s->device, s->st, sizeof(double) * 64)))
+        return rc;
+    double* ep = s->dNv.get();
+    double* yt = s->dNv.get() + Np;
+    double* sumvsq = s->dNv.get() + 2 * Np;
+    double* mu = s->dNv.get() + 3 * Np;
+    double* bv = s->dNv.get() + 4 * Np;
+    double* sq_lmv = s->dNv.get() + 5 * Np;
+    double* sq_lv = s->dNv.get() + 6 * Np;
+    double* r = s->dNv.get() + 7 * Np;
+    double* big = s->dNv.get() + 8 * Np;
+    double* bet = s->dMv.get();
+    double* u = s->dMv.get() + Mp;
+    double* b1 = s->dMv.get() + 2 * Mp;
     const double half_nm = (double)((N - M) / 2); // spgp.hpp:491: (n - _m) / 2 in integer arithmetic
-    spgp_value_kernel<<<1, 1024, 0, s->st>>>(s->a->dL, Mp, M, bet, yt, ep, N, s->dS);
+    spgp_value_kernel<<<1, 1024, 0, s->st>>>(s->a->dL, Mp, M, bet, yt, ep, N, s->dS.get());
     s->launches++;
     if (!grad) {
-        spgp_final_kernel<<<1, 64, 0, s->st>>>(s->dS, nullptr, 0, nullptr, 0, nullptr, 0, s->dSb, M, D, half_nm, (double)N, sig, jitter, 0,
-            s->dOut, s->dOut + 1);
+        spgp_final_kernel<<<1, 64, 0, s->st>>>(s->dS.get(), nullptr, 0, nullptr, 0, nullptr, 0, s->dSb.get(), M, D, half_nm, (double)N, sig, jitter, 0,
+            s->dOut.get(), s->dOut.get() + 1);
         s->launches++;
         LB_CUDA(cudaGetLastError());
         if ((rc = read_info(s))) return rc;
-        LB_CUDA(cudaMemcpy(f, s->dOut, sizeof(double), cudaMemcpyDeviceToHost));
+        LB_CUDA(cudaMemcpy(f, s->dOut.get(), sizeof(double), cudaMemcpyDeviceToHost));
         return LB_OK;
     }
     // bet^T invLmV and colsum(invLmV^2); u = Lm^-T bet; b1 = L^-T u; mu = u^T V~  (spgp.hpp:503, 512, 516)
-    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dP1, Mp, Np, bet, bv, sq_lmv);
-    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->a->dLinv, Mp, Mp, bet, u, nullptr);
-    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->q->dLinv, Mp, Mp, u, b1, nullptr);
-    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dV, Mp, Np, u, mu, nullptr);
+    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dP1.get(), Mp, Np, bet, bv, sq_lmv);
+    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->a->dLinv.get(), Mp, Mp, bet, u, nullptr);
+    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->q->dLinv.get(), Mp, Mp, u, b1, nullptr);
+    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dV.get(), Mp, Np, u, mu, nullptr);
     s->launches += 4;
     // B1 = L^-T (Lm^-T invLmV) (:502), invLV = L^-T V~ (:505)
-    if ((rc = gemm<true, true>(s, s->a->dLinv, Mp, s->dP1, Mp, s->dP2, Mp, Mp, Np, Mp, 2, 0.0))) return rc;
-    if ((rc = gemm<true, true>(s, s->q->dLinv, Mp, s->dP2, Mp, s->dP3, Mp, Mp, Np, Mp, 2, 0.0))) return rc;
-    if ((rc = gemm<true, true>(s, s->q->dLinv, Mp, s->dV, Mp, s->dP2, Mp, Mp, Np, Mp, 2, 0.0))) return rc;
-    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dP2, Mp, Np, nullptr, nullptr, sq_lv);
-    spgp_nvec_kernel<<<1, 1024, 0, s->st>>>(yt, mu, bv, sq_lmv, ep, sumvsq, sq_lv, N, Np, c, sig, jitter, r, big, s->dS);
+    if ((rc = gemm<true, true>(s, s->a->dLinv.get(), Mp, s->dP1.get(), Mp, s->dP2.get(), Mp, Mp, Np, Mp, 2, 0.0))) return rc;
+    if ((rc = gemm<true, true>(s, s->q->dLinv.get(), Mp, s->dP2.get(), Mp, s->dP3.get(), Mp, Mp, Np, Mp, 2, 0.0))) return rc;
+    if ((rc = gemm<true, true>(s, s->q->dLinv.get(), Mp, s->dV.get(), Mp, s->dP2.get(), Mp, Mp, Np, Mp, 2, 0.0))) return rc;
+    spgp_coldot_kernel<<<nblocks(Np, 8), 256, 0, s->st>>>(s->dP2.get(), Mp, Np, nullptr, nullptr, sq_lv);
+    spgp_nvec_kernel<<<1, 1024, 0, s->st>>>(yt, mu, bv, sq_lmv, ep, sumvsq, sq_lv, N, Np, c, sig, jitter, r, big, s->dS.get());
     // TT = invLV diag(bigsum) invLV^T (:518)
-    spgp_scale_cols_kernel<<<nblocks(Mp * Np, 256), 256, 0, s->st>>>(s->dP2, Mp, Np, big, s->dP1);
+    spgp_scale_cols_kernel<<<nblocks(Mp * Np, 256), 256, 0, s->st>>>(s->dP2.get(), Mp, Np, big, s->dP1.get());
     s->launches += 3;
-    if ((rc = gemm<false, false>(s, s->dP2, Mp, s->dP1, Mp, s->dTT, Mp, Mp, Mp, Np, 0, 0.0))) return rc;
+    if ((rc = gemm<false, false>(s, s->dP2.get(), Mp, s->dP1.get(), Mp, s->dTT.get(), Mp, Mp, Mp, Np, 0, 0.0))) return rc;
     // invQ = L^-T L^-1 (:507), invA = Z^T Z with Z = Lm^-1 L^-1 (:508-509)
     if ((rc = lb_launch_kinv(s->q))) return rc;
-    if ((rc = lb_launch_symmetrize(s->q, s->q->dKinv))) return rc;
-    if ((rc = gemm<false, true>(s, s->a->dLinv, Mp, s->q->dLinv, Mp, s->dZ, Mp, Mp, Mp, Mp, 1, 0.0))) return rc;
-    if ((rc = gemm<true, true>(s, s->dZ, Mp, s->dZ, Mp, s->dInvA, Mp, Mp, Mp, Mp, 2, 0.0))) return rc;
+    if ((rc = lb_launch_symmetrize(s->q, s->q->dKinv.get()))) return rc;
+    if ((rc = gemm<false, true>(s, s->a->dLinv.get(), Mp, s->q->dLinv.get(), Mp, s->dZ.get(), Mp, Mp, Mp, Mp, 1, 0.0))) return rc;
+    if ((rc = gemm<true, true>(s, s->dZ.get(), Mp, s->dZ.get(), Mp, s->dInvA.get(), Mp, Mp, Mp, Mp, 2, 0.0))) return rc;
     // the two weighted passes
     int nsG, nsH;
     const int64_t stripG = pick_strip(s, Mp, N, &nsG), stripH = pick_strip(s, Mp, M, &nsH);
@@ -755,32 +707,32 @@ int likelihood(lb_spgp* s, int M, const double* w, double jitter, double* f, dou
     const size_t offH = (size_t)nsG * (D + 1) * Mp, offBG = offH + (size_t)nsH * (D + 1) * Mp;
     const size_t offBH = offBG + (size_t)nsG * mtb * D, offX = offBH + (size_t)nsH * mtb * 5;
     const int nxb = (M + 127) / 128;
-    if ((rc = ensure_buf(s, &s->dWork, &s->work_cap, sizeof(double) * (offX + (size_t)D * nxb)))) return rc;
+    if ((rc = s->dWork.reserve(s->device, s->st, sizeof(double) * (offX + (size_t)D * nxb)))) return rc;
     PassArgs pa{};
-    pa.E0 = s->dK; pa.E1 = s->dP3; pa.E2 = s->dP2; pa.E3 = nullptr; pa.ld = Mp;
+    pa.E0 = s->dK.get(); pa.E1 = s->dP3.get(); pa.E2 = s->dP2.get(); pa.E3 = nullptr; pa.ld = Mp;
     pa.b1 = b1; pa.r = r; pa.big = big;
-    pa.xc = s->dXt; pa.ldxc = Np; pa.xr = s->dXbt; pa.ldxr = Mp;
+    pa.xc = s->dXt.get(); pa.ldxc = Np; pa.xr = s->dXbt.get(); pa.ldxr = Mp;
     pa.cols = N; pa.strip = stripG; pa.D = D; pa.sig = sig;
-    pa.rowpart = s->dWork; pa.blkpart = s->dWork + offBG;
+    pa.rowpart = s->dWork.get(); pa.blkpart = s->dWork.get() + offBG;
     spgp_pass_kernel<0><<<dim3((unsigned)mtb, nsG), 128, 0, s->st>>>(pa);
     PassArgs ph = pa;
-    ph.E0 = s->dQ; ph.E1 = s->q->dKinv; ph.E2 = s->dInvA; ph.E3 = s->dTT;
-    ph.xc = s->dXbt; ph.ldxc = Mp; ph.cols = M; ph.strip = stripH;
-    ph.rowpart = s->dWork + offH; ph.blkpart = s->dWork + offBH;
+    ph.E0 = s->dQ.get(); ph.E1 = s->q->dKinv.get(); ph.E2 = s->dInvA.get(); ph.E3 = s->dTT.get();
+    ph.xc = s->dXbt.get(); ph.ldxc = Mp; ph.cols = M; ph.strip = stripH;
+    ph.rowpart = s->dWork.get() + offH; ph.blkpart = s->dWork.get() + offBH;
     spgp_pass_kernel<1><<<dim3((unsigned)mtb, nsH), 128, 0, s->st>>>(ph);
-    spgp_dfxb_kernel<<<dim3(nxb, D), 128, 0, s->st>>>(s->dWork, nsG, s->dWork + offH, nsH, Mp, M, D, s->dXbt, s->dSb, s->dOut + 1,
-        s->dWork + offX);
-    spgp_final_kernel<<<1, 64, 0, s->st>>>(s->dS, s->dWork + offBG, nsG * (int)mtb, s->dWork + offBH, nsH * (int)mtb, s->dWork + offX, nxb,
-        s->dSb, M, D, half_nm, (double)N, sig, jitter, 1, s->dOut, s->dOut + 1);
+    spgp_dfxb_kernel<<<dim3(nxb, D), 128, 0, s->st>>>(s->dWork.get(), nsG, s->dWork.get() + offH, nsH, Mp, M, D, s->dXbt.get(), s->dSb.get(), s->dOut.get() + 1,
+        s->dWork.get() + offX);
+    spgp_final_kernel<<<1, 64, 0, s->st>>>(s->dS.get(), s->dWork.get() + offBG, nsG * (int)mtb, s->dWork.get() + offBH, nsH * (int)mtb, s->dWork.get() + offX, nxb,
+        s->dSb.get(), M, D, half_nm, (double)N, sig, jitter, 1, s->dOut.get(), s->dOut.get() + 1);
     s->launches += 4;
     LB_CUDA(cudaGetLastError());
     if ((rc = read_info(s))) return rc;
-    LB_CUDA(cudaMemcpy(f, s->dOut, sizeof(double), cudaMemcpyDeviceToHost));
-    LB_CUDA(cudaMemcpy(grad, s->dOut + 1, sizeof(double) * nw, cudaMemcpyDeviceToHost));
+    LB_CUDA(cudaMemcpy(f, s->dOut.get(), sizeof(double), cudaMemcpyDeviceToHost));
+    LB_CUDA(cudaMemcpy(grad, s->dOut.get() + 1, sizeof(double) * nw, cudaMemcpyDeviceToHost));
     return LB_OK;
 }
 
-// mu - mean and sigma^2 of Mq candidates (device row-major dQx) into s->dMu / s->dS2, in chunks of QCHUNK
+// mu - mean and sigma^2 of Mq candidates (device row-major dQx) into s->dMu.get() / s->dS2.get(), in chunks of QCHUNK
 int predict(lb_spgp* s, int64_t Mq, int optimized)
 {
     const int D = s->D;
@@ -788,22 +740,22 @@ int predict(lb_spgp* s, int64_t Mq, int optimized)
     const int64_t Cp = round_up(std::min<int64_t>(Mq, QCHUNK), LB_TILE);
     int rc;
     if ((rc = set_attrs())) return rc;
-    if ((rc = ensure_buf(s, &s->dQxt, &s->q_cap, sizeof(double) * (3 * Mp * Cp + (size_t)D * Cp + 2 * Cp)))) return rc;
-    double* ks = s->dQxt + (size_t)D * Cp;
+    if ((rc = s->dQxt.reserve(s->device, s->st, sizeof(double) * (3 * Mp * Cp + (size_t)D * Cp + 2 * Cp)))) return rc;
+    double* ks = s->dQxt.get() + (size_t)D * Cp;
     double* lst = ks + Mp * Cp;
     double* lmst = lst + Mp * Cp;
     double* sq1 = lmst + Mp * Cp;
     double* sq2 = sq1 + Cp;
     for (int64_t q0 = 0; q0 < Mq; q0 += QCHUNK) {
         const int64_t nq = std::min<int64_t>(QCHUNK, Mq - q0), nqp = round_up(nq, LB_TILE);
-        spgp_stage_kernel<<<dim3(nblocks(nqp, 256), D), 256, 0, s->st>>>(s->dQx + q0 * D, nq, D, s->dSb, s->dQxt, nqp);
-        spgp_kmat_kernel<<<nblocks(Mp * nqp, 256), 256, 0, s->st>>>(s->dXbt, Mp, s->M, s->dQxt, nqp, nq, D, s->c, ks, Mp, nqp, 0, 0.0, nullptr);
+        spgp_stage_kernel<<<dim3(nblocks(nqp, 256), D), 256, 0, s->st>>>(s->dQx.get() + q0 * D, nq, D, s->dSb.get(), s->dQxt.get(), nqp);
+        spgp_kmat_kernel<<<nblocks(Mp * nqp, 256), 256, 0, s->st>>>(s->dXbt.get(), Mp, s->M, s->dQxt.get(), nqp, nq, D, s->c, ks, Mp, nqp, 0, 0.0, nullptr);
         s->launches += 2;
-        if ((rc = gemm<false, true>(s, s->q->dLinv, Mp, ks, Mp, lst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
-        if ((rc = gemm<false, true>(s, s->a->dLinv, Mp, lst, Mp, lmst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
-        spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lmst, Mp, nq, s->dMv, s->dMu + q0, sq2);
+        if ((rc = gemm<false, true>(s, s->q->dLinv.get(), Mp, ks, Mp, lst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
+        if ((rc = gemm<false, true>(s, s->a->dLinv.get(), Mp, lst, Mp, lmst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
+        spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lmst, Mp, nq, s->dMv.get(), s->dMu.get() + q0, sq2);
         spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lst, Mp, nq, nullptr, nullptr, sq1);
-        spgp_pred_kernel<<<nblocks(nq, 256), 256, 0, s->st>>>(sq1, sq2, nq, s->c, s->sig, optimized ? s->sig : 0.0, s->dS2 + q0);
+        spgp_pred_kernel<<<nblocks(nq, 256), 256, 0, s->st>>>(sq1, sq2, nq, s->c, s->sig, optimized ? s->sig : 0.0, s->dS2.get() + q0);
         s->launches += 3;
         LB_CUDA(cudaGetLastError());
     }
@@ -812,43 +764,14 @@ int predict(lb_spgp* s, int64_t Mq, int optimized)
 
 int ensure_query(lb_spgp* s, int64_t Mq, const double* Xq)
 {
-    if (Mq > s->mq_cap) {
-        cudaStreamSynchronize(s->st);
-        SP_FREE(s->dQx); SP_FREE(s->dMu); SP_FREE(s->dS2); SP_FREE(s->dAcq); SP_FREE(s->dMeanQ); SP_FREE(s->dBlk); SP_FREE(s->dBlkIdx); SP_FREE(s->dBest);
-        SP_FREE(s->dBestIdx);
-        s->mq_cap = 0;
-        const int64_t nblk = (Mq + 255) / 256;
-        SP_ALLOC(s, s->dQx, sizeof(double) * Mq * s->D);
-        SP_ALLOC(s, s->dMu, sizeof(double) * Mq);
-        SP_ALLOC(s, s->dS2, sizeof(double) * Mq);
-        SP_ALLOC(s, s->dAcq, sizeof(double) * Mq);
-        SP_ALLOC(s, s->dMeanQ, sizeof(double) * Mq);
-        SP_ALLOC(s, s->dBlk, sizeof(double) * nblk);
-        SP_ALLOC(s, s->dBlkIdx, sizeof(long long) * nblk);
-        SP_ALLOC(s, s->dBest, sizeof(double));
-        SP_ALLOC(s, s->dBestIdx, sizeof(long long));
-        s->mq_cap = Mq;
-    }
-    LB_CUDA(cudaMemcpyAsync(s->dQx, Xq, sizeof(double) * Mq * s->D, cudaMemcpyHostToDevice, s->st));
+    const size_t mq = sizeof(double) * Mq;
+    int rc;
+    for (DevBuf<double>* b : {&s->dMu, &s->dS2, &s->am.vals, &s->am.mean})
+        if ((rc = b->reserve(s->device, s->st, mq))) return rc;
+    if ((rc = s->dQx.reserve(s->device, s->st, mq * s->D)) || (rc = s->am.reserve(s->device, s->st, Mq))) return rc;
+    LB_CUDA(cudaMemcpyAsync(s->dQx.get(), Xq, mq * s->D, cudaMemcpyHostToDevice, s->st));
     return LB_OK;
 }
-
-struct SpDevice {
-    int prev = -1;
-    bool ok = true;
-    explicit SpDevice(int dev)
-    {
-        if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-        if (prev != dev && cudaSetDevice(dev) != cudaSuccess) ok = false;
-    }
-    ~SpDevice()
-    {
-        if (prev >= 0) cudaSetDevice(prev);
-    }
-};
-#define SP_DEVICE(s)                  \
-    SpDevice sp_dev__((s)->device);   \
-    if (!sp_dev__.ok) return LB_ERR_CUDA
 
 } // namespace
 
@@ -868,7 +791,7 @@ int lb_spgp_create(lb_spgp** out, int device)
         delete s;
         return rc;
     }
-    SpDevice g(device);
+    DeviceGuard g(device);
     s->st = s->q->stream;
     if ((rc = lb_set_stream(s->a, s->st))) { // one stream for the whole evaluation (A's factor has its own side stream)
         lb_spgp_destroy(s);
@@ -882,17 +805,11 @@ int lb_spgp_create(lb_spgp** out, int device)
 int lb_spgp_destroy(lb_spgp* s)
 {
     if (!s) return LB_OK;
-    {
-        SpDevice g(s->device);
-        cudaStreamSynchronize(s->st);
-        free_state(s);
-        SP_FREE(s->dX); SP_FREE(s->dY); SP_FREE(s->dW); SP_FREE(s->dS); SP_FREE(s->dOut); SP_FREE(s->dWork); SP_FREE(s->dQxt);
-        SP_FREE(s->dQx); SP_FREE(s->dMu); SP_FREE(s->dS2); SP_FREE(s->dAcq); SP_FREE(s->dMeanQ); SP_FREE(s->dBlk); SP_FREE(s->dBlkIdx); SP_FREE(s->dBest);
-        SP_FREE(s->dBestIdx);
-        if (s->a) { lb_set_stream(s->a, nullptr); free_inner(s->a); lb_destroy(s->a); }
-        if (s->q) { free_inner(s->q); lb_destroy(s->q); }
-    }
-    delete s;
+    DeviceGuard g(s->device);
+    cudaStreamSynchronize(s->st);
+    if (s->a) { lb_set_stream(s->a, nullptr); free_inner(s->a); lb_destroy(s->a); }
+    if (s->q) { free_inner(s->q); lb_destroy(s->q); }
+    delete s; // its buffers go back to the pool
     return LB_OK;
 }
 
@@ -905,22 +822,18 @@ int lb_spgp_set_data(lb_spgp* s, int64_t N, int D, const double* X_rowmajor, con
     for (int64_t i = 0; i < N; ++i)
         if (!std::isfinite(y_zm[i])) return LB_ERR_ARG;
     std::lock_guard<std::mutex> lk(s->mu);
-    SP_DEVICE(s);
+    LB_DEVICE(s);
     LB_CUDA(cudaStreamSynchronize(s->st));
     const int64_t Np = round_up(N, LB_TILE);
-    if (Np != s->Np || D != s->D) {
-        free_state(s);
-        SP_FREE(s->dX); SP_FREE(s->dY);
-        SP_ALLOC(s, s->dX, sizeof(double) * Np * D);
-        SP_ALLOC(s, s->dY, sizeof(double) * Np);
-    }
+    int rc;
+    if ((rc = s->dX.resize(s->device, s->st, sizeof(double) * Np * D)) || (rc = s->dY.resize(s->device, s->st, sizeof(double) * Np))) return rc;
     s->N = N;
     s->Np = Np;
     s->D = D;
     s->computed = false;
-    LB_CUDA(cudaMemcpyAsync(s->dX, X_rowmajor, sizeof(double) * N * D, cudaMemcpyHostToDevice, s->st));
-    LB_CUDA(cudaMemsetAsync(s->dY, 0, sizeof(double) * Np, s->st));
-    LB_CUDA(cudaMemcpyAsync(s->dY, y_zm, sizeof(double) * N, cudaMemcpyHostToDevice, s->st));
+    LB_CUDA(cudaMemcpyAsync(s->dX.get(), X_rowmajor, sizeof(double) * N * D, cudaMemcpyHostToDevice, s->st));
+    LB_CUDA(cudaMemsetAsync(s->dY.get(), 0, sizeof(double) * Np, s->st));
+    LB_CUDA(cudaMemcpyAsync(s->dY.get(), y_zm, sizeof(double) * N, cudaMemcpyHostToDevice, s->st));
     LB_CUDA(cudaStreamSynchronize(s->st));
     return LB_OK;
 }
@@ -932,7 +845,7 @@ int lb_spgp_lik(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double jitt
     int rc = check_w(s, M, n_w, w);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(s->mu);
-    SP_DEVICE(s);
+    LB_DEVICE(s);
     s->computed = false; // the factors now belong to this w
     return likelihood(s, (int)M, w, jitter, f, grad);
 }
@@ -944,7 +857,7 @@ int lb_spgp_compute(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double 
     int rc = check_w(s, M, n_w, w);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(s->mu);
-    SP_DEVICE(s);
+    LB_DEVICE(s);
     s->computed = false;
     double c, sig;
     if ((rc = forward(s, (int)M, w, jitter, &c, &sig))) return rc;
@@ -962,12 +875,12 @@ int lb_spgp_query(const lb_spgp* sc, int64_t Mq, const double* Xq_rowmajor, int 
     std::lock_guard<std::mutex> lk(s->mu);
     if (!s->computed) return LB_ERR_STATE;
     if (Mq == 0) return LB_OK;
-    SP_DEVICE(s);
+    LB_DEVICE(s);
     int rc;
     if ((rc = ensure_query(s, Mq, Xq_rowmajor))) return rc;
     if ((rc = predict(s, Mq, optimized))) return rc;
-    LB_CUDA(cudaMemcpyAsync(mu_minus_mean, s->dMu, sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
-    LB_CUDA(cudaMemcpyAsync(sigma2, s->dS2, sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
+    LB_CUDA(cudaMemcpyAsync(mu_minus_mean, s->dMu.get(), sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
+    LB_CUDA(cudaMemcpyAsync(sigma2, s->dS2.get(), sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
     LB_CUDA(cudaStreamSynchronize(s->st));
     return LB_OK;
 }
@@ -980,25 +893,20 @@ int lb_spgp_acq_argmax(const lb_spgp* sc, int acq_id, const double* acq_params, 
     if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
     std::lock_guard<std::mutex> lk(s->mu);
     if (!s->computed) return LB_ERR_STATE;
-    SP_DEVICE(s);
+    LB_DEVICE(s);
     int rc;
     if ((rc = ensure_query(s, Mq, Xq_rowmajor))) return rc;
     if ((rc = predict(s, Mq, optimized))) return rc;
+    ArgmaxWs& am = s->am;
     const double* dMean = nullptr;
     if (mean_at_q) {
-        LB_CUDA(cudaMemcpyAsync(s->dMeanQ, mean_at_q, sizeof(double) * Mq, cudaMemcpyHostToDevice, s->st));
-        dMean = s->dMeanQ;
+        LB_CUDA(cudaMemcpyAsync(am.mean.get(), mean_at_q, sizeof(double) * Mq, cudaMemcpyHostToDevice, s->st));
+        dMean = am.mean.get();
     }
-    if ((rc = lb_launch_acq_full(s->st, acq_id, acq_params[0], acq_params[1], Mq, s->dMu, 1, dMean, mean_const, s->dS2, s->dAcq, s->dBlk,
-             s->dBlkIdx, s->dBest, s->dBestIdx, &s->launches)))
+    if ((rc = lb_launch_acq_full(s->st, acq_id, acq_params[0], acq_params[1], Mq, s->dMu.get(), 1, dMean, mean_const, s->dS2.get(),
+             am.vals.get(), am.blk_val.get(), am.blk_idx.get(), am.best_val.get(), am.best_idx.get(), &s->launches)))
         return rc;
-    long long idx = 0;
-    LB_CUDA(cudaMemcpyAsync(best_val, s->dBest, sizeof(double), cudaMemcpyDeviceToHost, s->st));
-    LB_CUDA(cudaMemcpyAsync(&idx, s->dBestIdx, sizeof(long long), cudaMemcpyDeviceToHost, s->st));
-    if (acq_out) LB_CUDA(cudaMemcpyAsync(acq_out, s->dAcq, sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
-    LB_CUDA(cudaStreamSynchronize(s->st));
-    *best_idx = idx;
-    return LB_OK;
+    return am.read_best(s->st, best_val, best_idx, acq_out, Mq);
 }
 
 long long lb_spgp_launch_count(const lb_spgp* s) { return s ? s->launches + s->q->launches + s->a->launches : 0; }

@@ -763,19 +763,14 @@ int lb_tf32_prepare(lb_gp* h)
     if (!h->linv_valid && (rc = lb_launch_linv(h))) return rc;
     const int64_t Np = h->Np, Nr = (Np + BN - 1) / BN * BN;
     const size_t esz = split ? 4 : (f16 ? 2 : 4); // split: two fp16 planes of Nr x Np
-    if (!h->dLinv32 || h->linv32_rows != Nr) {
-        lb_dfree_sync(h, h->dLinv32);
-        h->dLinv32 = nullptr;
-        LB_ALLOC(h, h->dLinv32, esz * Nr * Np);
-        h->linv32_rows = Nr;
-    }
+    if ((rc = h->dLinv32.resize(h, esz * Nr * Np))) return rc;
     double scale = 1.0;
     if (f16) {
         if ((rc = lb_ensure_scratch(h, sizeof(double) * 1024))) return rc;
-        absmax_kernel<<<1024, 256, 0, h->stream>>>(h->dLinv, Np * Np, h->dScratch);
+        absmax_kernel<<<1024, 256, 0, h->stream>>>(h->dLinv.get(), Np * Np, h->dScratch.get());
         h->launches++;
         double part[1024];
-        LB_CUDA(cudaMemcpyAsync(part, h->dScratch, sizeof(part), cudaMemcpyDeviceToHost, h->stream));
+        LB_CUDA(cudaMemcpyAsync(part, h->dScratch.get(), sizeof(part), cudaMemcpyDeviceToHost, h->stream));
         LB_CUDA(cudaStreamSynchronize(h->stream));
         double mx = 0.0;
         for (double v : part) mx = v > mx ? v : mx;
@@ -783,21 +778,16 @@ int lb_tf32_prepare(lb_gp* h)
         scale = std::ldexp(1.0, 14 - (int)std::ceil(std::log2(mx)));
     }
     h->linv32_scale = scale;
-    __half* lo_plane = split ? reinterpret_cast<__half*>(h->dLinv32) + Nr * Np : nullptr;
-    if (split) LB_CUDA(cudaMemsetAsync(h->dLinv32, 0, esz * Nr * Np, h->stream)); // both planes incl. the padding rows
-    else if (Nr > Np) LB_CUDA(cudaMemsetAsync((char*)h->dLinv32 + esz * Np * Np, 0, esz * (Nr - Np) * Np, h->stream));
+    __half* lo_plane = split ? reinterpret_cast<__half*>(h->dLinv32.get()) + Nr * Np : nullptr;
+    if (split) LB_CUDA(cudaMemsetAsync(h->dLinv32.get(), 0, esz * Nr * Np, h->stream)); // both planes incl. the padding rows
+    else if (Nr > Np) LB_CUDA(cudaMemsetAsync((char*)h->dLinv32.get() + esz * Np * Np, 0, esz * (Nr - Np) * Np, h->stream));
     dim3 grid((unsigned)(Np / 32), (unsigned)(Np / 32));
     LbProfScope ps(h, h->stream, LB_PC_OTHER);
-    if (f16) linv_to_rowmajor_kernel<true><<<grid, 256, 0, h->stream>>>(h->dLinv, Np, h->dLinv32, Np, scale, lo_plane);
-    else linv_to_rowmajor_kernel<false><<<grid, 256, 0, h->stream>>>(h->dLinv, Np, h->dLinv32, Np, 1.0, nullptr);
+    if (f16) linv_to_rowmajor_kernel<true><<<grid, 256, 0, h->stream>>>(h->dLinv.get(), Np, h->dLinv32.get(), Np, scale, lo_plane);
+    else linv_to_rowmajor_kernel<false><<<grid, 256, 0, h->stream>>>(h->dLinv.get(), Np, h->dLinv32.get(), Np, 1.0, nullptr);
     h->launches++;
-    if (!h->dLinvW || h->linvw_np != Np) {
-        lb_dfree_sync(h, h->dLinvW);
-        h->dLinvW = nullptr;
-        LB_ALLOC(h, h->dLinvW, sizeof(double) * Np);
-        h->linvw_np = Np;
-    }
-    colnorm2_kernel<<<(unsigned)Np, 256, 0, h->stream>>>(h->dLinv, Np, h->dLinvW); // weights of the rounding-bias correction
+    if ((rc = h->dLinvW.resize(h, sizeof(double) * Np))) return rc;
+    colnorm2_kernel<<<(unsigned)Np, 256, 0, h->stream>>>(h->dLinv.get(), Np, h->dLinvW.get()); // weights of the rounding-bias correction
     h->launches++;
     LB_CUDA(cudaGetLastError());
     h->linv32_valid = true;
@@ -824,10 +814,10 @@ int lb_dinv_absmax(lb_gp* h, const double* dV, int G, double* out)
     using namespace tf32q;
     int rc;
     if ((rc = lb_ensure_scratch(h, sizeof(double) * 1024))) return rc;
-    absmax_kernel<<<1024, 256, 0, h->stream>>>(dV, h->Np * lb_linv_columns_width(h, G), h->dScratch);
+    absmax_kernel<<<1024, 256, 0, h->stream>>>(dV, h->Np * lb_linv_columns_width(h, G), h->dScratch.get());
     h->launches++;
     double part[1024];
-    LB_CUDA(cudaMemcpyAsync(part, h->dScratch, sizeof(part), cudaMemcpyDeviceToHost, h->stream));
+    LB_CUDA(cudaMemcpyAsync(part, h->dScratch.get(), sizeof(part), cudaMemcpyDeviceToHost, h->stream));
     LB_CUDA(cudaStreamSynchronize(h->stream));
     double mx = 0.0;
     for (double v : part) mx = v > mx ? v : mx;
@@ -877,22 +867,12 @@ int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all)
     double scale;
     int rc = dinv_scale(h, absmax_all, &scale);
     if (rc) return rc;
-    if (!h->dLinv32 || h->linv32_rows != Nr) {
-        lb_dfree_sync(h, h->dLinv32);
-        h->dLinv32 = nullptr;
-        LB_ALLOC(h, h->dLinv32, esz * Nr * Np);
-        h->linv32_rows = Nr;
-    }
-    if (!h->dLinvW || h->linvw_np != Np) {
-        lb_dfree_sync(h, h->dLinvW);
-        h->dLinvW = nullptr;
-        LB_ALLOC(h, h->dLinvW, sizeof(double) * Np);
-        h->linvw_np = Np;
-    }
+    if ((rc = h->dLinv32.resize(h, esz * Nr * Np))) return rc;
+    if ((rc = h->dLinvW.resize(h, sizeof(double) * Np))) return rc;
     h->linv32_scale = scale;
     const size_t chunk = lb_dinv_chunk_bytes_impl(h, G), plane = dinv_plane_bytes(h, G);
     const char* all = reinterpret_cast<const char*>(dAll);
-    char* out = reinterpret_cast<char*>(h->dLinv32);
+    char* out = reinterpret_cast<char*>(h->dLinv32.get());
     LbProfScope ps(h, h->stream, LB_PC_OTHER);
     if (Nr > Np) { // padding rows of both planes
         LB_CUDA(cudaMemsetAsync(out + el * Np * Np, 0, el * (Nr - Np) * Np, h->stream));
@@ -900,7 +880,7 @@ int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all)
     }
     linv_unpermute_kernel<<<(unsigned)Np, 256, 0, h->stream>>>(all, chunk, 0, G, T, Np, ldr, (int)el, out);
     if (split) linv_unpermute_kernel<<<(unsigned)Np, 256, 0, h->stream>>>(all, chunk, plane, G, T, Np, ldr, (int)el, out + el * Nr * Np);
-    linvw_unpermute_kernel<<<(unsigned)((Np + 255) / 256), 256, 0, h->stream>>>(all, chunk, plane * (split ? 2 : 1), G, Np, h->dLinvW);
+    linvw_unpermute_kernel<<<(unsigned)((Np + 255) / 256), 256, 0, h->stream>>>(all, chunk, plane * (split ? 2 : 1), G, Np, h->dLinvW.get());
     h->launches += split ? 3 : 2;
     LB_CUDA(cudaGetLastError());
     h->linv32_valid = true;
@@ -925,7 +905,7 @@ int lb_launch_kstar_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, const doub
             if (ib <= ia || jb <= ja) return;
             const int64_t tiles = (ib - ia) * (jb - ja);
             kstar_t32_kernel<decltype(kid)::value, decltype(f16c)::value, decltype(edgec)::value, DCH_WIDE><<<(unsigned)tiles, 256, 0, st>>>(h->dXs, Np,
-                h->N, dQs, Mcp, Mc, dKt, Np, h->kp, h->dAlpha, h->P, dMuPart, ia, ja, ib - ia, jb - ja, dBias ? h->dLinvW : nullptr, dKtLo);
+                h->N, dQs, Mcp, Mc, dKt, Np, h->kp, h->dAlpha, h->P, dMuPart, ia, ja, ib - ia, jb - ja, dBias ? h->dLinvW.get() : nullptr, dKtLo);
             if (launches) ++*launches;
         };
         auto go_prec = [&](auto kid) {
@@ -960,7 +940,7 @@ int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mc
     using namespace tf32q;
     const bool split = (h->precision == 3);
     const bool f16 = (h->precision == 2) || split;
-    const int64_t Np = h->Np;
+    const int64_t Np = h->Np, Nr = (Np + BN - 1) / BN * BN; // rows of the copy (lb_tf32_prepare)
     const double kscale = f16 ? 1.0 / h->kp.sf2 : 1.0;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -969,10 +949,10 @@ int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mc
     int rc;
     if (split) { // hi / lo planes, three MMAs per k-step, fp64 combination and norm (dNorm2 holds Mcp doubles)
         const __half* Ah = reinterpret_cast<const __half*>(dKt);
-        const __half* Bh = reinterpret_cast<const __half*>(h->dLinv32);
+        const __half* Bh = reinterpret_cast<const __half*>(h->dLinv32.get());
         {
             LbProfScope ps(h, st, LB_PC_QSTEP);
-            rc = lb_launch_split_gemm_norm(st, Ah, Ah + Mcp * Np, Np, Bh, Bh + h->linv32_rows * Np, Np, Mcp, h->linv32_rows, Np, 1,
+            rc = lb_launch_split_gemm_norm(st, Ah, Ah + Mcp * Np, Np, Bh, Bh + Nr * Np, Np, Mcp, Nr, Np, 1,
                 reinterpret_cast<double*>(dNorm2), dErr, sms);
         }
         if (rc) return rc;
@@ -983,7 +963,7 @@ int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mc
     }
     {
         LbProfScope ps(h, st, LB_PC_QSTEP);
-        rc = lb_launch_tf32_gemm_norm(st, dKt, Np, h->dLinv32, Np, Mcp, h->linv32_rows, Np, 1, dNorm2, nullptr, dErr, sms, f16);
+        rc = lb_launch_tf32_gemm_norm(st, dKt, Np, h->dLinv32.get(), Np, Mcp, Nr, Np, 1, dNorm2, nullptr, dErr, sms, f16);
     }
     if (rc) return rc;
     // u_r^2 for round-to-nearest with an 11-bit significand and log-uniform mantissas: (2^-22 / 3) * 0.541; both operands: x 2

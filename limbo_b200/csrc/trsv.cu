@@ -238,23 +238,19 @@ int lb_launch_trsv(lb_gp* h, double* dB, int nrhs, bool forward)
     }
     const int T = (int)(h->Np / LB_TILE);
     // scratch: the published solution blocks (NR columns of Np doubles), sentinel-filled per launch
-    if (!h->dTrsvX || h->trsvx_np != h->Np) {
-        lb_dfree_sync(h, h->dTrsvX);
-        h->dTrsvX = nullptr;
-        LB_ALLOC(h, h->dTrsvX, sizeof(double) * NR * h->Np);
-        h->trsvx_np = h->Np;
-    }
+    int rc = h->dTrsvX.resize(h, sizeof(double) * NR * h->Np);
+    if (rc) return rc;
     for (int p0 = 0; p0 < nrhs; p0 += NR) {
         const int nr = (nrhs - p0 < NR) ? (nrhs - p0) : NR;
-        LB_CUDA(cudaMemsetAsync(h->dFlags, 0, (T + 1) * sizeof(int), h->stream));
-        LB_CUDA(cudaMemsetAsync(h->dTrsvX, 0xFF, sizeof(double) * NR * h->Np, h->stream));
+        LB_CUDA(cudaMemsetAsync(h->dFlags.get(), 0, (T + 1) * sizeof(int), h->stream));
+        LB_CUDA(cudaMemsetAsync(h->dTrsvX.get(), 0xFF, sizeof(double) * NR * h->Np, h->stream));
         LbProfScope ps(h, h->stream, LB_PC_TRSV);
         if (forward)
-            trsv_fwd_kernel<<<T, 256, TRSV_SMEM, h->stream>>>(h->dL, h->Np, h->dInvD, dB + (int64_t)p0 * h->Np, h->Np, nr, T, h->dTrsvX,
-                h->dFlags + T, h->dInfo);
+            trsv_fwd_kernel<<<T, 256, TRSV_SMEM, h->stream>>>(h->dL, h->Np, h->dInvD, dB + (int64_t)p0 * h->Np, h->Np, nr, T, h->dTrsvX.get(),
+                h->dFlags.get() + T, h->dInfo.get());
         else
-            trsv_bwd_kernel<<<T, 256, TRSV_SMEM, h->stream>>>(h->dL, h->Np, h->dInvD, dB + (int64_t)p0 * h->Np, h->Np, nr, T, h->dTrsvX,
-                h->dFlags + T, h->dInfo);
+            trsv_bwd_kernel<<<T, 256, TRSV_SMEM, h->stream>>>(h->dL, h->Np, h->dInvD, dB + (int64_t)p0 * h->Np, h->Np, nr, T, h->dTrsvX.get(),
+                h->dFlags.get() + T, h->dInfo.get());
         h->launches++;
     }
     LB_CUDA(cudaGetLastError());
