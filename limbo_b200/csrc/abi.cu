@@ -382,8 +382,8 @@ int lb_destroy(lb_gp* hh)
     h->ex.ws = QueryWs{}; // the remaining private buffers go back with the handle (delete h)
     if (h->ex.hPoint) cudaFreeHost(h->ex.hPoint);
     for (cudaEvent_t e : h->ex.ev_eci) if (e) cudaEventDestroy(e);
-    for (cudaStream_t* ps : {&h->aux, &h->aux2, &h->aux3})
-        if (*ps) { cudaStreamSynchronize(*ps); cudaStreamDestroy(*ps); *ps = nullptr; }
+    for (cudaStream_t& s : h->group)
+        if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); s = nullptr; }
     Shell sh;
     sh.own = h->ex.own; sh.side = h->side;
     for (int i = 0; i < LB_NEV; ++i) sh.ev[i] = h->ev[i];
@@ -767,27 +767,19 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
     return check_info(h);
 }
 
-// Batches of at least this many candidates take the panel path (LB_QUERY_PANEL_MIN overrides).  The slab kernel keeps the
+// Batches of at least this many candidates take the panel path.  The slab kernel keeps the
 // one-point / small-batch latency, but its time does not shrink with the batch: every CTA streams all of L through L2 whatever
 // its slab width, while the panel path scales with the number of 128-candidate column tiles.  Measured on an H100 SXM at a 400 W
 // power limit, N = 16384, ms per batch of 32 / 64 / 128 / 256 / 512 candidates: slab path 86.1 for every size, panel path
 // 5.7 / 5.7 / 5.7 / 5.8 / 6.1: at this N the panel path wins from the smallest batch.  The default of 256 is not re-tuned:
 // batches at small N (the reference's own regime) have not been measured on H100, and below the threshold a batch is bit-identical
 // to one-point queries (query_point_kernel runs the slab body).
-static int64_t g_query_panel_min = -1;
-static int64_t query_panel_min()
-{
-    if (g_query_panel_min < 0) {
-        const char* e = getenv("LB_QUERY_PANEL_MIN");
-        int64_t v = e ? (int64_t)atoll(e) : 256;
-        g_query_panel_min = v < 1 ? 1 : v;
-    }
-    return g_query_panel_min;
-}
+static int64_t g_query_panel_min = 0; // 0: the default
+static int64_t query_panel_min() { return g_query_panel_min > 0 ? g_query_panel_min : 256; }
 // testing hook: batch size from which lb_query / lb_acq_argmax take the panel path (<= 0 restores the default)
 extern "C" int lb_debug_set_query_panel_min(long long m)
 {
-    g_query_panel_min = m > 0 ? (int64_t)m : -1;
+    g_query_panel_min = m > 0 ? (int64_t)m : 0;
     return LB_OK;
 }
 

@@ -19,7 +19,7 @@
 #include <vector>
 
 #define LB_TILE 128
-#define LB_NEV 8 // events per handle: fork / panel x2 / a-update x2 / join / second-group fork + join
+#define LB_NEV 6 // events per handle: Cholesky fork / panel x2 / a-update x2 / join (the panel query's fork and joins reuse 0..3)
 
 // ---- status codes (include/limbo_b200.h) ----------------------------------
 #define LB_OK 0
@@ -419,9 +419,8 @@ struct lb_gp {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
     cudaStream_t side = nullptr;   // high-priority stream for the look-ahead panel factorisation
-    cudaStream_t aux = nullptr;    // normal-priority second stream (panel query: second column group), created on first use
-    cudaStream_t aux2 = nullptr, aux3 = nullptr; // third / fourth column group of the panel query for small batches (created on first use)
-    cudaEvent_t ev[LB_NEV] = {};        // fork / panel / a-update / join events
+    cudaStream_t group[3] = {};    // streams of the panel query's second to fourth column groups, created on first use
+    cudaEvent_t ev[LB_NEV] = {};
 
     int64_t N = 0;   // live samples
     int64_t Np = 0;  // padded capacity (multiple of 128)

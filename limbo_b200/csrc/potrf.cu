@@ -12,7 +12,6 @@
 // A non-positive pivot is reported LAPACK-style through info (the reference
 // never checks Eigen's info(), SURVEY.md §5).
 #include "gemm.cuh"
-#include <cstdlib>
 
 namespace {
 
@@ -323,42 +322,38 @@ static inline int syrk_tiles(int T, int j0, int nc)
     return n;
 }
 
-// Right-looking factorisation with look-ahead, panels in QUADS of 128-column block columns (two pairs):
-//   side stream : pair(k)  = potf2(k) trsm(k) syrk[k -> col k+1] potf2(k+1) trsm(k+1)
-//                 a_in     = K=256 update of block columns k+2, k+3 with pair(k)            (inside the quad)
-//                 pair(k+2)
-//   main stream : a(q)     = K=512 update of the NEXT quad's four block columns with all four panels of this quad
-//                 b(q)     = K=512 update of everything right of them
-// quad(q+1) only needs a(q), so the latency-bound panel chain runs under b(q).  K=512 instead of the K=256 of round 1: every
-// trailing tile is loaded / stored half as often per flop (the C-tile prologue and store epilogue are what keeps a short-K GEMM
-// below the long-K kernels of this library: 0.76-0.84 against 0.90-0.92).  A tile's accumulator runs through the same sequence
-// of DMMAs as with two K=256 passes (the store / load in between does not round), so the factor is bit-identical to the
-// pair-wise distributed factorisation below (tests/test_gpu_dist_fit.py, tests/test_gpu_multirank.py).
-// LB_POTRF_QUAD=0 restores the pair scheme.
-static int launch_pair_panel(lb_gp* h, cudaStream_t side, int k, int T, int64_t ld)
+// syrk_kernel over the block columns [j0, j0 + nc) with the panel block columns [kb, kb + kd)
+static void launch_syrk(cudaStream_t st, double* L, int64_t ld, int kb, int kd, int j0, int nc, int T)
+{
+    syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nc) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, st>>>(L, ld, kb, kd, j0, nc, T);
+}
+
+// Pair panel (k, k + 1): potf2(k) trsm(k) syrk[k -> col k+1] (K = 128) potf2(k+1), and trsm(k+1) when k + 2 < T.  L, invD and
+// info are the bases from which the kernels address block (i, k) and the diagonal-block inverse k.
+static int launch_pair_panel(lb_gp* h, cudaStream_t st, double* L, double* invD, int* info, int64_t ld, int k, int T)
 {
     {
-        LbProfScope ps(h, side, LB_PC_POTF2);
-        potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo.get(), 1);
+        LbProfScope ps(h, st, LB_PC_POTF2);
+        potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(L, ld, k, invD, info, 1);
     }
     h->launches++;
     if (k + 1 < T) {
         {
-            LbProfScope ps(h, side, LB_PC_TRSM_PANEL);
-            trsm_panel_kernel<<<T - k - 1, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, side>>>(h->dL, ld, k, h->dInvD);
+            LbProfScope ps(h, st, LB_PC_TRSM_PANEL);
+            trsm_panel_kernel<<<T - k - 1, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, st>>>(L, ld, k, invD);
         }
         {
-            LbProfScope ps(h, side, LB_PC_SYRK_COL);
-            syrk_kernel<SyrkCfg><<<(T - k - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 1, k + 1, 1, T);
+            LbProfScope ps(h, st, LB_PC_SYRK_COL);
+            launch_syrk(st, L, ld, k, 1, k + 1, 1, T);
         }
         {
-            LbProfScope ps(h, side, LB_PC_POTF2);
-            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo.get(), 1);
+            LbProfScope ps(h, st, LB_PC_POTF2);
+            potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(L, ld, k + 1, invD, info, 1);
         }
         h->launches += 3;
         if (k + 2 < T) {
-            LbProfScope ps(h, side, LB_PC_TRSM_PANEL);
-            trsm_panel_kernel<<<T - k - 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, side>>>(h->dL, ld, k + 1, h->dInvD);
+            LbProfScope ps(h, st, LB_PC_TRSM_PANEL);
+            trsm_panel_kernel<<<T - k - 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, st>>>(L, ld, k + 1, invD);
             h->launches++;
         }
     }
@@ -366,8 +361,21 @@ static int launch_pair_panel(lb_gp* h, cudaStream_t side, int k, int T, int64_t 
     return LB_OK;
 }
 
-static int launch_potrf_quads(lb_gp* h)
+// Right-looking factorisation with look-ahead, panels in QUADS of 128-column block columns (two pairs):
+//   side stream : pair(k)  = potf2(k) trsm(k) syrk[k -> col k+1] potf2(k+1) trsm(k+1)
+//                 a_in     = K=256 update of block columns k+2, k+3 with pair(k)            (inside the quad)
+//                 pair(k+2)
+//   main stream : a(q)     = K=512 update of the NEXT quad's four block columns with all four panels of this quad
+//                 b(q)     = K=512 update of everything right of them
+// quad(q+1) only needs a(q), so the latency-bound panel chain runs under b(q).  With K=512 every trailing tile is loaded /
+// stored half as often per flop as with K=256 (the C-tile prologue and store epilogue are what keeps a short-K GEMM below the
+// long-K kernels of this library: 0.76-0.84 against 0.90-0.92).  A tile's accumulator runs through the same sequence of DMMAs
+// as with two K=256 passes (the store / load in between does not round), so the factor is bit-identical to the pair-wise
+// distributed factorisation below (tests/test_gpu_dist_fit.py, tests/test_gpu_multirank.py).
+int lb_launch_potrf(lb_gp* h)
 {
+    int rc = set_attrs();
+    if (rc) return rc;
     const int T = (int)(h->Np / LB_TILE);
     const int64_t ld = h->Np;
     cudaStream_t main = h->stream, side = h->side ? h->side : h->stream;
@@ -376,18 +384,18 @@ static int launch_potrf_quads(lb_gp* h)
         LB_CUDA(cudaEventRecord(h->ev[0], main)); // inputs (K) ready
         LB_CUDA(cudaStreamWaitEvent(side, h->ev[0], 0));
     }
-    int rc, q = 0;
+    int q = 0;
     for (int k = 0; k < T; k += 4, ++q) {
         // ---- quad(q) on the side stream ----
-        if ((rc = launch_pair_panel(h, side, k, T, ld))) return rc;
+        if ((rc = launch_pair_panel(h, side, h->dL, h->dInvD, h->dInfo.get(), ld, k, T))) return rc;
         if (k + 2 < T) {
             const int nc2 = (T - (k + 2) < 2) ? (T - (k + 2)) : 2;
             {
                 LbProfScope ps(h, side, LB_PC_SYRK_COL);
-                syrk_kernel<SyrkCfg><<<syrk_tiles(T, k + 2, nc2) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 2, k + 2, nc2, T);
+                launch_syrk(side, h->dL, ld, k, 2, k + 2, nc2, T);
             }
             h->launches++;
-            if ((rc = launch_pair_panel(h, side, k + 2, T, ld))) return rc;
+            if ((rc = launch_pair_panel(h, side, h->dL, h->dInvD, h->dInfo.get(), ld, k + 2, T))) return rc;
         }
         if (k + 4 >= T) break;
         if (side != main) {
@@ -399,7 +407,7 @@ static int launch_potrf_quads(lb_gp* h)
         const int nca = (T - j0 < 4) ? (T - j0) : 4;
         {
             LbProfScope ps(h, main, LB_PC_SYRK);
-            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nca) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0, nca, T);
+            launch_syrk(main, h->dL, ld, k, 4, j0, nca, T);
         }
         h->launches++;
         if (side != main) {
@@ -410,7 +418,7 @@ static int launch_potrf_quads(lb_gp* h)
         const int ncb = T - j0 - nca;
         if (ncb > 0) {
             LbProfScope ps(h, main, LB_PC_SYRK);
-            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0 + nca, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 4, j0 + nca, ncb, T);
+            launch_syrk(main, h->dL, ld, k, 4, j0 + nca, ncb, T);
             h->launches++;
         }
     }
@@ -422,130 +430,9 @@ static int launch_potrf_quads(lb_gp* h)
     return LB_OK;
 }
 
-// Pair scheme of round 1 (K = 256 trailing updates), kept behind LB_POTRF_QUAD=0:
-//   side stream : panel(p)  = potf2(k) trsm(k) syrk[k -> col k+1] potf2(k+1) trsm(k+1)
-//   main stream : a(p)      = K=256 update of the next pair's two block columns (k+2, k+3)
-//                 b(p)      = K=256 update of everything right of them
-// panel(p+1) only needs a(p), so the latency-bound panel work runs under b(p).
-int lb_launch_potrf(lb_gp* h)
-{
-    int rc = set_attrs();
-    if (rc) return rc;
-    static int quad = -1;
-    if (quad < 0) { const char* e = getenv("LB_POTRF_QUAD"); quad = (e && atoi(e) == 0) ? 0 : 1; }
-    if (quad) return launch_potrf_quads(h);
-    const int T = (int)(h->Np / LB_TILE);
-    const int64_t ld = h->Np;
-    cudaStream_t main = h->stream, side = h->side ? h->side : h->stream;
-    // b(p) is split at a FIXED block column cstar into a left group (main stream) and a right group (second, normal-priority
-    // stream): a tile never changes group, so each group's stream order carries its tile dependencies, and the tail of one
-    // group's launch (partial last wave, plus SMs handed to the side-stream panel kernels) is filled by the other group's CTAs.
-    // Here the side-stream panel kernels already fill most of the tails, and the per-class launch timers would double count
-    // concurrent launches - so it is an experiment, OFF unless LB_POTRF_SPLIT=1.
-    static int split_on = -1;
-    if (split_on < 0) { const char* e = getenv("LB_POTRF_SPLIT"); split_on = (e && atoi(e) != 0) ? 1 : 0; }
-    cudaStream_t second = main;
-    if (split_on && T >= 24 && side != main) {
-        if (!h->aux && cudaStreamCreateWithFlags(&h->aux, cudaStreamNonBlocking) != cudaSuccess) h->aux = nullptr;
-        if (h->aux) second = h->aux;
-    }
-    const int cstar = (second != main) ? (((int)(0.38 * T)) & ~1) : T; // even: a pair (k, k + 1) never straddles the boundary // left group: columns < cstar (long columns), right: >= cstar; ~equal tile counts at the start
-    LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), main));
-    if (side != main) {
-        LB_CUDA(cudaEventRecord(h->ev[0], main)); // inputs (K) ready
-        LB_CUDA(cudaStreamWaitEvent(side, h->ev[0], 0));
-        if (second != main) LB_CUDA(cudaStreamWaitEvent(second, h->ev[0], 0));
-    }
-    int p = 0;
-    for (int k = 0; k < T; k += 2, ++p) {
-        const bool pair = (k + 1 < T);
-        // ---- panel(p) on the side stream ----
-        {
-            LbProfScope ps(h, side, LB_PC_POTF2);
-            potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k, h->dInvD, h->dInfo.get(), 1);
-        }
-        h->launches++;
-        if (pair) {
-            {
-                LbProfScope ps(h, side, LB_PC_TRSM_PANEL);
-                trsm_panel_kernel<<<T - k - 1, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, side>>>(h->dL, ld, k, h->dInvD);
-            }
-            {
-                LbProfScope ps(h, side, LB_PC_SYRK_COL);
-                syrk_kernel<SyrkCfg><<<(T - k - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, side>>>(h->dL, ld, k, 1, k + 1, 1, T);
-            }
-            {
-                LbProfScope ps(h, side, LB_PC_POTF2);
-                potf2_inv_kernel<<<1, 256, POTF2_SMEM, side>>>(h->dL, ld, k + 1, h->dInvD, h->dInfo.get(), 1);
-            }
-            h->launches += 3;
-            if (k + 2 < T) {
-                LbProfScope ps(h, side, LB_PC_TRSM_PANEL);
-                trsm_panel_kernel<<<T - k - 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, side>>>(h->dL, ld, k + 1, h->dInvD);
-                h->launches++;
-            }
-        }
-        if (k + 2 >= T) break;
-        if (side != main) {
-            LB_CUDA(cudaEventRecord(h->ev[1 + (p & 1)], side));
-            LB_CUDA(cudaStreamWaitEvent(main, h->ev[1 + (p & 1)], 0));
-        }
-        // ---- a(p): the next pair's block columns ----
-        const int j0 = k + 2;
-        const int nca = (T - j0 < 2) ? (T - j0) : 2;
-        // once the factorisation has passed cstar the look-ahead columns belong to the right group: hand over to the second stream
-        // for good (its earlier updates of these tiles precede in stream order; main has nothing left)
-        cudaStream_t sa = (second != main && j0 >= cstar) ? second : main;
-        if (sa != main && side != main) LB_CUDA(cudaStreamWaitEvent(sa, h->ev[1 + (p & 1)], 0));
-        {
-            LbProfScope ps(h, sa, LB_PC_SYRK);
-            syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nca) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, sa>>>(h->dL, ld, k, 2, j0, nca, T);
-        }
-        h->launches++;
-        if (side != main) {
-            LB_CUDA(cudaEventRecord(h->ev[3 + (p & 1)], sa));
-            LB_CUDA(cudaStreamWaitEvent(side, h->ev[3 + (p & 1)], 0));
-        }
-        // ---- b(p): the rest of the trailing matrix ----
-        const int jb = j0 + nca;
-        if (sa == main && second != main) {
-            const int left_end = cstar < jb ? jb : cstar; // columns [jb, left_end) on main, [left_end, T) on the second stream
-            if (left_end > jb) {
-                LbProfScope ps(h, main, LB_PC_SYRK);
-                syrk_kernel<SyrkCfg><<<syrk_tiles(T, jb, left_end - jb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, main>>>(h->dL, ld, k, 2, jb, left_end - jb, T);
-                h->launches++;
-            }
-            if (T - left_end > 0) {
-                if (side != main) LB_CUDA(cudaStreamWaitEvent(second, h->ev[1 + (p & 1)], 0)); // the panel it multiplies with
-                LbProfScope ps(h, second, LB_PC_SYRK);
-                syrk_kernel<SyrkCfg><<<syrk_tiles(T, left_end, T - left_end) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, second>>>(h->dL, ld, k, 2, left_end, T - left_end, T);
-                h->launches++;
-            }
-        }
-        else {
-            const int ncb = T - jb;
-            if (ncb > 0) {
-                LbProfScope ps(h, sa, LB_PC_SYRK);
-                syrk_kernel<SyrkCfg><<<syrk_tiles(T, jb, ncb) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, sa>>>(h->dL, ld, k, 2, jb, ncb, T);
-                h->launches++;
-            }
-        }
-    }
-    if (side != main) { // join
-        LB_CUDA(cudaEventRecord(h->ev[5], side));
-        LB_CUDA(cudaStreamWaitEvent(main, h->ev[5], 0));
-    }
-    if (second != main) {
-        LB_CUDA(cudaEventRecord(h->ev[6], second));
-        LB_CUDA(cudaStreamWaitEvent(main, h->ev[6], 0));
-    }
-    LB_CUDA(cudaGetLastError());
-    return LB_OK;
-}
-
 // =====================================================================================================================
 // Multi-GPU Cholesky (BASELINE.json config 5, SURVEY.md §8e "stretch"): building blocks for a 1-D block-cyclic
-// right-looking factorisation over 256-column panels ("pairs" of 128-blocks, the same pair structure as lb_launch_potrf).
+// right-looking factorisation over 256-column panels ("pairs" of 128-blocks, the pairs lb_launch_potrf's quads are made of).
 // Pair p (global 128-block columns 2p, 2p+1) lives on rank p mod G; a rank stores its pairs side by side, full height:
 //   local 128-block column l  <->  global block column  j(l) = 2 * (G * (l / 2) + rank) + (l & 1)
 // One step = owner factors its pair (potf2, trsm, K=128 column update, potf2, trsm: the kernels above on its local
@@ -680,17 +567,12 @@ int lb_dchol_panel(lb_gp* h, double* dCols, int64_t Nd, int kpair, double* dInvD
     // the kernels above address block (i, k) as L + i*128 + k*128*ld: shift the bases so that block column kpair is dCols
     double* Lb = dCols - (int64_t)kpair * LB_TILE * Nd;
     double* Ib = dInvD - (int64_t)kpair * LB_TILE * LB_TILE;
-    potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(Lb, Nd, kpair, Ib, dInfo, 1);
-    trsm_panel_kernel<<<T - kpair - 1, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, st>>>(Lb, Nd, kpair, Ib);
-    syrk_kernel<SyrkCfg><<<(T - kpair - 1) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, st>>>(Lb, Nd, kpair, 1, kpair + 1, 1, T);
-    potf2_inv_kernel<<<1, 256, POTF2_SMEM, st>>>(Lb, Nd, kpair + 1, Ib, dInfo, 1);
-    h->launches += 4;
+    if ((rc = launch_pair_panel(h, st, Lb, Ib, dInfo, Nd, kpair, T))) return rc;
     if (kpair + 2 < T) {
-        trsm_panel_kernel<<<T - kpair - 2, lbg::CfgWide::THREADS, lbg::CfgWide::PIPE_BYTES, st>>>(Lb, Nd, kpair + 1, Ib);
         const int64_t ldp = Nd - (int64_t)(kpair + 2) * LB_TILE;
         dim3 grid((unsigned)((ldp + 255) / 256), 2 * LB_TILE);
         dchol_pack_kernel<<<grid, 256, 0, st>>>(dCols, Nd, (int64_t)(kpair + 2) * LB_TILE, dPanel, ldp);
-        h->launches += 2;
+        h->launches++;
     }
     LB_CUDA(cudaGetLastError());
     return LB_OK;

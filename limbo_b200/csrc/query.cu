@@ -9,7 +9,6 @@
 //                                           -> acq_kernel + argmax reduction
 #include "gemm.cuh"
 #include <cfloat>
-#include <cstdlib>
 
 namespace {
 
@@ -797,7 +796,7 @@ LbOncePerDevice g_attr_once2;
 } // namespace slab
 
 // ===========================================================================
-// Panel path for large candidate batches (M >= LB_QUERY_PANEL_MIN): V = L^-1 K* as a blocked solve over super-blocks of
+// Panel path for large candidate batches (M >= 256, abi.cu query_panel_min): V = L^-1 K* as a blocked solve over super-blocks of
 // SB = 16 row tiles (2048 rows), everything on the GEMM core of gemm.cuh with long K ranges:
 //     update_s :  T_s   = K*_s - L[s, 0:s] V[0:s]            (SB x Mp/128 tiles of 128 x 128, K = s * 2048)
 //     solve_s  :  V_s   = inv(L_ss) T_s                      (same tiles, K = (i + 1) * 128: inv(L_ss) is lower triangular)
@@ -950,54 +949,25 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
     // The chain update_s -> solve_s -> update_s+1 -> ... only couples tiles of the SAME candidate column tile, so the column tiles
     // can walk it in groups on separate streams, the tail of one group's launch being filled by another group's CTAs.
     const int ctiles = (int)(Mp / LB_TILE);
-    static int split_pct = -1, use_side = -1;
-    if (split_pct < 0) {
-        const char* e = getenv("LB_PANEL_SPLIT");   // percentage of the column tiles in the first group; 100 = one stream
-        split_pct = e ? atoi(e) : 100; // see the group choice below
-        if (split_pct < 1 || split_pct > 100) split_pct = 100;
-        const char* e2 = getenv("LB_PANEL_SIDE");   // 1: second group on the high-priority side stream instead of a normal-priority one
-        use_side = (e2 && atoi(e2) != 0) ? 1 : 0;
-    }
     constexpr int wmul = LB_TILE / CD::BN; // 64-wide column tiles per 128 candidates
-    // Groups of column tiles, each walking the chain on its own stream.  A launch of all column tiles under one round of the machine
-    // (M = 640 at N = 16384: 160 CTAs for 264 slots): four equal groups, so that the groups, drifting apart, keep the SMs full.
-    // Otherwise one stream, unless LB_PANEL_SPLIT=<1..99> asks for two groups (that percentage / the rest).  LB_PANEL_GROUPS=<1..4>
-    // forces the count.  Measured on an H100 SXM at a 400 W power limit, N = 16384, ms per batch (process-to-process spread up to
-    // ~10 % at that limit): M = 10^4: one stream 121.9, 90 / 80 / 70 / 60 / 50 % splits 120.8 / 130.3 / 131.5 / 130.9 / 132.0;
-    // 1 / 2 / 3 / 4 groups: M = 640: 10.9 / 10.1 / 9.6 / 9.1, 1250: 16.3 / 15.2 / 15.5 / 16.0, 2500: 28.9 / 28.1 / 30.9 / 30.9.
-    // Results do not depend on the grouping (every tile's arithmetic is unchanged).
-    static int force_groups = -1;
-    if (force_groups < 0) { const char* e = getenv("LB_PANEL_GROUPS"); force_groups = e ? atoi(e) : 0; }
+    // Four equal groups, each walking the chain on its own stream, when a launch of all column tiles is under one round of the
+    // machine (M = 640 at N = 16384: 160 CTAs for 264 slots), so that the groups, drifting apart, keep the SMs full; otherwise
+    // one stream.  Measured on an H100 SXM at a 400 W power limit, N = 16384, ms per batch (process-to-process spread up to ~10 %
+    // at that limit), 1 / 2 / 3 / 4 groups: M = 640: 10.9 / 10.1 / 9.6 / 9.1, 1250: 16.3 / 15.2 / 15.5 / 16.0, 2500: 28.9 / 28.1 /
+    // 30.9 / 30.9; M = 10^4: one stream 121.9, two groups of 90 / 80 / 70 / 60 / 50 % of the column tiles 120.8 / 130.3 / 131.5 /
+    // 130.9 / 132.0.  Results do not depend on the grouping (every tile's arithmetic is unchanged).
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const int slots = sms * CD::CTAS_PER_SM;
-    int ngroups = 1;
-    if (ctiles >= 4 && (int64_t)ctiles * wmul * SB < (int64_t)slots) ngroups = 4;
-    else if (split_pct < 100 && ctiles >= 4) ngroups = 2;
-    if (force_groups >= 1 && force_groups <= 4) ngroups = force_groups;
-    if (ngroups > ctiles) ngroups = ctiles;
+    int ngroups = (ctiles >= 4 && (int64_t)ctiles * wmul * SB < (int64_t)slots) ? 4 : 1;
     cudaStream_t sts[4] = {st, st, st, st};
-    if (ngroups >= 2) {
-        if (use_side && h->side && ngroups == 2) sts[1] = h->side;
-        else {
-            cudaStream_t* extra[3] = {&h->aux, &h->aux2, &h->aux3};
-            for (int g = 1; g < ngroups; ++g) {
-                if (!*extra[g - 1] && cudaStreamCreateWithFlags(extra[g - 1], cudaStreamNonBlocking) != cudaSuccess) *extra[g - 1] = nullptr;
-                if (!*extra[g - 1]) { ngroups = g; break; } // no stream: fewer groups
-                sts[g] = *extra[g - 1];
-            }
-        }
+    for (int g = 1; g < ngroups; ++g) {
+        if (!h->group[g - 1] && cudaStreamCreateWithFlags(&h->group[g - 1], cudaStreamNonBlocking) != cudaSuccess) h->group[g - 1] = nullptr;
+        if (!h->group[g - 1]) { ngroups = g; break; } // no stream: fewer groups
+        sts[g] = h->group[g - 1];
     }
-    int gbeg[5] = {0, ctiles, ctiles, ctiles, ctiles}; // first column tile (128 wide) of each group
-    if (ngroups == 2) {
-        int split = (ctiles * split_pct + 50) / 100;
-        if (split < 1) split = 1;
-        if (split > ctiles - 1) split = ctiles - 1;
-        gbeg[1] = split;
-    }
-    else
-        for (int g = 1; g < ngroups; ++g) gbeg[g] = (int)((int64_t)ctiles * g / ngroups);
-    gbeg[ngroups] = ctiles;
+    int gbeg[5]; // first column tile (128 wide) of each group
+    for (int g = 0; g <= ngroups; ++g) gbeg[g] = (int)((int64_t)ctiles * g / ngroups);
     {
         LbProfScope ps(h, st, LB_PC_QSTEP);
         if (ngroups >= 2) {

@@ -427,44 +427,3 @@ def factor_outputs(h: Handle, case: ExactCase, X) -> dict:
     assert info == 0, info
     h.refit_alpha(case.Y)
     return dict(L=h.get(1), alpha=h.get(2), kinv=h.get(3))
-
-
-# cases of the schedule-variant runs: (N, P, seed); T = 5, 9, 13, 24, 26, 33
-SCHEDULE_CASES = [(640, 2, 11), (1025, 1, 12), (1663, 3, 13), (3072, 1, 14), (3327, 2, 15), (4224, 1, 16)]
-PANEL_CASES = [(2048, 1, 21), (4097, 2, 22)]  # T = 16, 33
-PANEL_M = (640, 1000, 2049)
-
-
-def schedule_outputs(lib) -> dict:
-    """Everything the schedule-variant runs compare, as a flat dict of arrays (same seeds in every process)."""
-    out = {}
-    h = Handle(lib)
-    try:
-        for N, P, seed in SCHEDULE_CASES:
-            case = ExactCase(N, P, seed)
-            X = np.random.default_rng(seed).uniform(0.0, 1.0, size=(N, 2))
-            r = factor_outputs(h, case, X)
-            for k, v in r.items():
-                out[f"potrf_{N}_{k}"] = v
-        for N, P, seed in PANEL_CASES:
-            qc = QueryCase(N, 3, P, seed)
-            p = kernel_params(1, 3, qc.rng)
-            Xq = qc.rng.uniform(0.0, 1.0, size=(max(PANEL_M), 3))
-            L, _, _, _, _ = qc.reference(1, p, 0.01, Xq)
-            h.set_data(qc.X, np.zeros((N, P)))
-            h.set_kernel(1, p, 0.01)
-            h.load_factor(L, qc.alpha)
-            for M in PANEL_M:
-                mu, s2 = h.query(Xq[:M])
-                out[f"panel_{N}_{M}_mu"], out[f"panel_{N}_{M}_s2"] = mu, s2
-    finally:
-        h.close()
-    return out
-
-
-if __name__ == "__main__":  # python tests/linalg_exact.py OUT.npz: schedule_outputs of this process's settings
-    import os
-    import sys
-    sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    from limbo_b200 import _lib as _L
-    np.savez(sys.argv[1], **schedule_outputs(_L.load()))

@@ -4,9 +4,6 @@ nca < 4, ncb == 0, every T mod 4) and of the recursive trtri (short last problem
 ragged 16-tile super-blocks of the panel query, N mod 128 in {0, 1, 127} the edge tiles.  Every bar is a first-order
 rounding-error bound; each case prints its observed / bound ratio."""
 import math
-import os
-import subprocess
-import sys
 import threading
 
 import numpy as np
@@ -15,9 +12,6 @@ import pytest
 import linalg_exact as E
 
 pytestmark = pytest.mark.gpu
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 
 EXACT = E.exact_shapes()
 RATIOS = {}
@@ -176,7 +170,7 @@ def test_query_multi_launch_from_shape(handle, T, what):
                  f"[T={T} {what}]")
 
 
-# ---- schedules, races, pivots ----------------------------------------------------------------------------------------
+# ---- repeatability, races, grouping, pivots --------------------------------------------------------------------------
 def test_factor_repeatable_across_calls_and_handles(lib):
     case = E.ExactCase(128 * 9 - 1, 2, 77)
     X = np.random.default_rng(78).uniform(0.0, 1.0, size=(case.N, 2))
@@ -221,37 +215,48 @@ def test_concurrent_factorisations_match_sequential(lib):
             h.close()
 
 
-def _variant_run(tmp_path, name, env_extra):
-    env = {k: v for k, v in os.environ.items() if not k.startswith(("LB_POTRF_", "LB_PANEL_", "LB_QUERY_PANEL_MIN"))}
-    env.update(env_extra)
-    out = tmp_path / f"{name}.npz"
-    r = subprocess.run([sys.executable, os.path.join(HERE, "linalg_exact.py"), str(out)], env=env, cwd=ROOT,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    return dict(np.load(out))
+@pytest.mark.parametrize("N,P,seed", [(2048, 1, 21), (4097, 2, 22)], ids=["T16", "T33"])
+def test_panel_grouping_bit_identical(handle, lib, N, P, seed):
+    """The panel query walks its candidate column tiles in four stream groups when a launch of all of them is under one
+    round of the machine, otherwise on one stream.  Nested prefixes of one candidate set on either side of that rule give
+    bit-identical mu and sigma^2 for the shared candidates: the grouping does not change any tile's arithmetic, and a
+    candidate's value does not depend on the batch it is in."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    slots = 2 * sms  # CfgDual: two CTAs per SM
+    per_ct = 2 * 16  # CTAs per 128-candidate column tile in one launch: two 64-wide tiles x a 16-row-tile super-block
 
+    def groups(M):
+        ct = -(-M // 128)
+        return 4 if ct >= 4 and ct * per_ct < slots else 1
 
-@pytest.fixture(scope="module")
-def default_schedule(tmp_path_factory):
-    return _variant_run(tmp_path_factory.mktemp("sched"), "default", {})
+    m4 = (slots - 1) // per_ct * 128  # the largest batch that takes four groups
+    m1 = m4 + 1                       # the smallest batch above it, on one stream
+    mid = (4 * 128 + m4) // 2 - 3     # a ragged batch with four uneven groups
+    sizes = (m1, m4, mid)
+    assert [groups(M) for M in sizes] == [1, 4, 4], (sms, sizes)
+    assert min(sizes) >= 256  # all on the panel path
 
-
-@pytest.mark.parametrize("name,env", [
-    ("pairs", {"LB_POTRF_QUAD": "0"}),
-    ("pairs_split", {"LB_POTRF_QUAD": "0", "LB_POTRF_SPLIT": "1"}),
-    ("panel_groups1", {"LB_PANEL_GROUPS": "1"}),
-    ("panel_groups2", {"LB_PANEL_GROUPS": "2"}),
-    ("panel_groups3", {"LB_PANEL_GROUPS": "3"}),
-    ("panel_groups4", {"LB_PANEL_GROUPS": "4"}),
-    ("panel_split60", {"LB_PANEL_SPLIT": "60"}),
-])
-def test_schedule_variants_bit_identical(tmp_path, default_schedule, name, env):
-    """The pair scheme, its split trailing update (T >= 24 here), and every panel column-tile grouping give results
-    bit-identical to the default schedule (same DMMA sequence per tile, only the launch order differs)."""
-    got = _variant_run(tmp_path, name, env)
-    assert set(got) == set(default_schedule)
-    bad = [f"{k}: {E.worst_tile(got[k] - default_schedule[k])}" for k in sorted(got) if not np.array_equal(got[k], default_schedule[k])]
-    assert not bad, bad
+    qc = E.QueryCase(N, 3, P, seed)
+    p = E.kernel_params(1, 3, qc.rng)
+    Xq = qc.rng.uniform(0.0, 1.0, size=(m1, 3))
+    L, _, _, _, _ = qc.reference(1, p, 0.01, Xq)
+    handle.set_data(qc.X, np.zeros((N, P)))
+    handle.set_kernel(1, p, 0.01)
+    handle.load_factor(L, qc.alpha)
+    handle.query(Xq[:m1])  # builds the cached diagonal-block inverses, so every query below launches the same fixed kernels
+    T = -(-N // 128)
+    nsb = -(-T // 16)  # super-blocks
+    out, fixed = {}, set()
+    for M in sizes:
+        n0 = lib.lb_launch_count(handle.h)
+        out[M] = handle.query(Xq[:M])
+        # one update and one solve launch per super-block and group; the rest of the query launches the same for every M
+        fixed.add(lib.lb_launch_count(handle.h) - n0 - 2 * nsb * groups(M))
+    assert len(fixed) == 1, f"the launch count does not follow the grouping rule: {fixed}"
+    for M in sizes[1:]:
+        for k, (a, b) in enumerate(zip(out[M], out[m1])):
+            assert np.array_equal(a, b[:M]), f"M={M} {('mu', 'sigma2')[k]}: {E.worst_tile(a - b[:M])}"
 
 
 PIVOT_T = (1, 3, 5, 9)

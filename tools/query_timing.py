@@ -1,6 +1,5 @@
 """Times lb_acq_argmax_dev (UCB) for M candidates at N=16384 (panel / slab path as the library chooses).
-usage: python tools/query_timing.py [M ...]        (LB_PANEL_GROUPS / LB_PANEL_SPLIT / LB_QUERY_PANEL_MIN are read
-once per process)"""
+usage: python tools/query_timing.py [M ...]"""
 import ctypes as C, os, sys, numpy as np, torch
 sys.path.insert(0, os.getcwd())
 from limbo_b200 import _lib, kernel, mean, model, synth
@@ -22,5 +21,4 @@ for M in Ms:
     e0.record(st)
     for _ in range(5): q()
     e1.record(st); torch.cuda.synchronize()
-    print("M", M, "groups", os.environ.get("LB_PANEL_GROUPS"), "split", os.environ.get("LB_PANEL_SPLIT"), "panel_min",
-          os.environ.get("LB_QUERY_PANEL_MIN"), "query ms", e0.elapsed_time(e1) / 5, "best", dB.item(), dI.item())
+    print("M", M, "query ms", e0.elapsed_time(e1) / 5, "best", dB.item(), dI.item())
