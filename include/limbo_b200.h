@@ -129,6 +129,29 @@ int lb_acq_argmax(const lb_gp* h, int acq_id, const double* acq_params, int64_t 
 int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* dXq_rowmajor,
     const double* dMean_at_q, double mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
 
+/* Candidate gradients for M candidates (row-major M x D), extending lb_query with what the reference's gradient optimisers
+ * (opt/gradient_ascent.hpp, opt/adam.hpp, opt/rprop.hpp) ask of f(x, gradient), which acqui/ucb.hpp:83-90 and acqui/ei.hpp:85-116
+ * leave unimplemented (assert(!gradient)).  mu_minus_mean (M x P row-major, without mean(v)) and sigma2 (M, clamped + noise) are
+ * bit-identical to lb_query's on its large-batch path; dmu (M x D row-major) is the gradient of the first output of mu_minus_mean,
+ * dsigma2 (M x D) that of sigma2, 0 where the clamp of gp.hpp:623 is active.  Any output may be NULL.  With N == 0 the gradients are
+ * 0.  fp64 handles only (LB_ERR_UNSUPPORTED otherwise); LB_ERR_ARG for M <= 0 or a non-finite coordinate.  May be called from
+ * several threads, as lb_query. */
+int lb_query_grad(const lb_gp* h, int64_t M, const double* Xq_rowmajor, double* mu_minus_mean, double* sigma2,
+    double* dmu, double* dsigma2);
+/* same, device pointers (the coordinates are not checked) */
+int lb_query_grad_dev(const lb_gp* h, int64_t M, const double* dXq_rowmajor, double* dMu_minus_mean, double* dSigma2,
+    double* dDmu, double* dDsigma2);
+/* Acquisition value (M) and gradient (M x D row-major) with the FirstElem aggregator, extending lb_acq_argmax (same acq_id and
+ * acq_params, same values on its large-batch path): UCB / GP_UCB grad = grad mu + params[0] grad sigma2 / (2 sqrt(sigma2)), EI
+ * (ei.hpp:85-116) grad = Phi(Z) grad mu + phi(Z) grad sigma with f_max and the jitter fixed, value and gradient 0 where
+ * sigma < 1e-10.  mean_at_q / mean_const as in lb_acq_argmax; mean_grad_at_q: M x D gradient of mean(v)'s first component, or NULL
+ * when the mean does not depend on v.  LB_ERR_ARG for M <= 0, a non-finite coordinate or an unknown acq_id; fp64 handles only. */
+int lb_acq_grad(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* Xq_rowmajor,
+    const double* mean_at_q, double mean_const, const double* mean_grad_at_q, double* acq_out, double* grad_out);
+/* same, device pointers except acq_params (the coordinates are not checked) */
+int lb_acq_grad_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* dXq_rowmajor,
+    const double* dMean_at_q, double mean_const, const double* dMean_grad_at_q, double* dAcq_out, double* dGrad_out);
+
 /* experimental/acqui/eci.hpp:76-107 over an objective and a constraint model, FirstElem aggregator:
  *   ECI = Pf * EI,  EI as LB_ACQ_EI on obj,  Pf = Phi((mu_c[0] - 1) / sigma_c) on con (eci.hpp:116-130).
  * eci_params = {f_max, jitter}; con may be NULL (no constraints: Pf = 1), as may a con without samples.  An obj without samples

@@ -24,6 +24,7 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <vector>
 
 #include <Eigen/Core>
@@ -36,6 +37,12 @@ namespace limbo {
         template <typename Params> struct MaternFiveHalves;
         template <typename Params> struct MaternThreeHalves;
         template <typename Params> struct Exp;
+    }
+    namespace mean {
+        template <typename Params> struct NullFunction;
+        template <typename Params> struct Constant;
+        template <typename Params> struct Data;
+        template <typename Params, typename MeanFunction> struct FunctionARD;
     }
 }
 
@@ -61,6 +68,15 @@ namespace limbo_b200 {
             static constexpr int id = LB_KERNEL_EXP;
             static void check() {}
         };
+
+        // Means whose value does not depend on the input: the candidate gradients (acq_grad, query_grad) add no mean term for them.
+        // FunctionARD is an affine map of its inner mean's value (mean/function_ard.hpp:88-92).  Other means have no input
+        // gradient here, and requesting one does not compile.
+        template <typename M> struct mean_is_input_free : std::false_type {};
+        template <typename P> struct mean_is_input_free<limbo::mean::NullFunction<P>> : std::true_type {};
+        template <typename P> struct mean_is_input_free<limbo::mean::Constant<P>> : std::true_type {};
+        template <typename P> struct mean_is_input_free<limbo::mean::Data<P>> : std::true_type {};
+        template <typename P, typename M> struct mean_is_input_free<limbo::mean::FunctionARD<P, M>> : mean_is_input_free<M> {};
 
         inline void lb_check(int rc, const char* where)
         {
@@ -161,7 +177,8 @@ namespace limbo_b200 {
                 }
             }
             // fused UCB / EI + argmax on the device with the FirstElem aggregator (bo_base.hpp:99-105)
-            std::pair<double, long> acq_argmax(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs) const
+            std::pair<double, long> acq_argmax(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs,
+                std::vector<double>* values = nullptr) const
             {
                 const long M = (long)vs.size();
                 const int D = (int)vs[0].size();
@@ -172,8 +189,58 @@ namespace limbo_b200 {
                 }
                 double params[2] = {p0, p1}, best = 0;
                 int64_t idx = 0;
-                lb_check(lb_acq_argmax(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, nullptr, &best, &idx), "lb_acq_argmax");
+                if (values) values->resize((size_t)M);
+                lb_check(lb_acq_argmax(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, values ? values->data() : nullptr, &best, &idx),
+                    "lb_acq_argmax");
                 return std::make_pair(best, (long)idx);
+            }
+            // UCB / EI values (M) and gradients (M x D) with the FirstElem aggregator in one device pass (lb_acq_grad): what the
+            // reference's gradient optimisers ask of acqui::UCB / EI (ucb.hpp:83-90, ei.hpp:85-116 assert(!gradient) there)
+            void acq_grad(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs, Eigen::VectorXd& values,
+                Eigen::MatrixXd& grads) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "acq_grad: the mean function has no input gradient");
+                const long M = (long)vs.size();
+                const int D = (int)vs[0].size();
+                std::vector<double> xq((size_t)M * D), mean0((size_t)M), v((size_t)M), g((size_t)M * D);
+                for (long i = 0; i < M; ++i) {
+                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
+                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
+                }
+                double params[2] = {p0, p1};
+                lb_check(lb_acq_grad(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, nullptr, v.data(), g.data()), "lb_acq_grad");
+                values = Eigen::VectorXd((Eigen::Index)M);
+                grads = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                for (long i = 0; i < M; ++i) {
+                    values(i) = v[(size_t)i];
+                    for (int d = 0; d < D; ++d) grads(i, d) = g[(size_t)i * D + d];
+                }
+            }
+            // mu (M x P, mean added), sigma^2 (M) and their candidate gradients: dmu (M x D, of the first output), dsigma2 (M x D)
+            // in one device pass (lb_query_grad)
+            void query_grad(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu, Eigen::VectorXd& sigma2, Eigen::MatrixXd& dmu,
+                Eigen::MatrixXd& dsigma2) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "query_grad: the mean function has no input gradient");
+                const long M = (long)vs.size();
+                const int D = (int)vs[0].size(), P = (int)_dim_out;
+                std::vector<double> xq((size_t)M * D), m((size_t)M * P), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
+                for (long i = 0; i < M; ++i)
+                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
+                lb_check(lb_query_grad(_h, M, xq.data(), m.data(), s.data(), gm.data(), gs.data()), "lb_query_grad");
+                mu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)P);
+                sigma2 = Eigen::VectorXd((Eigen::Index)M);
+                dmu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                dsigma2 = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                for (long i = 0; i < M; ++i) {
+                    Eigen::VectorXd mv = _mean_function(vs[i], *this);
+                    for (int p = 0; p < P; ++p) mu(i, p) = m[(size_t)i * P + p] + mv(p);
+                    sigma2(i) = s[(size_t)i];
+                    for (int d = 0; d < D; ++d) {
+                        dmu(i, d) = gm[(size_t)i * D + d];
+                        dsigma2(i, d) = gs[(size_t)i * D + d];
+                    }
+                }
             }
             // fused ECI + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem aggregator): this GP is the objective,
             // `con` the constraint model, whose first output gives Pf (Pf = 1 while it has no samples).  Both mean functors run on

@@ -57,10 +57,26 @@ namespace limbo_b200 {
             bool answered = false;
             double best_value = 0.0;
             long best_index = -1;
+            std::vector<double>* values = nullptr; // when set, the answer also files every candidate's value here
+            bool gradients = false;                // the answering functor also answers a GradRequest (BatchedGradient)
         };
         inline BatchRequest*& current_batch()
         {
             static thread_local BatchRequest* req = nullptr;
+            return req;
+        }
+
+        // The start points announced by BatchedGradient (opt/batched_gradient.hpp) for one call of f: a batch-aware UCB / EI over
+        // limbo_b200::model::GP files every point's value and gradient (one lb_acq_grad).
+        struct GradRequest {
+            const std::vector<Eigen::VectorXd>* points = nullptr;
+            bool answered = false;
+            Eigen::VectorXd values;
+            Eigen::MatrixXd grads;
+        };
+        inline GradRequest*& current_grad_batch()
+        {
+            static thread_local GradRequest* req = nullptr;
             return req;
         }
 
@@ -148,10 +164,36 @@ namespace limbo_b200 {
             template <typename Model>
             inline void answer_batch(const Model& model, int acq_id, double p0, double p1)
             {
-                answer_batch([&](const std::vector<Eigen::VectorXd>& c) { return model.acq_argmax(acq_id, p0, p1, c); });
+                opt::BatchRequest* req = opt::current_batch();
+                std::vector<double>* values = req ? req->values : nullptr;
+                answer_batch([&](const std::vector<Eigen::VectorXd>& c) { return model.acq_argmax(acq_id, p0, p1, c, values); });
+                if (req && req->answered) req->gradients = true;
+            }
+            // files every start point's value and gradient in the pending GradRequest, if any (one lb_acq_grad)
+            template <typename Model>
+            inline void answer_grad_batch(const Model& model, int acq_id, double p0, double p1)
+            {
+                opt::GradRequest* req = opt::current_grad_batch();
+                if (!req || req->answered || !req->points || req->points->empty()) return;
+                model.acq_grad(acq_id, p0, p1, *req->points, req->values, req->grads);
+                req->answered = true;
+            }
+            // value and gradient at one point from one lb_acq_grad call
+            template <typename Model>
+            inline limbo::opt::eval_t one_point_grad(const Model& model, int acq_id, double p0, double p1, const Eigen::VectorXd& v)
+            {
+                Eigen::VectorXd vals;
+                Eigen::MatrixXd grads;
+                model.acq_grad(acq_id, p0, p1, std::vector<Eigen::VectorXd>{v}, vals, grads);
+                Eigen::VectorXd g((Eigen::Index)v.size());
+                for (int d = 0; d < (int)v.size(); ++d) g(d) = grads(0, d);
+                return limbo::opt::eval_t{vals(0), g};
             }
             template <typename M> struct is_device_gp : std::false_type {};
             template <typename P, typename K, typename Mf, typename H> struct is_device_gp<model::GP<P, K, Mf, H>> : std::true_type {};
+            template <typename M> struct has_candidate_grad : std::false_type {};
+            template <typename P, typename K, typename Mf, typename H>
+            struct has_candidate_grad<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
         }
 
         // acqui::UCB (acqui/ucb.hpp:83-90), batch-aware
@@ -165,9 +207,20 @@ namespace limbo_b200 {
             template <typename AggregatorFunction>
             limbo::opt::eval_t operator()(const Eigen::VectorXd& v, const AggregatorFunction& afun, bool gradient) const
             {
-                assert(!gradient);
-                if (opt::current_batch() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                if constexpr (detail::has_candidate_grad<Model>::value) {
+                    if (gradient) { // one lb_acq_grad call, FirstElem aggregator only
+                        assert(detail::acts_like_first_elem(afun, (int)_model.dim_out()));
+                        return detail::one_point_grad(_model, LB_ACQ_UCB, Params::acqui_ucb::alpha(), 0.0, v);
+                    }
+                    if (opt::current_grad_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                        detail::answer_grad_batch(_model, LB_ACQ_UCB, Params::acqui_ucb::alpha(), 0.0);
+                }
+                else
+                    assert(!gradient);
+                if (opt::current_batch() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
                     detail::answer_batch(_model, LB_ACQ_UCB, Params::acqui_ucb::alpha(), 0.0);
+                    if (!detail::has_candidate_grad<Model>::value) opt::current_batch()->gradients = false;
+                }
                 Eigen::VectorXd mu;
                 double sigma;
                 std::tie(mu, sigma) = _model.query(v);
@@ -189,8 +242,10 @@ namespace limbo_b200 {
             template <typename AggregatorFunction>
             limbo::opt::eval_t operator()(const Eigen::VectorXd& v, const AggregatorFunction& afun, bool gradient) const
             {
-                assert(!gradient);
-                if (_model.samples().size() < 1) return limbo::opt::no_grad(0.0);
+                if constexpr (!detail::has_candidate_grad<Model>::value)
+                    assert(!gradient);
+                if (_model.samples().size() < 1) // ei.hpp:88-89; the gradient is 0 too
+                    return gradient ? limbo::opt::eval_t{0.0, Eigen::VectorXd(Eigen::VectorXd::Zero((Eigen::Index)v.size()))} : limbo::opt::no_grad(0.0);
                 if (_nb_samples != (int)_model.nb_samples()) { // ei.hpp:100-108
                     Eigen::MatrixXd mus;
                     Eigen::VectorXd s2;
@@ -204,8 +259,18 @@ namespace limbo_b200 {
                     }
                     _nb_samples = (int)_model.nb_samples();
                 }
-                if (opt::current_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                if constexpr (detail::has_candidate_grad<Model>::value) {
+                    if (gradient) { // one lb_acq_grad call, FirstElem aggregator only
+                        assert(detail::acts_like_first_elem(afun, (int)_model.dim_out()));
+                        return detail::one_point_grad(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter(), v);
+                    }
+                    if (opt::current_grad_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                        detail::answer_grad_batch(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter());
+                }
+                if (opt::current_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
                     detail::answer_batch(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter());
+                    if (!detail::has_candidate_grad<Model>::value) opt::current_batch()->gradients = false;
+                }
                 Eigen::VectorXd mu;
                 double sigma_sq;
                 std::tie(mu, sigma_sq) = _model.query(v);

@@ -29,12 +29,23 @@ class UCB:
         return float(get(self._params, "acqui_ucb", "alpha"))
 
     def __call__(self, v, afun=first_elem, gradient: bool = False):  # ucb.hpp:83-90
-        assert not gradient
+        if gradient:  # one device call (lb_acq_grad), FirstElem aggregator only
+            return _one_point_grad(self, v, afun)
         mu, sigma = self._model.query(v)
         return opt.no_grad(afun(mu) + self._alpha() * math.sqrt(sigma))
 
     def argmax_batch(self, Xq, return_values: bool = False):
         return self._model.acq_argmax_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], Xq, return_values)
+
+    def grad_batch(self, Xq):
+        """values (M) and gradients (M x D) at M candidates in one device pass"""
+        return self._model.acq_grad_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], Xq)
+
+
+def _one_point_grad(acqui, v, afun):
+    assert afun is first_elem
+    vals, grads = acqui.grad_batch(np.atleast_2d(np.asarray(v, dtype=np.float64)))
+    return float(vals[0]), grads[0]
 
 
 class GP_UCB(UCB):
@@ -74,7 +85,8 @@ class EI(_Improvement):
         super().__init__(model, params)
 
     def __call__(self, v, afun=first_elem, gradient: bool = False):  # ei.hpp:85-116
-        assert not gradient
+        if gradient:  # one device call (lb_acq_grad), FirstElem aggregator only
+            return _one_point_grad(self, v, afun)
         mu, sigma_sq = self._model.query(v)
         sigma = math.sqrt(sigma_sq)
         if sigma < 1e-10 or len(self._model.samples()) < 1:
@@ -93,6 +105,14 @@ class EI(_Improvement):
         self._update_f_max(first_elem)
         return self._model.acq_argmax_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], Xq,
                                             return_values)
+
+    def grad_batch(self, Xq):
+        """values (M) and gradients (M x D) at M candidates in one device pass; 0 before the model has samples"""
+        Xq = np.atleast_2d(Xq)
+        if len(self._model.samples()) < 1:
+            return np.zeros(len(Xq)), np.zeros(Xq.shape)
+        self._update_f_max(first_elem)
+        return self._model.acq_grad_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], Xq)
 
 
 class ECI(_Improvement):

@@ -22,6 +22,12 @@ class defaults_bo:
         refinements = 2
         shrink = 0.1
 
+    class opt_batchedgradient:  # DESIGN.md §4.10 gives the measurement behind these
+        candidates = 10000
+        starts = 32
+        iterations = 30
+        alpha = 0.01
+
 
 def _get(params, section, name):
     sec = getattr(params, section, None) if params is not None else None
@@ -58,6 +64,65 @@ class BatchedRandomSearch:
             if b2 >= best:
                 best, x = b2, cand[i2].copy()
         return x
+
+
+class BatchedGradientSearch:
+    """acquiopt<> policy: one random pass of `candidates` uniform points in [0,1]^D scored in one device pass, then the best
+    `starts` distinct points climb the acquisition in lockstep for `iterations` steps of Adam with the reference's update
+    (opt/adam.hpp: b1 = 0.9, b2 = 0.999, epsilon = 1e-8, step `alpha`, clipped to [0, 1] when bounded), each step one batched
+    value-and-gradient call (the acquisition's grad_batch) for all starts.  Returns the best point seen, the random pass included;
+    with an acquisition that has no grad_batch, or whose model or mean gives no candidate gradient, the best point of the random
+    pass."""
+
+    B1, B2, EPS = 0.9, 0.999, 1e-8
+
+    def __init__(self, params=None, rng: np.random.Generator | None = None):
+        self._params = params
+        self._rng = rng if rng is not None else np.random.default_rng()
+
+    def _p(self, name):
+        return _get(self._params, "opt_batchedgradient", name)
+
+    def __call__(self, acqui, dim: int, bounded: bool = True) -> np.ndarray:
+        cand = self._rng.random((int(self._p("candidates")), dim))
+        best, idx, vals = acqui.argmax_batch(cand, return_values=True)
+        x_best = cand[idx].copy()
+        grad_batch = getattr(acqui, "grad_batch", None)
+        if grad_batch is None:
+            return x_best
+        order = np.argsort(-np.nan_to_num(np.asarray(vals), nan=-np.inf), kind="stable")
+        chosen, seen = [], set()
+        for i in order:
+            key = cand[i].tobytes()
+            if key not in seen:
+                seen.add(key)
+                chosen.append(i)
+            if len(chosen) == int(self._p("starts")):
+                break
+        x = cand[chosen].copy()
+        alpha = float(self._p("alpha"))
+        m, v = np.zeros_like(x), np.zeros_like(x)
+        b1_t, b2_t = self.B1, self.B2
+        for it in range(int(self._p("iterations"))):
+            try:
+                f, g = grad_batch(x)
+            except (AttributeError, NotImplementedError):
+                # a model without candidate gradients (model.SPGP, model.MultiGP) or a mean without an input gradient
+                if it == 0:
+                    return x_best
+                raise
+            f = np.nan_to_num(np.asarray(f, dtype=np.float64), nan=-np.inf)
+            j = int(np.argmax(f))
+            if f[j] > best:
+                best, x_best = float(f[j]), x[j].copy()
+            m = self.B1 * m + (1.0 - self.B1) * g
+            v = self.B2 * v + (1.0 - self.B2) * g * g
+            x = x + alpha * (m / (1.0 - b1_t)) / (np.sqrt(v / (1.0 - b2_t)) + self.EPS)
+            if bounded:
+                x = np.clip(x, 0.0, 1.0)
+            b1_t *= self.B1
+            b2_t *= self.B2
+        return x_best
 
 
 class BOptimizer:

@@ -31,6 +31,9 @@ int lb_launch_query_point(const lb_gp* h, cudaStream_t st, const double* x_host,
     long long* launches);
 int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
     long long* launches);
+int lb_launch_query_grad(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
+    const LbGradOut& out, long long* launches);
+int lb_launch_prior_grad(cudaStream_t st, int64_t M, int D, int P, double s2, const LbGradOut& out, double* dMu, double* dS2);
 size_t lb_query_fused_scratch_doubles(const lb_gp* h, int grid);
 int lb_launch_query_fused(const lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dVscratch,
     int grid, double* dMu, double* dS2, long long* launches);
@@ -1003,6 +1006,132 @@ int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int6
     if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_UNSUPPORTED;
     return query_common(h, M, dXq, true, nullptr, nullptr, true, acq_id, acq_params, dMean_at_q, mean_const, dAcq_out,
         dBest_val, dBest_idx, true);
+}
+
+// lb_query_grad / lb_acq_grad and their _dev variants: mu, sigma^2 and their candidate gradients, and with acq_id >= 0 the
+// acquisition's value and gradient (query_grad.cu), always on the panel path so that mu, sigma^2 and the values are bit-identical to
+// lb_query / lb_acq_argmax on that path.  dev: every array is a device pointer (the coordinates are then not checked on the host).
+static int grad_common(const lb_gp* hc, int64_t M, const double* Xq, bool dev, double* mu_out, double* s2_out, double* dmu_out,
+    double* ds2_out, int acq_id, const double* acq_params, const double* mean_at_q, double mean_const, const double* mean_grad,
+    double* acq_out, double* grad_out)
+{
+    if (!hc || M <= 0 || !Xq) return LB_ERR_ARG;
+    if (acq_id >= 0 && ((acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) || !acq_params)) return LB_ERR_ARG;
+    lb_gp_full* h = full(hc);
+    if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
+    if (h->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
+    const int D = h->D, De = h->kp.D, P = h->P > 0 ? h->P : 1;
+    if (!dev)
+        for (int64_t i = 0; i < M * D; ++i)
+            if (!std::isfinite(Xq[i])) return LB_ERR_ARG;
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex);
+    QueryWs& w = h->ex.ws;
+    cudaStream_t st = h->stream;
+    const double p0 = acq_id >= 0 ? acq_params[0] : 0.0, p1 = acq_id == LB_ACQ_EI ? acq_params[1] : 0.0;
+    const cudaMemcpyKind d2o = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    const bool prior = (h->N == 0 || !h->fitted);
+    if (prior && h->N != 0) return LB_ERR_STATE;
+    int rc;
+    const double* dQraw = Xq;
+    if (!dev && !prior) {
+        if ((rc = ensure(h, w.dQraw, sizeof(double) * M * D))) return rc;
+        LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
+        dQraw = w.dQraw.get();
+    }
+    if ((rc = ensure(h, w.dMu, sizeof(double) * M * P))) return rc;
+    if ((rc = ensure(h, w.dS2, sizeof(double) * M))) return rc;
+    StreamTemps tmp(h->device, st); // host mode: device copies of the outputs and of the means
+    LbGradOut out{};
+    out.acq_id = acq_id;
+    out.p0 = p0;
+    out.p1 = p1;
+    out.mean_const = mean_const;
+    double* douts[4] = {dmu_out, ds2_out, acq_out, grad_out};
+    const size_t ncols[4] = {(size_t)D, (size_t)D, 1, (size_t)D};
+    double* dptr[4] = {};
+    for (int k = 0; k < 4; ++k) {
+        if (!douts[k] || (acq_id < 0 && k >= 2)) continue;
+        if (dev) dptr[k] = douts[k];
+        else if ((rc = tmp.alloc(sizeof(double) * M * ncols[k], &dptr[k]))) return rc;
+    }
+    const double* dMean = mean_at_q;
+    const double* dMeanGrad = mean_grad;
+    if (acq_id >= 0 && !dev) {
+        double* p;
+        if (mean_at_q) {
+            if ((rc = tmp.alloc(sizeof(double) * M, &p))) return rc;
+            LB_CUDA(cudaMemcpyAsync(p, mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
+            dMean = p;
+        }
+        if (mean_grad) {
+            if ((rc = tmp.alloc(sizeof(double) * M * D, &p))) return rc;
+            LB_CUDA(cudaMemcpyAsync(p, mean_grad, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
+            dMeanGrad = p;
+        }
+    }
+    if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma^2 = k(v, v) + noise, both constant in v: zero gradients
+        out.mean = dMean;
+        out.mean_grad = dMeanGrad;
+        out.dmu = dptr[0];
+        out.ds2 = dptr[1];
+        out.acq = dptr[2];
+        out.grad = dptr[3];
+        if ((rc = lb_launch_prior_grad(st, M, D, P, h->kp.sf2 + h->kp.noise, out, w.dMu.get(), w.dS2.get()))) return rc;
+        h->launches++;
+    }
+    // candidate chunks as the panel path of query_fill: V (Np x Mc) <= ~6 GiB
+    const int64_t Mp = (M + LB_TILE - 1) / LB_TILE * LB_TILE;
+    const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)6 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
+    const int64_t Mc = prior ? M : std::min(Mp, maxcols);
+    if (!prior && ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc)) || (rc = ensure(h, w.dV, sizeof(double) * lb_query_panel_scratch_doubles(h, Mc)))))
+        return rc;
+    for (int64_t m0 = 0; m0 < M && !prior; m0 += Mc) {
+        const int64_t mc = std::min(Mc, M - m0);
+        const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
+        dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
+        pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
+        h->launches++;
+        out.mean = dMean ? dMean + m0 : nullptr;
+        out.mean_grad = dMeanGrad ? dMeanGrad + m0 * D : nullptr;
+        out.dmu = dptr[0] ? dptr[0] + m0 * D : nullptr;
+        out.ds2 = dptr[1] ? dptr[1] + m0 * D : nullptr;
+        out.acq = dptr[2] ? dptr[2] + m0 : nullptr;
+        out.grad = dptr[3] ? dptr[3] + m0 * D : nullptr;
+        if ((rc = lb_launch_query_grad(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, out, &h->launches)))
+            return rc;
+    }
+    if (mu_out) LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu.get(), sizeof(double) * M * P, d2o, st));
+    if (s2_out) LB_CUDA(cudaMemcpyAsync(s2_out, w.dS2.get(), sizeof(double) * M, d2o, st));
+    if (!dev)
+        for (int k = 0; k < 4; ++k)
+            if (dptr[k]) LB_CUDA(cudaMemcpyAsync(douts[k], dptr[k], sizeof(double) * M * ncols[k], cudaMemcpyDeviceToHost, st));
+    LB_CUDA(cudaStreamSynchronize(st));
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+
+int lb_query_grad(const lb_gp* h, int64_t M, const double* Xq, double* mu, double* s2, double* dmu, double* ds2)
+{
+    return grad_common(h, M, Xq, false, mu, s2, dmu, ds2, -1, nullptr, nullptr, 0.0, nullptr, nullptr, nullptr);
+}
+int lb_query_grad_dev(const lb_gp* h, int64_t M, const double* dXq, double* dMu, double* dS2, double* dDmu, double* dDs2)
+{
+    return grad_common(h, M, dXq, true, dMu, dS2, dDmu, dDs2, -1, nullptr, nullptr, 0.0, nullptr, nullptr, nullptr);
+}
+int lb_acq_grad(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* Xq, const double* mean_at_q,
+    double mean_const, const double* mean_grad_at_q, double* acq_out, double* grad_out)
+{
+    if (acq_id < 0) return LB_ERR_ARG;
+    return grad_common(h, M, Xq, false, nullptr, nullptr, nullptr, nullptr, acq_id, acq_params, mean_at_q, mean_const, mean_grad_at_q,
+        acq_out, grad_out);
+}
+int lb_acq_grad_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* dXq, const double* dMean_at_q,
+    double mean_const, const double* dMean_grad_at_q, double* dAcq_out, double* dGrad_out)
+{
+    if (acq_id < 0) return LB_ERR_ARG;
+    return grad_common(h, M, dXq, true, nullptr, nullptr, nullptr, nullptr, acq_id, acq_params, dMean_at_q, mean_const, dMean_grad_at_q,
+        dAcq_out, dGrad_out);
 }
 
 static int ensure_eci_events(lb_gp_full* h)

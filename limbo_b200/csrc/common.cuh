@@ -180,6 +180,41 @@ __device__ __forceinline__ double lb_unit_kernel_from_z(double z, const KernPara
     return lb_exp_nonpos(-0.5 * (z * kp.c1));
 }
 
+// expected improvement of mu over f_max + jitter, 0 when sigma < 1e-10: ei.hpp:92-115, and the factor eci.hpp:86-106 weights
+__device__ __forceinline__ double lb_ei_factor(double mu, double s2, double f_max, double jitter)
+{
+    double sigma = sqrt(s2);
+    if (sigma < 1e-10) return 0.0;
+    double X = mu - f_max - jitter;
+    double Z = X / sigma;
+    double phi = exp(-0.5 * (Z * Z)) / sqrt(2.0 * M_PI);
+    double Phi = 0.5 * erfc(-Z / sqrt(2.0));
+    return X * Phi + sigma * phi;
+}
+
+// acquisition value per candidate (FirstElem aggregator, bo_base.hpp:99-105)
+//   acq_id 0: UCB / GP_UCB  mu + p0 * sqrt(s2)                 ucb.hpp:89, gp_ucb.hpp:102
+//   acq_id 1: EI  (p0 = f_max, p1 = jitter)                    ei.hpp:92-115
+__device__ __forceinline__ double lb_acq_value(int acq_id, double mu, double s2, double p0, double p1)
+{
+    if (acq_id == 0) return mu + p0 * sqrt(s2);
+    return lb_ei_factor(mu, s2, p0, p1);
+}
+
+// What the candidate-gradient pass (query_grad.cu) writes for one candidate chunk; every pointer may be NULL and starts at
+// the chunk's first candidate.
+struct LbGradOut {
+    int acq_id;               // -1: no acquisition; otherwise an lb_acq_value id
+    double p0, p1;            // acquisition parameters, as lb_acq_argmax takes them
+    const double* mean;       // M first components of mean(v), or NULL and mean_const
+    double mean_const;
+    const double* mean_grad;  // M x Draw gradient of the mean's first component, or NULL (= 0)
+    double* dmu;              // M x Draw: gradient of k^T alpha[:, 0]
+    double* ds2;              // M x Draw: gradient of sigma^2, 0 where the clamp of gp.hpp:623 is active
+    double* acq;              // M acquisition values
+    double* grad;             // M x Draw acquisition gradients
+};
+
 // staged coordinate d (0 <= d < kp.D) of a raw point given by x(r), r < kp.Draw
 template <typename F>
 __device__ __forceinline__ double lb_staged_coord(const KernParams& kp, int d, F&& x)

@@ -157,27 +157,6 @@ colnorm_kernel(const double* __restrict__ V, int64_t Np, double kvv, double nois
     }
 }
 
-// expected improvement of mu over f_max + jitter, 0 when sigma < 1e-10: ei.hpp:92-115, and the factor eci.hpp:86-106 weights
-__device__ __forceinline__ double ei_factor(double mu, double s2, double f_max, double jitter)
-{
-    double sigma = sqrt(s2);
-    if (sigma < 1e-10) return 0.0;
-    double X = mu - f_max - jitter;
-    double Z = X / sigma;
-    double phi = exp(-0.5 * (Z * Z)) / sqrt(2.0 * M_PI);
-    double Phi = 0.5 * erfc(-Z / sqrt(2.0));
-    return X * Phi + sigma * phi;
-}
-
-// acquisition value per candidate (FirstElem aggregator, bo_base.hpp:99-105)
-//   acq_id 0: UCB / GP_UCB  mu + p0 * sqrt(s2)                 ucb.hpp:89, gp_ucb.hpp:102
-//   acq_id 1: EI  (p0 = f_max, p1 = jitter)                    ei.hpp:92-115
-__device__ __forceinline__ double acq_value(int acq_id, double mu, double s2, double p0, double p1)
-{
-    if (acq_id == 0) return mu + p0 * sqrt(s2);
-    return ei_factor(mu, s2, p0, p1);
-}
-
 // (value, index) of a 256-thread block's best candidate into blk_val / blk_idx[blockIdx.x].  NaN never wins; the lowest
 // index wins ties.  Threads without a candidate pass (-DBL_MAX, LLONG_MAX).
 __device__ __forceinline__ void block_argmax(double v, long long idx, double* __restrict__ blk_val, long long* __restrict__ blk_idx)
@@ -215,7 +194,7 @@ acq_kernel(int acq_id, double p0, double p1, int64_t M, const double* __restrict
     long long idx = LLONG_MAX;
     if (m < M) {
         double mu = mu0[m * mu_stride] + (mean_at_q ? mean_at_q[m] : mean_const);
-        v = acq_value(acq_id, mu, s2[m], p0, p1);
+        v = lb_acq_value(acq_id, mu, s2[m], p0, p1);
         if (acq) acq[m] = v;
         idx = m;
     }
@@ -250,7 +229,7 @@ eci_kernel(double f_max, double jitter, int64_t M, const double* __restrict__ mu
                 }
             }
             const double mu = mu_obj[m * p_obj] + (mean_obj ? mean_obj[m] : mean_obj_const);
-            v = pf * ei_factor(mu, s2, f_max, jitter);
+            v = pf * lb_ei_factor(mu, s2, f_max, jitter);
         }
         if (acq) acq[m] = v;
         idx = m;
@@ -919,6 +898,36 @@ size_t lb_query_panel_scratch_doubles(const lb_gp* h, int64_t Mp)
     const int64_t T = h->Np / LB_TILE;
     return (size_t)(h->Np * Mp + (int64_t)panel::SB * LB_TILE * Mp + T * Mp);
 }
+double* lb_query_panel_tbuf(const lb_gp* h, double* dWork, int64_t Mp) { return dWork + h->Np * Mp; }
+double* lb_query_panel_norms(const lb_gp* h, double* dWork, int64_t Mp) { return dWork + h->Np * Mp + (int64_t)panel::SB * LB_TILE * Mp; }
+
+// The chain update_s -> solve_s -> update_s+1 -> ... of a panel walk (forward here, backward in query_grad.cu) only couples tiles of
+// the SAME candidate column tile, so the column tiles can walk it in groups on separate streams, the tail of one group's launch being
+// filled by another group's CTAs.  Four equal groups, each walking the chain on its own stream, when a launch of all column tiles is
+// under one round of the machine (M = 640 at N = 16384: 160 CTAs for 264 slots), so that the groups, drifting apart, keep the SMs
+// full; otherwise one stream.  Measured on an H100 SXM at a 400 W power limit, N = 16384, ms per batch (process-to-process spread up
+// to ~10 % at that limit), 1 / 2 / 3 / 4 groups: M = 640: 10.9 / 10.1 / 9.6 / 9.1, 1250: 16.3 / 15.2 / 15.5 / 16.0, 2500: 28.9 /
+// 28.1 / 30.9 / 30.9; M = 10^4: one stream 121.9, two groups of 90 / 80 / 70 / 60 / 50 % of the column tiles 120.8 / 130.3 / 131.5 /
+// 130.9 / 132.0.  Results do not depend on the grouping (every tile's arithmetic is unchanged).
+// Returns the number of groups; sts[g] is group g's stream (sts[0] = st), gbeg[g] its first 128-wide column tile (gbeg[ngroups] =
+// ctiles).
+int lb_query_panel_groups(lb_gp* h, cudaStream_t st, int ctiles, cudaStream_t sts[4], int gbeg[5])
+{
+    using CD = lbg::CfgDual;
+    constexpr int wmul = LB_TILE / CD::BN; // 64-wide column tiles per 128 candidates
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    const int slots = sms * CD::CTAS_PER_SM;
+    int ngroups = (ctiles >= 4 && (int64_t)ctiles * wmul * panel::SB < (int64_t)slots) ? 4 : 1;
+    for (int g = 0; g < 4; ++g) sts[g] = st;
+    for (int g = 1; g < ngroups; ++g) {
+        if (!h->group[g - 1] && cudaStreamCreateWithFlags(&h->group[g - 1], cudaStreamNonBlocking) != cudaSuccess) h->group[g - 1] = nullptr;
+        if (!h->group[g - 1]) { ngroups = g; break; } // no stream: fewer groups
+        sts[g] = h->group[g - 1];
+    }
+    for (int g = 0; g <= ngroups; ++g) gbeg[g] = (int)((int64_t)ctiles * g / ngroups);
+    return ngroups;
+}
 
 int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
     long long* launches)
@@ -932,8 +941,8 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
     const int T = (int)(h->Np / LB_TILE);
     const int64_t ld = h->Np, ldt = (int64_t)SB * LB_TILE;
     double* dV = dWork;
-    double* dT = dV + ld * Mp;
-    double* dNorm = dT + ldt * Mp;
+    double* dT = lb_query_panel_tbuf(h, dWork, Mp);
+    double* dNorm = lb_query_panel_norms(h, dWork, Mp);
     int rc = lb_launch_linv_levels(h, SB); // inverse of the 16-tile diagonal blocks (kept until the next fit)
     if (rc) return rc;
     dim3 grid((unsigned)T, (unsigned)(Mp / LB_TILE));
@@ -946,28 +955,10 @@ int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQ
         mu_kernel<<<(unsigned)M, 256, 0, st>>>(dV, h->Np, h->dAlpha, h->P, dMu);
     }
     if (launches) *launches += 2;
-    // The chain update_s -> solve_s -> update_s+1 -> ... only couples tiles of the SAME candidate column tile, so the column tiles
-    // can walk it in groups on separate streams, the tail of one group's launch being filled by another group's CTAs.
-    const int ctiles = (int)(Mp / LB_TILE);
-    constexpr int wmul = LB_TILE / CD::BN; // 64-wide column tiles per 128 candidates
-    // Four equal groups, each walking the chain on its own stream, when a launch of all column tiles is under one round of the
-    // machine (M = 640 at N = 16384: 160 CTAs for 264 slots), so that the groups, drifting apart, keep the SMs full; otherwise
-    // one stream.  Measured on an H100 SXM at a 400 W power limit, N = 16384, ms per batch (process-to-process spread up to ~10 %
-    // at that limit), 1 / 2 / 3 / 4 groups: M = 640: 10.9 / 10.1 / 9.6 / 9.1, 1250: 16.3 / 15.2 / 15.5 / 16.0, 2500: 28.9 / 28.1 /
-    // 30.9 / 30.9; M = 10^4: one stream 121.9, two groups of 90 / 80 / 70 / 60 / 50 % of the column tiles 120.8 / 130.3 / 131.5 /
-    // 130.9 / 132.0.  Results do not depend on the grouping (every tile's arithmetic is unchanged).
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
-    const int slots = sms * CD::CTAS_PER_SM;
-    int ngroups = (ctiles >= 4 && (int64_t)ctiles * wmul * SB < (int64_t)slots) ? 4 : 1;
-    cudaStream_t sts[4] = {st, st, st, st};
-    for (int g = 1; g < ngroups; ++g) {
-        if (!h->group[g - 1] && cudaStreamCreateWithFlags(&h->group[g - 1], cudaStreamNonBlocking) != cudaSuccess) h->group[g - 1] = nullptr;
-        if (!h->group[g - 1]) { ngroups = g; break; } // no stream: fewer groups
-        sts[g] = h->group[g - 1];
-    }
-    int gbeg[5]; // first column tile (128 wide) of each group
-    for (int g = 0; g <= ngroups; ++g) gbeg[g] = (int)((int64_t)ctiles * g / ngroups);
+    constexpr int wmul = LB_TILE / CD::BN;
+    cudaStream_t sts[4];
+    int gbeg[5];
+    const int ngroups = lb_query_panel_groups(h, st, (int)(Mp / LB_TILE), sts, gbeg);
     {
         LbProfScope ps(h, st, LB_PC_QSTEP);
         if (ngroups >= 2) {

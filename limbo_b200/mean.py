@@ -31,8 +31,19 @@ class BaseMean:
     def is_constant(self) -> bool:
         return False
 
+    def grad_x(self, xs: np.ndarray, gp) -> np.ndarray:
+        """Gradient of the mean with respect to the input at M points (M x D): M x dim_out x D.  Only the means whose value does
+        not depend on the input define it; the candidate-gradient calls of model.GP pass this error on."""
+        raise NotImplementedError(f"{type(self).__name__} has no input gradient")
 
-class NullFunction(BaseMean):
+
+class _InputFree(BaseMean):
+    def grad_x(self, xs, gp) -> np.ndarray:
+        xs = np.atleast_2d(xs)
+        return np.zeros((xs.shape[0], self._dim_out, xs.shape[1]))
+
+
+class NullFunction(_InputFree):
     """mean/null_function.hpp:57-63"""
 
     def __call__(self, v, gp) -> np.ndarray:
@@ -45,7 +56,7 @@ class NullFunction(BaseMean):
         return True
 
 
-class Constant(BaseMean):
+class Constant(_InputFree):
     """mean/constant.hpp:66-94"""
 
     def __init__(self, params=None, dim_out: int = 1):
@@ -74,7 +85,7 @@ class Constant(BaseMean):
         return True
 
 
-class Data(BaseMean):
+class Data(_InputFree):
     """mean/data.hpp:55-64: the mean of the observations."""
 
     def __call__(self, v, gp) -> np.ndarray:
@@ -131,6 +142,10 @@ class FunctionARD(BaseMean):
     def __call__(self, v, gp) -> np.ndarray:
         m = np.asarray(self._mean_function(v, gp), dtype=np.float64)
         return self._tr @ np.concatenate([m, [1.0]])
+
+    def grad_x(self, xs, gp) -> np.ndarray:
+        # an affine map of the inner mean's value: the chain rule through _tr's linear part
+        return np.einsum("ij,mjd->mid", self._tr[:, :-1], self._mean_function.grad_x(xs, gp))
 
 
 def function_ard(inner_cls):

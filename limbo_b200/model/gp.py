@@ -267,6 +267,40 @@ class GP:
             return best.value, idx.value, vals
         return best.value, idx.value
 
+    def query_grad_batch(self, Xq):
+        """mu (M x P), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D, of the first output) and
+        grad sigma^2 (M x D), in one device pass (lb_query_grad); the mean's value and input gradient are added.  Raises
+        NotImplementedError for a mean without an input gradient (mean.BaseMean.grad_x)."""
+        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        M, D = Xq.shape
+        P = max(self._dim_out, 1)
+        mgrad = self._mean_function.grad_x(Xq, self)
+        if len(self._samples) == 0:
+            self._ensure_dims_for_prior(D)
+        mu, s2 = np.empty((M, P)), np.empty(M)
+        dmu, ds2 = np.empty((M, D)), np.empty((M, D))
+        _lib.check(self._lib.lb_query_grad(self._h, M, _ptr(Xq), _ptr(mu), _ptr(s2), _ptr(dmu), _ptr(ds2)), "lb_query_grad")
+        mu += self._mean_function.batch(Xq, self)
+        dmu += mgrad[:, 0, :]
+        return mu, s2, dmu, ds2
+
+    def acq_grad_batch(self, acq_id: int, acq_params, Xq):
+        """Acquisition values (M) and gradients (M x D) of UCB / GP_UCB (acq_id 0) or EI (acq_id 1) with the FirstElem aggregator,
+        in one device pass (lb_acq_grad); parameters and values as acq_argmax_batch."""
+        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        M, D = Xq.shape
+        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
+        if ap.size < 2:
+            ap = np.append(ap, 0.0)
+        mgrad = np.ascontiguousarray(self._mean_function.grad_x(Xq, self)[:, 0, :])
+        if len(self._samples) == 0:
+            self._ensure_dims_for_prior(D)
+        mean0, mconst = self._first_mean(Xq)
+        vals, grads = np.empty(M), np.empty((M, D))
+        _lib.check(self._lib.lb_acq_grad(self._h, acq_id, _ptr(ap), M, _ptr(Xq), _ptr(mean0) if mean0 is not None else None, mconst,
+                                         _ptr(mgrad) if np.any(mgrad) else None, _ptr(vals), _ptr(grads)), "lb_acq_grad")
+        return vals, grads
+
     def _first_mean(self, Xq):
         """First output of the mean functor at every candidate, as (array, 0.0), or (None, constant) for a constant mean."""
         if self._mean_function.is_constant():
