@@ -14,6 +14,7 @@
 //     every triangular solve.
 #pragma once
 #include <cuda_runtime.h>
+#include <cfloat>
 #include <cstdint>
 #include <cstdio>
 #include <vector>
@@ -139,6 +140,12 @@ __device__ __forceinline__ double lb_rsqrt_nr(double x)
     r = fma(r, fma(-h * r, r, 0.5), r);
     return r;
 }
+// d = sqrt(z) for the Matern functors.  rsqrt.approx.ftz flushes a subnormal z to zero (seed +inf, NaN after the Newton steps),
+// so z < DBL_MIN (d < 1.5e-154, c1 d < 1e-150) gives d = 0, which is exact to rounding in every formula that uses d.
+__device__ __forceinline__ double lb_dist_from_z(double z)
+{
+    return (z >= DBL_MIN) ? z * lb_rsqrt_nr(z) : 0.0;
+}
 __device__ __forceinline__ double lb_kernel_from_z(int id, double z, const KernParams& kp)
 {
     switch (id) {
@@ -148,12 +155,12 @@ __device__ __forceinline__ double lb_kernel_from_z(int id, double z, const KernP
         // sigma_f^2 (1 + c1 d + c2 d^2) exp(-c1 d) with d^2 = z and sigma_f^2 folded into the polynomial (two FMAs instead of
         // two products and two sums; <= 2 ulp from the reference's operation order, matern_five_halves.hpp:106-112): the
         // Matern K build is bound by the fp64 pipe, not by HBM (~45 fp64 instructions per element)
-        const double d = (z > 0.0) ? z * lb_rsqrt_nr(z) : 0.0;
+        const double d = lb_dist_from_z(z);
         const double term1 = kp.c1 * d;
         return fma(kp.c2 * kp.sf2, z, fma(kp.sf2, term1, kp.sf2)) * lb_exp_nonpos(-term1);
     }
     case LB_K_MATERN32: {
-        const double d = (z > 0.0) ? z * lb_rsqrt_nr(z) : 0.0;
+        const double d = lb_dist_from_z(z);
         const double term = kp.c1 * d;
         return fma(kp.sf2, term, kp.sf2) * lb_exp_nonpos(-term);
     }
@@ -168,12 +175,12 @@ __device__ __forceinline__ double lb_unit_kernel_from_z(double z, const KernPara
 {
     if (KID == LB_K_SE_ARD) return lb_exp_nonpos(-0.5 * z);
     if (KID == LB_K_MATERN52) {
-        const double d = (z > 0.0) ? z * lb_rsqrt_nr(z) : 0.0;
+        const double d = lb_dist_from_z(z);
         const double term1 = kp.c1 * d;
         return (1 + term1 + kp.c2 * (d * d)) * lb_exp_nonpos(-term1);
     }
     if (KID == LB_K_MATERN32) {
-        const double d = (z > 0.0) ? z * lb_rsqrt_nr(z) : 0.0;
+        const double d = lb_dist_from_z(z);
         const double term = kp.c1 * d;
         return (1 + term) * lb_exp_nonpos(-term);
     }

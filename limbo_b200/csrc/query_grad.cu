@@ -72,7 +72,7 @@ __device__ __forceinline__ double grad_coef(double z, const KernParams& kp)
 {
     if (KID == LB_K_SE_ARD) return -lb_kernel_from_z(LB_K_SE_ARD, z, kp); // -k
     if (KID == LB_K_EXP) return -lb_kernel_from_z(LB_K_EXP, z, kp) * kp.c1; // -k / l^2
-    const double d = (z > 0.0) ? z * lb_rsqrt_nr(z) : 0.0;
+    const double d = lb_dist_from_z(z);
     const double e = lb_exp_nonpos(-kp.c1 * d);
     if (KID == LB_K_MATERN52) return -kp.sf2 * kp.c2 * fma(kp.c1, d, 1.0) * e; // -(5 sf2 / 3 l^2)(1 + sqrt5 d / l) e^(-sqrt5 d / l)
     return -kp.sf2 * (kp.c1 * kp.c1) * e;                                        // -(3 sf2 / l^2) e^(-sqrt3 d / l)

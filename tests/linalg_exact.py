@@ -315,6 +315,26 @@ class QueryCase:
         s2 = sf2 - (V * V).sum(0) + noise
         return L, mu, s2, V, Ks
 
+    def grad_reference(self, kid, p, noise, Xq, L=None) -> dict:
+        """mu, sigma^2 (s2), grad mu of output 0 (dmu), grad sigma^2 (ds2), V = L^-1 K* and W = L^-T V of candidates Xq, with
+        two triangular solves in staged coordinates u = x J (oracle/acq_grad.staging: SE-ARD's Lambda columns enter only
+        through J); also the factor L, K* (Ks) and the pairs' differences Q, distances d and coefficients c for grad_bounds.
+        L: c (I + E) with c fitted to this candidate set as in reference(), unless given."""
+        import scipy.linalg as sl
+        J, _, _, Q, d, k, cc = _staged_pairs(kid, p, self.X, Xq)
+        sf2 = staging(kid, p, self.D)[1]
+        if L is None:
+            V1 = sl.solve_triangular(np.eye(self.N) + self.E, k, lower=True)
+            c = math.sqrt(2.0 * float((V1 * V1).sum(0).max()) / sf2)
+            L = np.asfortranarray(c * (np.eye(self.N) + self.E))
+        V = sl.solve_triangular(L, k, lower=True)
+        W = sl.solve_triangular(L, V, lower=True, trans="T")
+        a0 = self.alpha[:, 0]
+        return dict(L=L, Ks=k, V=V, W=W, Q=Q, d=d, c=cc,
+                    mu=k.T @ self.alpha, s2=sf2 - (V * V).sum(0) + noise,
+                    dmu=np.stack([(cc * q).T @ a0 for q in Q], axis=1) @ J.T,
+                    ds2=np.stack([-2.0 * ((cc * q) * W).sum(0) for q in Q], axis=1) @ J.T)
+
 
 def bound_mu(kid, p, Ks, alpha, xmax, D):
     """|mu^ - mu| per candidate and output: the dot product (device and host) and the kernel evaluation."""
@@ -339,19 +359,207 @@ def bound_s2(kid, p, V, c, normE, xmax, D, noise):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# candidate gradients on a loaded factor (lb_query_grad / lb_acq_grad)
+# ---------------------------------------------------------------------------------------------------------------------
+def staging(kid, p, D):
+    """(J, sf2, l, a): staged coordinates u = x J as oracle/acq_grad.staging (SE-ARD: [diag(1/ell) | Lambda], the identity
+    otherwise), and the scale a of the distance d = |u - u_n| in the exponent (Matern: sqrt(5)/l, sqrt(3)/l)."""
+    from oracle import acq_grad as AG
+    J, sf2, l = AG.staging(kid, p, D)
+    a = {0: 1.0, 1: math.sqrt(5.0) / l, 2: math.sqrt(3.0) / l, 3: 1.0 / l}[kid]
+    return J, sf2, l, a
+
+
+def grad_params(kid, D, klam, rng) -> np.ndarray:
+    """Hyper-parameters for the candidate-gradient cases: kernel_params' ranges with the length scales grown by sqrt(D / 3),
+    so that distances in [0,1]^D stay of order one; SE-ARD with klam Lambda columns of entries N(0, 0.25 / D)."""
+    s = 0.5 * math.log(max(D, 3) / 3.0)
+    if kid == 0:
+        return np.concatenate([rng.uniform(-0.7, 0.3, D) + s, rng.normal(0.0, 0.5 / math.sqrt(D), D * klam), [rng.uniform(-0.3, 0.3)]])
+    return np.array([rng.uniform(-1.0, 0.0) + s, rng.uniform(-0.3, 0.3)])
+
+
+def coef_lipschitz(kid, sf2, l, a):
+    """(Lk, Lc): bounds of |dk/dd| and |dc/dd| over d >= 0, with k(d) the kernel value and c(d) the gradient coefficient
+    (dk/du = c (u - u_n)) of oracle/acq_grad.kernel_and_coef:
+      SE:   k = sf2 e^(-d^2/2),          c = -k:                     |k'|, |c'| <= sf2 d e^(-d^2/2) <= sf2
+      Exp:  k = sf2 e^(-d^2/2l^2),       c = -k / l^2:               |k'| <= sf2 / l,  |c'| <= sf2 / l^3
+      M5/2: k = sf2 (1 + ad + a^2d^2/3) e^(-ad), c = -sf2 a^2/3 (1 + ad) e^(-ad): |k'| = sf2 a (ad)(1 + ad)/3 e^(-ad) <= sf2 a,
+            |c'| = sf2 a^3 (ad) e^(-ad) / 3 <= sf2 a^3
+      M3/2: k = sf2 (1 + ad) e^(-ad),    c = -sf2 a^2 e^(-ad):      |k'| = sf2 a (ad) e^(-ad) <= sf2 a,  |c'| <= sf2 a^3"""
+    if kid == 0:
+        return sf2, sf2
+    if kid == 3:
+        return sf2 / l, sf2 / l ** 3
+    return sf2 * a, sf2 * a ** 3
+
+
+def _staged_pairs(kid, p, X, Xq):
+    """Staged coordinates, the per-dimension differences q_e = u_e(candidate) - u_e(training point) (N x M each), the
+    distances d and the kernel values k and coefficients c of every pair, in fp64."""
+    from oracle import acq_grad as AG
+    J, sf2, l, _ = staging(kid, p, X.shape[1])
+    U_, Uq = X @ J, Xq @ J
+    Q = [Uq[None, :, e] - U_[:, e, None] for e in range(J.shape[1])]
+    z = np.zeros_like(Q[0])
+    for q in Q:
+        z += q * q
+    k, c = AG.kernel_and_coef(kid, z, sf2, l)
+    return J, U_, Uq, Q, np.sqrt(z), k, c
+
+
+def grad_reference_ld(kid, p, X, Xq, L, alpha):
+    """The same quantities as QueryCase.grad_reference (mu, sigma^2, grad mu of output 0, grad sigma^2), in np.longdouble
+    throughout: staging, kernel values and coefficients, and both triangular solves by substitution.  For the host check
+    that the fp64 reference stays inside the bounds below."""
+    ld = np.longdouble
+    X, Xq, p = X.astype(ld), Xq.astype(ld), np.asarray(p).astype(ld)
+    D = X.shape[1]
+    if kid == 0:
+        klam = (p.size - 1 - D) // D
+        J = np.hstack([np.diag(np.exp(-p[:D])), p[D:D + D * klam].reshape(klam, D).T])
+        sf2, l = np.exp(2 * p[-1]), ld(1)
+    else:
+        J, sf2, l = np.eye(D, dtype=ld), np.exp(2 * p[1]), np.exp(p[0])
+    U_, Uq = X @ J, Xq @ J
+    Q = [Uq[None, :, e] - U_[:, e, None] for e in range(J.shape[1])]
+    z = sum(q * q for q in Q)
+    d = np.sqrt(z)
+    if kid == 0:
+        k = sf2 * np.exp(-z / 2)
+        c = -k
+    elif kid == 3:
+        k = sf2 * np.exp(-z / (2 * l * l))
+        c = -k / (l * l)
+    elif kid == 1:
+        a = np.sqrt(ld(5)) / l
+        e = np.exp(-a * d)
+        k, c = sf2 * (1 + a * d + a * a * z / 3) * e, -sf2 * (a * a / 3) * (1 + a * d) * e
+    else:
+        a = np.sqrt(ld(3)) / l
+        e = np.exp(-a * d)
+        k, c = sf2 * (1 + a * d) * e, -sf2 * a * a * e
+    Lq = L.astype(ld)
+    n, m = k.shape
+    V = np.zeros((n, m), dtype=ld)
+    for i in range(n):
+        V[i] = (k[i] - Lq[i, :i] @ V[:i]) / Lq[i, i]
+    W = np.zeros((n, m), dtype=ld)
+    for i in range(n - 1, -1, -1):
+        W[i] = (V[i] - Lq[i + 1:, i] @ W[i + 1:]) / Lq[i, i]
+    a0 = alpha[:, 0].astype(ld)
+    gmu = np.stack([(c * q).T @ a0 for q in Q], axis=1) @ J.T
+    gs2 = np.stack([-2 * ((c * q) * W).sum(0) for q in Q], axis=1) @ J.T
+    mu = k.T @ alpha.astype(ld)
+    s2 = sf2 - (V * V).sum(0)
+    return mu, s2, gmu, gs2
+
+
+def grad_bounds(kid, p, X, Xq, alpha, noise, normE, ref):
+    """First-order bounds on |x^ - x| for mu, sigma^2, grad mu (output 0) and grad sigma^2 of ONE fp64 evaluation (the
+    device's or the host reference's: a comparison of the two uses twice these), per candidate (and dimension).  In staged
+    coordinates u = x J, for each pair of a candidate and a training point n:
+      staging:  |du_e| <= gamma_{D+3} (|x| |J|)_e per point (the reciprocal 1/ell, the Lambda dot product; 0 when J = I),
+                |dq_ne| <= du_e(candidate) + du_e(n) + u |q_ne|;
+      distance: |dd_n| <= ||dq_n||_2 + gamma_{De+6} d_n (the sum of De squares, the reciprocal square root);
+      k and c:  |dk_n| <= Lk |dd_n| + gamma_16 (1 + rho_n) |k_n|, likewise c with Lc (coef_lipschitz), rho_n the exponent
+                (exp < 3 ulp, its argument rho u, the polynomial and products < 8 roundings);
+      solves:   ||dV_c|| <= kap^2 gamma_N ||V_c|| + ||L^-1|| ||dK*_c||,  ||dW_c|| <= kap^2 gamma_N ||W_c|| + ||L^-1|| ||dV_c||
+                (bound_s2's forward bound, applied to L and then to L^T; kap = (1 + |E|)/(1 - |E|), ||L^-1|| <= 1/(c(1 - |E|)));
+      sums:     gamma_{N+2} times the sum of |products| (two products, then N terms in any order: the device's per-thread
+                chains, lane and warp trees; the host's BLAS);
+      map:      g_x = J g_u with gamma_{De+3} |J| |g_u| (the products, the sum, and the rounding of J itself).
+    ref: QueryCase.grad_reference's dict."""
+    N, D = X.shape
+    J, sf2, l, a = staging(kid, p, D)
+    De = J.shape[1]
+    aJ = np.abs(J)
+    ident = kid != 0
+    eu_x = np.zeros((N, De)) if ident else gamma(D + 3) * (np.abs(X) @ aJ)
+    eu_q = np.zeros((Xq.shape[0], De)) if ident else gamma(D + 3) * (np.abs(Xq) @ aJ)
+    Q, d, k, cc = ref["Q"], ref["d"], ref["Ks"], ref["c"]
+    dQ = [eu_q[None, :, e] + eu_x[:, e, None] + U * np.abs(Q[e]) for e in range(De)]
+    dd = np.sqrt(sum(x * x for x in dQ)) + gamma(De + 6) * d
+    rho = {0: 0.5 * d * d, 3: 0.5 * (d / l) ** 2}.get(kid, a * d)
+    Lk, Lc = coef_lipschitz(kid, sf2, l, a)
+    g16 = gamma(16) * (1.0 + rho)
+    dk = Lk * dd + g16 * np.abs(k)
+    dc = Lc * dd + g16 * np.abs(cc)
+    c = float(ref["L"][0, 0])
+    kap = (1.0 + normE) / (1.0 - normE)
+    nli = 1.0 / (c * (1.0 - normE))
+    V, W = ref["V"], ref["W"]
+    nv, nw = np.linalg.norm(V, axis=0), np.linalg.norm(W, axis=0)
+    dV = kap * kap * gamma(N) * nv + nli * np.linalg.norm(dk, axis=0)
+    dW = kap * kap * gamma(N) * nw + nli * dV
+    a0 = np.abs(alpha[:, 0])[:, None]
+    aW = np.abs(W)
+    gN = gamma(N + 2)
+    bmu_u, bs2_u, gu_mu, gu_s2 = [], [], [], []
+    for e in range(De):
+        aq, acq = np.abs(Q[e]), np.abs(cc * Q[e])
+        pert = np.abs(cc) * dQ[e] + aq * dc
+        bmu_u.append((a0 * pert).sum(0) + gN * (a0 * acq).sum(0))
+        bs2_u.append(2.0 * ((aW * pert).sum(0) + gN * (aW * acq).sum(0) + np.linalg.norm(acq, axis=0) * dW))
+        gu_mu.append(np.abs((cc * Q[e]).T @ alpha[:, 0]))
+        gu_s2.append(np.abs(2.0 * ((cc * Q[e]) * W).sum(0)))
+    bmu_u, bs2_u = np.stack(bmu_u, 1), np.stack(bs2_u, 1)
+    gu_mu, gu_s2 = np.stack(gu_mu, 1), np.stack(gu_s2, 1)
+    gJ = gamma(De + 3)
+    v2 = nv * nv
+    aal = np.abs(alpha)
+    return dict(
+        mu=gN * (np.abs(k).T @ aal) + dk.T @ aal,
+        s2=2.0 * nv * dV + gN * v2 + 2.0 * U * (sf2 + v2 + abs(noise)),
+        dmu=bmu_u @ aJ.T + gJ * (gu_mu @ aJ.T),
+        ds2=bs2_u @ aJ.T + gJ * (gu_s2 @ aJ.T))
+
+
+def bound_acq(acq_id, params, mu0, s2, dmu, ds2):
+    """(value bound, gradient bound) of the UCB / EI epilogue evaluated in fp64 from given mu (output 0 plus the mean),
+    sigma^2, grad mu and grad sigma^2, on the device and on the host (oracle/acq_grad.ucb / ei) together.
+      UCB: v = mu + a sigma, g = grad mu + a grad s2 / (2 sigma): 4 roundings each side on |mu| + |a sigma| and on
+           |grad mu| + |a grad s2 / 2 sigma|.
+      EI:  X = mu - f - j (|dX| <= 2u(|mu| + |f| + |j|)), Z = X / sigma (|dZ| <= |dX| / sigma + 3u |Z|), Phi = erfc(-Z/sqrt2)/2
+           (erfc <= 5 ulp on either side, plus phi |dZ| + u phi |Z| from its argument), phi = exp(-Z^2/2)/sqrt(2 pi)
+           (phi (|Z| |dZ| + 6u)); g = Phi grad mu + phi grad s2 / (2 sigma) with 4 more roundings per term; the value
+           X Phi + sigma phi likewise."""
+    mu0, s2 = np.asarray(mu0), np.asarray(s2)
+    sg = np.sqrt(s2)
+    if acq_id == 0:
+        aa = params[0]
+        t = np.abs(aa * ds2 / (2.0 * sg)[:, None])
+        return 2 * 4.0 * U * (np.abs(mu0) + np.abs(aa) * sg), 2 * 4.0 * U * (np.abs(dmu) + t)
+    f, j = params
+    from scipy.special import erfc
+    Xv = mu0 - f - j
+    Z = Xv / sg
+    phi = np.exp(-0.5 * Z * Z) / math.sqrt(2.0 * math.pi)
+    Phi = 0.5 * erfc(-Z / math.sqrt(2.0))
+    dX = 2.0 * U * (np.abs(mu0) + abs(f) + abs(j))
+    dZ = dX / sg + 3.0 * U * np.abs(Z)
+    dPhi = 10.0 * U * Phi + phi * dZ + U * phi * np.abs(Z)
+    dphi = phi * (np.abs(Z) * dZ + 6.0 * U)
+    t = np.abs(ds2 / (2.0 * sg)[:, None])
+    bg = dPhi[:, None] * np.abs(dmu) + dphi[:, None] * t + 2 * 4.0 * U * (Phi[:, None] * np.abs(dmu) + phi[:, None] * t)
+    bv = np.abs(Xv) * dPhi + Phi * dX + sg * dphi + 2 * 4.0 * U * (np.abs(Xv) * Phi + sg * phi)
+    return bv, bg
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # the device side (C ABI, include/limbo_b200.h)
 # ---------------------------------------------------------------------------------------------------------------------
 class Handle:
     """One lb_gp handle on device 0."""
 
-    def __init__(self, lib):
+    def __init__(self, lib, precision: int = 0):
         import ctypes as C
         from limbo_b200 import _lib
         self.C, self._lib, self.lib = C, _lib, lib
         lib.lb_debug_force_unfused_query.argtypes = [C.c_void_p, C.c_int]
         lib.lb_debug_force_unfused_query.restype = C.c_int
         self.h = C.c_void_p()
-        _lib.check(lib.lb_create(C.byref(self.h), 0, 0), "lb_create")
+        _lib.check(lib.lb_create(C.byref(self.h), 0, precision), "lb_create")
 
     def close(self):
         if self.h:
@@ -374,6 +582,9 @@ class Handle:
         L = np.asfortranarray(L, dtype=np.float64)
         alpha = np.asfortranarray(alpha, dtype=np.float64)
         self._lib.check(self.lib.lb_load_factor(self.h, L.ctypes.data, alpha.ctypes.data), "lb_load_factor")
+
+    def fit(self):
+        self._lib.check(self.lib.lb_fit(self.h), "lb_fit")
 
     def factor(self, K) -> int:
         """Factor K in place of the stored factor: lb_load_factor puts K (and the identity in the padding) where lb_fit's
@@ -417,6 +628,41 @@ class Handle:
         finally:
             self.lib.lb_debug_force_unfused_query(self.h, 0)
         return mu, s2
+
+    def query_grad(self, Xq):
+        """lb_query_grad: mu (M x P), sigma^2, grad mu and grad sigma^2 (M x D)."""
+        Xq = np.ascontiguousarray(Xq, dtype=np.float64)
+        M = Xq.shape[0]
+        mu, s2, dmu, ds2 = np.empty((M, self.P)), np.empty(M), np.empty((M, self.D)), np.empty((M, self.D))
+        self._lib.check(self.lib.lb_query_grad(self.h, M, Xq.ctypes.data, mu.ctypes.data, s2.ctypes.data, dmu.ctypes.data,
+                                               ds2.ctypes.data), "lb_query_grad")
+        return mu, s2, dmu, ds2
+
+    def acq_grad(self, acq_id, params, Xq, mean=None, mean_const=0.0, mean_grad=None):
+        """lb_acq_grad: the acquisition's values and gradients (M, M x D)."""
+        Xq = np.ascontiguousarray(Xq, dtype=np.float64)
+        M = Xq.shape[0]
+        ap = np.array(list(params) + [0.0] * (2 - len(params)), dtype=np.float64)
+        mean = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+        mean_grad = None if mean_grad is None else np.ascontiguousarray(mean_grad, dtype=np.float64)
+        v, g = np.empty(M), np.empty((M, self.D))
+        self._lib.check(self.lib.lb_acq_grad(self.h, acq_id, ap.ctypes.data, M, Xq.ctypes.data,
+                                             None if mean is None else mean.ctypes.data, float(mean_const),
+                                             None if mean_grad is None else mean_grad.ctypes.data, v.ctypes.data, g.ctypes.data),
+                        "lb_acq_grad")
+        return v, g
+
+    def acq_argmax(self, acq_id, params, Xq, mean=None, mean_const=0.0):
+        """lb_acq_argmax: (values, best value, best index)."""
+        Xq = np.ascontiguousarray(Xq, dtype=np.float64)
+        M = Xq.shape[0]
+        ap = np.array(list(params) + [0.0] * (2 - len(params)), dtype=np.float64)
+        mean = None if mean is None else np.ascontiguousarray(mean, dtype=np.float64)
+        v, best, idx = np.empty(M), self.C.c_double(), self.C.c_int64()
+        self._lib.check(self.lib.lb_acq_argmax(self.h, acq_id, ap.ctypes.data, M, Xq.ctypes.data,
+                                               None if mean is None else mean.ctypes.data, float(mean_const), v.ctypes.data,
+                                               self.C.addressof(best), self.C.addressof(idx)), "lb_acq_argmax")
+        return v, best.value, idx.value
 
 
 def factor_outputs(h: Handle, case: ExactCase, X) -> dict:

@@ -137,3 +137,101 @@ def test_query_case_conditioning():
     bm = E.bound_mu(1, p, Ks, qc.alpha, 1.0, 3)
     mu2 = np.einsum("ij,ip->jp", Ks, qc.alpha)
     assert np.all(np.abs(mu2 - mu) <= bm)
+
+
+# ---- candidate gradients on a loaded factor ----------------------------------------------------------------------------
+GRAD_CASES = [(0, 3, 0), (0, 3, 2), (1, 3, 0), (2, 3, 0), (3, 3, 0), (0, 17, 1), (1, 17, 0)]
+
+
+def _grad_case(kid, D, klam, N, M, seed, P=2):
+    qc = E.QueryCase(N, D, P, seed)
+    p = E.grad_params(kid, D, klam, qc.rng)
+    Xq = qc.rng.uniform(0.0, 1.0, size=(M, D))
+    return qc, p, Xq
+
+
+@pytest.mark.parametrize("kid,D,klam", GRAD_CASES)
+def test_grad_reference_central_differences(kid, D, klam):
+    """The reference's gradients against central differences of its own mu (output 0) and sigma^2, the factor fixed."""
+    qc, p, Xq = _grad_case(kid, D, klam, 200, 12, 300 + 10 * kid + klam)
+    r = qc.grad_reference(kid, p, 0.01, Xq)
+    H = 1e-5
+    scale = np.maximum(np.abs(np.hstack([r["dmu"], r["ds2"]])).max(axis=1), 1e-3)
+    for d in range(D):
+        e = np.zeros(D)
+        e[d] = H
+        rp, rm = qc.grad_reference(kid, p, 0.01, Xq + e, L=r["L"]), qc.grad_reference(kid, p, 0.01, Xq - e, L=r["L"])
+        fd_mu = (rp["mu"][:, 0] - rm["mu"][:, 0]) / (2 * H)
+        fd_s2 = (rp["s2"] - rm["s2"]) / (2 * H)
+        assert np.all(np.abs(r["dmu"][:, d] - fd_mu) <= 1e-6 * scale), np.abs(r["dmu"][:, d] - fd_mu).max()
+        assert np.all(np.abs(r["ds2"][:, d] - fd_s2) <= 1e-6 * scale), np.abs(r["ds2"][:, d] - fd_s2).max()
+
+
+@pytest.mark.parametrize("kid,D,klam", GRAD_CASES)
+def test_grad_reference_matches_oracle_formulas(kid, D, klam):
+    """oracle/acq_grad.query_grad (K^-1 K* by cho_solve, differences in one M x N x De array) on the same L, within twice
+    the one-evaluation bounds."""
+    from oracle import acq_grad as AG
+    qc, p, Xq = _grad_case(kid, D, klam, 300, 40, 400 + 10 * kid + klam)
+    r = qc.grad_reference(kid, p, 0.01, Xq)
+    b = E.grad_bounds(kid, p, qc.X, Xq, qc.alpha, 0.01, qc.norm_E(), r)
+    mu, s2, dmu, ds2, _ = AG.query_grad(kid, p, 0.01, qc.X, r["L"], qc.alpha, Xq)
+    for name, got in (("mu", mu), ("s2", s2), ("dmu", dmu), ("ds2", ds2)):
+        ratio = float(np.max(np.abs(got - r[name]) / (2.0 * b[name])))
+        print(f"kid={kid} D={D} klam={klam} {name} ratio={ratio:.2e}")
+        assert ratio <= 1.0, name
+
+
+@pytest.mark.parametrize("kid,D,klam,N", [(1, 3, 0, 127), (2, 3, 0, 2049), (3, 16, 0, 300), (0, 15, 2, 1000), (0, 3, 0, 4224),
+                                          (1, 3, 0, 4224)])
+def test_grad_bounds_hold_for_scipy(kid, D, klam, N):
+    """SciPy's fp64 gradients stay inside the one-evaluation bounds against a long-double substitution reference; scaling
+    W's last 128-row tile by 1 + 2^-30 (the size of a one-tile slip of the backward walk) leaves them."""
+    qc, p, Xq = _grad_case(kid, D, klam, N, 6, 500 + N + kid)
+    r = qc.grad_reference(kid, p, 0.01, Xq)
+    b = E.grad_bounds(kid, p, qc.X, Xq, qc.alpha, 0.01, qc.norm_E(), r)
+    mu, s2, dmu, ds2 = E.grad_reference_ld(kid, p, qc.X, Xq, r["L"], qc.alpha)
+    s2 = s2 + 0.01
+    ratios = {}
+    for name, ref in (("mu", mu), ("s2", s2), ("dmu", dmu), ("ds2", ds2)):
+        err = np.abs(r[name] - ref).astype(np.float64)
+        ratios[name] = float(np.max(err / b[name]))
+    print(f"kid={kid} D={D} klam={klam} N={N} ratios", {k: f"{v:.2e}" for k, v in ratios.items()})
+    assert all(v <= 1.0 for v in ratios.values()), ratios
+    # a perturbation the size of the last super-block's 2^-30 slip exceeds the bound
+    W = r["W"].copy()
+    t0 = (N - 1) // 128 * 128
+    W[t0:] *= 1.0 + 2.0 ** -30
+    J = E.staging(kid, p, D)[0]
+    ds2p = np.stack([-2.0 * ((r["c"] * q) * W).sum(0) for q in r["Q"]], axis=1) @ J.T
+    assert float(np.max(np.abs(ds2p - ds2).astype(np.float64) / b["ds2"])) > 1.0
+
+
+def test_acq_bounds_hold_for_long_double():
+    """bound_acq covers the UCB / EI epilogue of oracle/acq_grad against the same formulas in long double."""
+    from oracle import acq_grad as AG
+    rng = np.random.default_rng(600)
+    M, D = 400, 3
+    mu0 = rng.normal(size=M)
+    s2 = np.exp(rng.uniform(-4.0, 1.0, M))
+    dmu, ds2 = rng.normal(size=(M, D)), rng.normal(size=(M, D)) * s2[:, None]
+    for acq_id, params in ((0, [0.6]), (1, [0.4, 0.01]), (1, [3.0, 0.0])):
+        v, g = AG.ucb(mu0, s2, dmu, ds2, params[0]) if acq_id == 0 else AG.ei(mu0, s2, dmu, ds2, *params)
+        bv, bg = E.bound_acq(acq_id, params, mu0, s2, dmu, ds2)
+        ld = np.longdouble
+        sg = np.sqrt(s2.astype(ld))
+        if acq_id == 0:
+            rv = mu0 + ld(params[0]) * sg
+            rg = dmu + ld(params[0]) * ds2 / (2 * sg)[:, None]
+        else:
+            import mpmath
+            Xv = mu0.astype(ld) - ld(params[0]) - ld(params[1])
+            Z = Xv / sg
+            with mpmath.workdps(30):
+                Phi = np.array([ld(str(mpmath.ncdf(mpmath.mpf(str(z))))) for z in Z], dtype=ld)
+            phi = np.exp(-Z * Z / 2) / np.sqrt(2 * ld(np.pi))
+            rv = Xv * Phi + sg * phi
+            rg = Phi[:, None] * dmu + phi[:, None] * ds2 / (2 * sg)[:, None]
+        rv_, rg_ = float(np.max(np.abs(v - rv).astype(np.float64) / bv)), float(np.max(np.abs(g - rg).astype(np.float64) / bg))
+        print(f"acq={acq_id} {params} ratio value={rv_:.2e} grad={rg_:.2e}")
+        assert rv_ <= 1.0 and rg_ <= 1.0
