@@ -12,46 +12,6 @@
 #include <new>
 #include <string>
 
-int lb_launch_potf2_block(lb_gp* h, int k, int do_factor);
-int lb_debug_potf2_clocks(lb_gp* h, int k, long long* out_host, int n);
-int lb_launch_linv(lb_gp* h);
-int lb_launch_symmetrize(lb_gp* h, double* dA);
-int lb_launch_loo_value(lb_gp* h, double* dOut);
-int lb_launch_loo_grad(lb_gp* h, int optimize_noise, double* dGrad);
-int lb_launch_kinv_obs(lb_gp* h, double* dOut);
-int lb_query_fused_supported(const lb_gp* h);
-size_t lb_query_panel_scratch_doubles(const lb_gp* h, int64_t Mp);
-size_t lb_linv_columns_scratch_doubles(const lb_gp* h, int G);
-int lb_launch_linv_columns(lb_gp* h, cudaStream_t st, int rank, int G, double* dWork, long long* launches);
-size_t lb_dinv_chunk_bytes_impl(const lb_gp* h, int G);
-int lb_dinv_absmax(lb_gp* h, const double* dV, int G, double* out);
-int lb_dinv_pack_impl(lb_gp* h, const double* dV, int rank, int G, double absmax_all, void* dChunk);
-int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all);
-int lb_launch_query_point(const lb_gp* h, cudaStream_t st, const double* x_host, double* dQs, double* dVscratch, double* dOutMapped,
-    long long* launches);
-int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
-    long long* launches);
-int lb_launch_query_grad(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
-    const LbGradOut& out, long long* launches);
-int lb_launch_prior_grad(cudaStream_t st, int64_t M, int D, int P, double s2, const LbGradOut& out, double* dMu, double* dS2);
-size_t lb_query_fused_scratch_doubles(const lb_gp* h, int grid);
-int lb_launch_query_fused(const lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dVscratch,
-    int grid, double* dMu, double* dS2, long long* launches);
-int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu, int mu_stride,
-    const double* dMeanAtQ, double mean_const, const double* dS2, double* dAcq, double* dBlkVal, long long* dBlkIdx,
-    double* dBestVal, long long* dBestIdx, long long* launches);
-int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
-    double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
-    const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches);
-int lb_launch_values_argmax(cudaStream_t st, int64_t M, const double* dVals, double* dBlkVal, long long* dBlkIdx, double* dBestVal,
-    long long* dBestIdx, long long* launches);
-int lb_launch_ehvi(cudaStream_t st, double r0, double r1, int64_t k, const double* dFront, int64_t M, const double* dMu0, int p0,
-    const double* dMean0, double mean0_const, const double* dS2_0, const double* dMu1, int p1, const double* dMean1, double mean1_const,
-    const double* dS2_1, double* dAcq, long long* launches);
-int lb_launch_pareto(cudaStream_t st, int64_t n, int K, const double* dObjs, int* dKeep, int* dErr, long long* launches);
-int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const double* dX, int64_t max_points, long long* dKept,
-    int64_t* n_kept, long long* dRemoved, double* dRemovedScore, long long* launches);
-
 static thread_local std::string g_last_cuda_error;
 void lb_set_last_cuda_error(cudaError_t e, const char* file, int line)
 {
@@ -129,6 +89,7 @@ struct lb_gp_full : lb_gp {
     Extra ex;
 };
 static inline lb_gp_full* full(const lb_gp* h) { return static_cast<lb_gp_full*>(const_cast<lb_gp*>(h)); }
+static inline int n_outputs(const lb_gp* h) { return h->P > 0 ? h->P : 1; } // columns of mu (a handle without observations: 1)
 
 namespace {
 
@@ -256,6 +217,15 @@ __global__ void append_row_kernel(double* __restrict__ L, int64_t np, int64_t n,
     }
 }
 
+// byte sizes of the six buffers lb_clone shares, for a model of padded order Np (invD: Np / LB_TILE blocks of LB_TILE x LB_TILE)
+struct SharedBytes { size_t X, Xs, Y, L, InvD, Alpha; };
+SharedBytes shared_bytes(int64_t Np, int D, int P)
+{
+    const size_t row = sizeof(double) * Np;
+    return {row * D, row * (D + LB_MAX_LAMBDA), row * P, row * Np, row * LB_TILE, row * P};
+}
+SharedBytes shared_bytes(const lb_gp* h) { return shared_bytes(h->Np, h->D, h->P); }
+
 // callers synchronise the handle's stream first
 void free_model(lb_gp* h)
 {
@@ -269,31 +239,20 @@ void free_model(lb_gp* h)
     h->Np = 0;
 }
 
-int alloc_model(lb_gp* h, int64_t Np, int D, int P)
+// What every (re)factorisation starts with.  Private Xs / L / invD / alpha: allocated when missing, replaced without a copy when
+// still shared with a clone (every byte is rewritten by the fit); then the samples staged for the kernel in Xs.
+int stage_fit(lb_gp* h)
 {
-    const int64_t T = Np / LB_TILE;
-    LB_ALLOC(h, h->dX, sizeof(double) * D * Np);
-    LB_ALLOC(h, h->dY, sizeof(double) * P * Np);
-    int rc = h->dFlags.resize(h, sizeof(int) * (T + 8));
-    if (rc) return rc;
-    h->Np = Np;
-    return LB_OK; // Xs, L, invD, alpha: ensure_fit_buffers (a clone that refits never needs its source's copies)
-}
-
-// Private Xs / L / invD / alpha for a handle that is about to (re)factorise: allocated when missing, replaced without a
-// copy when still shared with a clone (every byte is rewritten by the fit).
-int ensure_fit_buffers(lb_gp* h)
-{
-    const int64_t Np = h->Np, T = Np / LB_TILE;
+    const SharedBytes sz = shared_bytes(h);
     int rc;
     bool fresh = false;
-    if ((rc = make_unique(h, &h->dXs, sizeof(double) * (h->D + LB_MAX_LAMBDA) * Np, false))) return rc;
-    if ((rc = make_unique(h, &h->dL, sizeof(double) * Np * Np, false))) return rc;
-    if ((rc = make_unique(h, &h->dAlpha, sizeof(double) * h->P * Np, false))) return rc;
-    if ((rc = make_unique(h, &h->dInvD, sizeof(double) * T * LB_TILE * LB_TILE, false, &fresh))) return rc;
+    if ((rc = make_unique(h, &h->dXs, sz.Xs, false))) return rc;
+    if ((rc = make_unique(h, &h->dL, sz.L, false))) return rc;
+    if ((rc = make_unique(h, &h->dAlpha, sz.Alpha, false))) return rc;
+    if ((rc = make_unique(h, &h->dInvD, sz.InvD, false, &fresh))) return rc;
     if (fresh) // the panel kernels only write the lower part of every block; consumers read whole blocks
-        LB_CUDA(cudaMemsetAsync(h->dInvD, 0, sizeof(double) * T * LB_TILE * LB_TILE, h->stream));
-    return LB_OK;
+        LB_CUDA(cudaMemsetAsync(h->dInvD, 0, sz.InvD, h->stream));
+    return lb_launch_scale_x(h);
 }
 
 int check_info(lb_gp* h)
@@ -306,10 +265,49 @@ int check_info(lb_gp* h)
     return LB_OK;
 }
 
-int upload_kernel_scaled(lb_gp* h)
+// lb_fit without the final host sync / info read
+int fit_enqueue(lb_gp* h)
 {
-    if (h->N == 0 && h->Np == 0) return LB_OK;
-    return lb_launch_scale_x(h);
+    int rc;
+    if ((rc = stage_fit(h))) return rc;
+    if ((rc = lb_launch_kbuild(h, h->dL))) return rc;
+    if ((rc = lb_launch_potrf(h))) return rc;
+    h->fitted = true;
+    lb_factor_changed(h);
+    return lb_launch_solve_alpha(h);
+}
+
+// The M candidates Xq (row-major M x D) on the device: Xq itself when dev, otherwise a copy in h's dQraw, uploaded on h->stream.
+int candidates_on_device(lb_gp_full* h, const double* Xq, int64_t M, bool dev, const double** out)
+{
+    *out = Xq;
+    if (dev) return LB_OK;
+    QueryWs& w = h->ex.ws;
+    int rc = ensure(h, w.dQraw, sizeof(double) * M * h->D);
+    if (rc) return rc;
+    LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * h->D, cudaMemcpyHostToDevice, h->stream));
+    *out = w.dQraw.get();
+    return LB_OK;
+}
+
+// The candidate-chunk loop of every query path: sizes h's dQs for De x Mc and dV for the path's v_doubles of scratch, and per chunk of
+// at most Mc candidates stages it for the kernel in dQs (De x mcp, mcp = mc rounded up to `granule`, zero padded) and calls body(m0, mc, mcp).
+template <typename Body>
+int for_each_chunk(lb_gp_full* h, const double* dQraw, int64_t M, int64_t Mc, int64_t granule, size_t v_doubles, Body&& body)
+{
+    DevBuf<double>& dQs = h->ex.ws.dQs;
+    const int D = h->D, De = h->kp.D; // raw / staged input dimension
+    int rc;
+    if ((rc = ensure(h, dQs, sizeof(double) * De * Mc)) || (rc = ensure(h, h->ex.ws.dV, sizeof(double) * v_doubles))) return rc;
+    for (int64_t m0 = 0; m0 < M; m0 += Mc) {
+        const int64_t mc = std::min(Mc, M - m0);
+        const int64_t mcp = (mc + granule - 1) / granule * granule;
+        dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
+        pack_soa_kernel<<<g1, 256, 0, h->stream>>>(dQraw + m0 * D, mc, D, dQs.get(), mcp, h->kp, 1);
+        h->launches++;
+        if ((rc = body(m0, mc, mcp))) return rc;
+    }
+    return LB_OK;
 }
 
 } // namespace
@@ -442,17 +440,17 @@ static int set_data_common(lb_gp* h, int64_t N, int D, int P, const double* X, c
     if (N > 0 && (!X || !Y)) return LB_ERR_ARG;
     LB_DEVICE(h);
     const int64_t Np = std::max<int64_t>(LB_TILE, (N + LB_TILE - 1) / LB_TILE * LB_TILE);
-    if (Np != h->Np || D != h->D || P != h->P) {
+    const bool reshape = Np != h->Np || D != h->D || P != h->P;
+    if (reshape) {
         LB_CUDA(cudaStreamSynchronize(h->stream));
         free_model(h);
-        int rc = alloc_model(h, Np, D, P);
-        if (rc) return rc;
     }
-    else { // same shape: rewrite in place unless a clone still reads the buffers
-        int rc;
-        if ((rc = make_unique(h, &h->dX, sizeof(double) * D * Np, false))) return rc;
-        if ((rc = make_unique(h, &h->dY, sizeof(double) * P * Np, false))) return rc;
-    }
+    // X and Y, rewritten in place unless a clone still reads them; Xs, L, invD, alpha: stage_fit (a clone that refits never needs its source's)
+    const SharedBytes sz = shared_bytes(Np, D, P);
+    int rc;
+    if ((rc = make_unique(h, &h->dX, sz.X, false)) || (rc = make_unique(h, &h->dY, sz.Y, false))) return rc;
+    if (reshape && (rc = h->dFlags.resize(h, sizeof(int) * (Np / LB_TILE + 8)))) return rc;
+    h->Np = Np;
     if (D != h->D) h->kp.klam = 0; // the Lambda matrix belongs to the previous input dimension
     h->N = N; h->D = D; h->P = P;
     h->kp.Draw = D;
@@ -486,8 +484,8 @@ int lb_dchol_set_points(lb_gp* h, int64_t N, int D, const double* X)
     LB_CUDA(cudaStreamSynchronize(h->stream));
     free_model(h);
     const int64_t Np = (N + LB_TILE - 1) / LB_TILE * LB_TILE;
-    LB_ALLOC(h, h->dX, sizeof(double) * D * Np);
-    LB_ALLOC(h, h->dXs, sizeof(double) * (D + LB_MAX_LAMBDA) * Np);
+    LB_ALLOC(h, h->dX, shared_bytes(Np, D, 0).X);
+    LB_ALLOC(h, h->dXs, shared_bytes(Np, D, 0).Xs);
     h->Np = Np;
     if (D != h->D) h->kp.klam = 0;
     h->N = N; h->D = D; h->P = 0;
@@ -585,15 +583,8 @@ int lb_fit(lb_gp* h)
     if (!h->kernel_set || h->Np == 0 || !h->dX) return LB_ERR_STATE;
     LB_DEVICE(h);
     if (h->N == 0) return LB_ERR_STATE; // gp.hpp:90 assert(samples.size() != 0)
-    int rc;
-    if ((rc = ensure_fit_buffers(h))) return rc;
-    if ((rc = lb_launch_scale_x(h))) return rc;
-    if ((rc = lb_launch_kbuild(h, h->dL))) return rc;
-    if ((rc = lb_launch_potrf(h))) return rc;
-    h->fitted = true;
-    lb_factor_changed(h);
-    if ((rc = lb_launch_solve_alpha(h))) return rc;
-    return check_info(h);
+    int rc = fit_enqueue(h);
+    return rc ? rc : check_info(h);
 }
 
 int lb_fit_async(lb_gp* h) // same as lb_fit without the final host sync / info read (bench "value" leg)
@@ -601,14 +592,7 @@ int lb_fit_async(lb_gp* h) // same as lb_fit without the final host sync / info 
     if (!h) return LB_ERR_ARG;
     if (!h->kernel_set || h->Np == 0 || h->N == 0 || !h->dX) return LB_ERR_STATE;
     LB_DEVICE(h);
-    int rc;
-    if ((rc = ensure_fit_buffers(h))) return rc;
-    if ((rc = lb_launch_scale_x(h))) return rc;
-    if ((rc = lb_launch_kbuild(h, h->dL))) return rc;
-    if ((rc = lb_launch_potrf(h))) return rc;
-    h->fitted = true;
-    lb_factor_changed(h);
-    return lb_launch_solve_alpha(h);
+    return fit_enqueue(h);
 }
 
 int lb_check_info(lb_gp* h)
@@ -633,9 +617,8 @@ int lb_stage_kbuild(lb_gp* h)
 {
     if (!h || !h->kernel_set || h->N == 0) return LB_ERR_STATE;
     LB_DEVICE(h);
-    int rc;
-    if ((rc = ensure_fit_buffers(h))) return rc;
-    if ((rc = lb_launch_scale_x(h))) return rc;
+    int rc = stage_fit(h);
+    if (rc) return rc;
     h->fitted = false;
     return lb_launch_kbuild(h, h->dL);
 }
@@ -664,8 +647,7 @@ int lb_load_factor(lb_gp* h, const double* L_colmajor, const double* alpha_colma
     const int64_t N = h->N, Np = h->Np;
     const int T = (int)(Np / LB_TILE);
     int rc;
-    if ((rc = ensure_fit_buffers(h))) return rc;
-    if ((rc = lb_launch_scale_x(h))) return rc;
+    if ((rc = stage_fit(h))) return rc;
     LB_CUDA(cudaMemsetAsync(h->dL, 0, sizeof(double) * Np * Np, h->stream));
     LB_CUDA(cudaMemcpy2DAsync(h->dL, Np * 8, L_colmajor, N * 8, N * 8, N, cudaMemcpyHostToDevice, h->stream));
     identity_pad_kernel<<<1024, 256, 0, h->stream>>>(h->dL, Np, N);
@@ -687,8 +669,8 @@ int lb_refit_alpha(lb_gp* h, const double* Y)
     LB_DEVICE(h);
     int rc = lb_ensure_scratch(h, sizeof(double) * (size_t)h->N * h->P);
     if (rc) return rc;
-    if ((rc = make_unique(h, &h->dY, sizeof(double) * h->P * h->Np, false))) return rc;
-    if ((rc = make_unique(h, &h->dAlpha, sizeof(double) * h->P * h->Np, false))) return rc;
+    if ((rc = make_unique(h, &h->dY, shared_bytes(h).Y, false))) return rc;
+    if ((rc = make_unique(h, &h->dAlpha, shared_bytes(h).Alpha, false))) return rc;
     LB_CUDA(cudaMemcpyAsync(h->dScratch.get(), Y, sizeof(double) * h->N * h->P, cudaMemcpyHostToDevice, h->stream));
     dim3 g2((unsigned)((h->Np + 255) / 256), (unsigned)h->P);
     pad_cols_kernel<<<g2, 256, 0, h->stream>>>(h->dScratch.get(), h->N, h->P, h->dY, h->Np);
@@ -708,21 +690,22 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
     if (n + 1 > h->Np) { // grow by one tile, keep the factor
         const int64_t oldNp = h->Np, newNp = oldNp + LB_TILE;
         const int64_t oldT = oldNp / LB_TILE, newT = newNp / LB_TILE;
+        const SharedBytes sz = shared_bytes(newNp, D, P);
         double *nX, *nXs, *nY, *nA, *nL, *nI;
         LB_CUDA(cudaStreamSynchronize(h->stream));
-        LB_ALLOC(h, nX, sizeof(double) * D * newNp);
-        LB_ALLOC(h, nXs, sizeof(double) * (D + LB_MAX_LAMBDA) * newNp);
-        LB_ALLOC(h, nY, sizeof(double) * P * newNp);
-        LB_ALLOC(h, nA, sizeof(double) * P * newNp);
-        LB_ALLOC(h, nL, sizeof(double) * newNp * newNp);
-        LB_ALLOC(h, nI, sizeof(double) * newT * LB_TILE * LB_TILE);
+        LB_ALLOC(h, nX, sz.X);
+        LB_ALLOC(h, nXs, sz.Xs);
+        LB_ALLOC(h, nY, sz.Y);
+        LB_ALLOC(h, nA, sz.Alpha);
+        LB_ALLOC(h, nL, sz.L);
+        LB_ALLOC(h, nI, sz.InvD);
         int rc = h->dFlags.resize(h, sizeof(int) * (newT + 8));
         if (rc) return rc;
-        LB_CUDA(cudaMemsetAsync(nX, 0, sizeof(double) * D * newNp, h->stream));
-        LB_CUDA(cudaMemsetAsync(nY, 0, sizeof(double) * P * newNp, h->stream));
+        LB_CUDA(cudaMemsetAsync(nX, 0, sz.X, h->stream));
+        LB_CUDA(cudaMemsetAsync(nY, 0, sz.Y, h->stream));
         LB_CUDA(cudaMemcpy2DAsync(nX, newNp * 8, h->dX, oldNp * 8, oldNp * 8, D, cudaMemcpyDeviceToDevice, h->stream));
         LB_CUDA(cudaMemcpy2DAsync(nL, newNp * 8, h->dL, oldNp * 8, oldNp * 8, oldNp, cudaMemcpyDeviceToDevice, h->stream));
-        LB_CUDA(cudaMemcpyAsync(nI, h->dInvD, sizeof(double) * oldT * LB_TILE * LB_TILE, cudaMemcpyDeviceToDevice, h->stream));
+        LB_CUDA(cudaMemcpyAsync(nI, h->dInvD, shared_bytes(oldNp, D, P).InvD, cudaMemcpyDeviceToDevice, h->stream));
         identity_pad_kernel<<<1024, 256, 0, h->stream>>>(nL, newNp, oldNp);
         identity_blocks_kernel<<<(unsigned)(newT - oldT), 256, 0, h->stream>>>(nI, (int)oldT, (int)newT);
         h->launches += 2;
@@ -736,13 +719,13 @@ int lb_append(lb_gp* h, const double* x, const double* Yall)
     int rc = lb_ensure_scratch(h, sizeof(double) * (size_t)((n + 1) * P + D + Np));
     if (rc) return rc;
     { // copy-on-write: a clone may still read these (the row update keeps the rest of X, L, invD)
-        const int64_t T = Np / LB_TILE;
-        if ((rc = make_unique(h, &h->dX, sizeof(double) * D * Np, true))) return rc;
-        if ((rc = make_unique(h, &h->dL, sizeof(double) * Np * Np, true))) return rc;
-        if ((rc = make_unique(h, &h->dInvD, sizeof(double) * T * LB_TILE * LB_TILE, true))) return rc;
-        if ((rc = make_unique(h, &h->dY, sizeof(double) * P * Np, false))) return rc;
-        if ((rc = make_unique(h, &h->dXs, sizeof(double) * (D + LB_MAX_LAMBDA) * Np, false))) return rc;
-        if ((rc = make_unique(h, &h->dAlpha, sizeof(double) * P * Np, false))) return rc;
+        const SharedBytes sz = shared_bytes(h);
+        if ((rc = make_unique(h, &h->dX, sz.X, true))) return rc;
+        if ((rc = make_unique(h, &h->dL, sz.L, true))) return rc;
+        if ((rc = make_unique(h, &h->dInvD, sz.InvD, true))) return rc;
+        if ((rc = make_unique(h, &h->dY, sz.Y, false))) return rc;
+        if ((rc = make_unique(h, &h->dXs, sz.Xs, false))) return rc;
+        if ((rc = make_unique(h, &h->dAlpha, sz.Alpha, false))) return rc;
     }
     full(h)->ex.n_append++;
     double* dYs = h->dScratch.get();
@@ -786,109 +769,126 @@ extern "C" int lb_debug_set_query_panel_min(long long m)
     return LB_OK;
 }
 
-// Fills h's query workspace, w.dMu.get() (M x P, k^T alpha) and w.dS2.get() (M), for M candidates on h->stream: the prior, the
-// reduced-precision path, the panel path for large batches, the fused slab path or the multi-launch path.  Xq is row-major
-// M x D, a device pointer when xq_dev.  The caller holds h->ex.qmutex and has checked the handle's state.  A reduced-precision
-// fill leaves its timeout flag in w.dErr (query_timed_out).
-static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
+// The path a batch of M candidates takes on h.  host_point: the call has the shape of the one-point kernel (the candidate and the
+// results on the host, no acquisition); lb_query of one point then always takes that kernel, whatever the panel threshold.
+enum QueryPath { QP_PRIOR, QP_POINT, QP_REDUCED, QP_PANEL, QP_SLAB, QP_MULTI };
+static QueryPath query_path(const lb_gp* h, int64_t M, bool host_point = false)
+{
+    if (h->N == 0 || !h->fitted) return QP_PRIOR;
+    if (h->precision != LB_PREC_FP64) return QP_REDUCED;
+    if (h->force_unfused) return QP_MULTI;
+    const bool fused = lb_query_fused_supported(h);
+    if (host_point && M == 1 && fused) return QP_POINT;
+    if (M >= query_panel_min()) return QP_PANEL;
+    return fused ? QP_SLAB : QP_MULTI;
+}
+
+// Widest candidate chunk, a multiple of the tile, whose V (Np x Mc doubles) stays within `bytes`; no wider than the padded batch
+static int64_t v_chunk(const lb_gp* h, int64_t M, int64_t bytes)
+{
+    const int64_t Mp = (M + LB_TILE - 1) / LB_TILE * LB_TILE;
+    return std::min(Mp, std::max<int64_t>(LB_TILE, bytes / (8 * h->Np) / LB_TILE * LB_TILE));
+}
+// the panel path and the gradients: candidate chunks bounded so that V (Np x Mc) stays <= ~6 GiB
+static int64_t panel_chunk(const lb_gp* h, int64_t M) { return v_chunk(h, M, (int64_t)6 << 30); }
+// the multi-launch path: candidate chunks bounded so that V (Np x Mc) stays <= ~4 GiB
+static int64_t multi_chunk(const lb_gp* h, int64_t M) { return v_chunk(h, M, (int64_t)4 << 30); }
+// The reduced-precision path: candidate chunks of k x (SMs x 128 candidates), whole waves of the persistent wgmma GEMM (one
+// 128-candidate tile per CTA per wave); K*^T chunk <= 4 GiB.
+static int64_t reduced_chunk(const lb_gp* h, int64_t M, int sms)
+{
+    const int64_t CH = 2 * LB_TILE, wave = (int64_t)(sms / 2) * CH;
+    const int64_t cap = std::max<int64_t>(CH, ((int64_t)4 << 30) / (4 * h->Np) / CH * CH);
+    return std::min((M + CH - 1) / CH * CH, (cap >= wave) ? cap / wave * wave : cap);
+}
+
+// The fills of query_fill, one per path: h's dMu (M x P) and dS2 (M) from the row-major device candidates dQraw, on h->stream.
+// The prior, gp.hpp:161-163: mu = mean(v) (added by the caller), sigma2 = k(v,v) + noise
+static int fill_prior(lb_gp_full* h, int64_t M)
+{
+    LB_CUDA(cudaMemsetAsync(h->ex.ws.dMu.get(), 0, sizeof(double) * M * n_outputs(h), h->stream));
+    fill_kernel<<<(unsigned)((M + 255) / 256), 256, 0, h->stream>>>(h->ex.ws.dS2.get(), M, h->kp.sf2 + h->kp.noise);
+    h->launches++;
+    return LB_OK;
+}
+
+// reduced-precision variance on wgmma (tf32_query.cu); mu is accumulated in fp64 from the fp64 kernel values
+static int fill_reduced(lb_gp_full* h, int64_t M, const double* dQraw)
 {
     QueryWs& w = h->ex.ws;
     cudaStream_t st = h->stream;
-    const int D = h->D, De = h->kp.D, P = h->P > 0 ? h->P : 1; // raw / staged input dimension
+    const int P = n_outputs(h);
+    int rc, sms = 132;
+    if ((rc = lb_tf32_prepare(h))) return rc;
+    LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    const int64_t Mc = reduced_chunk(h, M, sms);
+    if ((rc = ensure(h, w.dKt, sizeof(float) * (size_t)Mc * h->Np))) return rc;
+    if ((rc = ensure(h, w.dNorm2, sizeof(double) * (size_t)Mc))) return rc; // Mc floats (split mode: Mc doubles)
+    if ((rc = ensure(h, w.dBias, sizeof(double) * Mc))) return rc;
+    if ((rc = w.dErr.reserve(h, sizeof(int)))) return rc;
+    LB_CUDA(cudaMemsetAsync(w.dErr.get(), 0, sizeof(int), st));
+    const size_t partials = (size_t)(P + 1) * (h->Np / LB_TILE) * Mc; // dV: mean (+ bias) partials per training tile
+    return for_each_chunk(h, dQraw, M, Mc, 2 * LB_TILE, partials, [&](int64_t m0, int64_t mc, int64_t mcp) {
+        double* dBias = (h->precision == LB_PREC_FP16X3) ? nullptr : w.dBias.get(); // 22-bit operands: no rounding-bias term
+        int rc = lb_launch_kstar_tf32(h, st, mc, w.dQs.get(), mcp, w.dKt.get(), w.dV.get(), w.dMu.get() + m0 * P, dBias, &h->launches);
+        if (rc) return rc;
+        return lb_launch_sigma_tf32(h, st, mc, mcp, w.dKt.get(), w.dNorm2.get(), w.dErr.get(), dBias, w.dS2.get() + m0, &h->launches);
+    });
+}
+
+// large batches: blocked solve over 2048-row super-blocks on the GEMM core (query.cu, namespace panel)
+static int fill_panel(lb_gp_full* h, int64_t M, const double* dQraw)
+{
+    QueryWs& w = h->ex.ws;
+    const int64_t Mc = panel_chunk(h, M);
+    return for_each_chunk(h, dQraw, M, Mc, LB_TILE, lb_query_panel_scratch_doubles(h, Mc), [&](int64_t m0, int64_t mc, int64_t mcp) {
+        return lb_launch_query_panel(h, h->stream, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * n_outputs(h), w.dS2.get() + m0,
+            &h->launches);
+    });
+}
+
+// fused persistent path: one CTA per candidate slab, private V scratch per CTA; the whole padded batch is one chunk
+static int fill_slab(lb_gp_full* h, int64_t M, const double* dQraw)
+{
+    QueryWs& w = h->ex.ws;
+    int sms = 0;
+    LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    const int grid = (int)std::min<int64_t>(sms, (M + 7) / 8);
     const int64_t Mp = (M + LB_TILE - 1) / LB_TILE * LB_TILE;
+    return for_each_chunk(h, dQraw, M, Mp, LB_TILE, lb_query_fused_scratch_doubles(h, grid), [&](int64_t, int64_t mc, int64_t mcp) {
+        return lb_launch_query_fused(h, h->stream, mc, w.dQs.get(), mcp, w.dV.get(), grid, w.dMu.get(), w.dS2.get(), &h->launches);
+    });
+}
+
+// one launch per step of the solve (query.cu): the only path for D > DMAXF or P > PMAXF, and the tests' reference
+static int fill_multi(lb_gp_full* h, int64_t M, const double* dQraw)
+{
+    QueryWs& w = h->ex.ws;
+    const int64_t Mc = multi_chunk(h, M);
+    return for_each_chunk(h, dQraw, M, Mc, LB_TILE, (size_t)h->Np * Mc, [&](int64_t m0, int64_t mc, int64_t mcp) {
+        return lb_launch_query(h, h->stream, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * n_outputs(h), w.dS2.get() + m0, &h->launches);
+    });
+}
+
+// Fills h's query workspace, w.dMu.get() (M x P, k^T alpha) and w.dS2.get() (M), for M candidates on h->stream, on the path
+// query_path chooses.  Xq is row-major M x D, a device pointer when xq_dev.  The caller holds h->ex.qmutex and has checked the
+// handle's state.  A reduced-precision fill leaves its timeout flag in w.dErr (query_timed_out).
+static int query_fill(lb_gp_full* h, int64_t M, const double* Xq, bool xq_dev)
+{
+    QueryWs& w = h->ex.ws;
     int rc;
-    if ((rc = ensure(h, w.dMu, sizeof(double) * M * P))) return rc;
+    if ((rc = ensure(h, w.dMu, sizeof(double) * M * n_outputs(h)))) return rc;
     if ((rc = ensure(h, w.dS2, sizeof(double) * M))) return rc;
-    const bool prior = (h->N == 0 || !h->fitted);
-    if (prior && h->N != 0) return LB_ERR_STATE;
-    if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma2 = k(v,v) + noise
-        LB_CUDA(cudaMemsetAsync(w.dMu.get(), 0, sizeof(double) * M * P, st));
-        fill_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(w.dS2.get(), M, h->kp.sf2 + h->kp.noise);
-        h->launches++;
+    const QueryPath path = query_path(h, M);
+    if (path == QP_PRIOR) return h->N != 0 ? LB_ERR_STATE : fill_prior(h, M);
+    const double* dQraw = nullptr;
+    if ((rc = candidates_on_device(h, Xq, M, xq_dev, &dQraw))) return rc;
+    switch (path) {
+    case QP_REDUCED: return fill_reduced(h, M, dQraw);
+    case QP_PANEL: return fill_panel(h, M, dQraw);
+    case QP_SLAB: return fill_slab(h, M, dQraw);
+    default: return fill_multi(h, M, dQraw);
     }
-    else {
-        const double* dQraw = Xq;
-        if (!xq_dev) {
-            if ((rc = ensure(h, w.dQraw, sizeof(double) * M * D))) return rc;
-            LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
-            dQraw = w.dQraw.get();
-        }
-        if (h->precision == LB_PREC_TF32 || h->precision == LB_PREC_FP16 || h->precision == LB_PREC_FP16X3) {
-            // reduced-precision variance on wgmma (tf32_query.cu); mu is accumulated in fp64 from the fp64 kernel values
-            if ((rc = lb_tf32_prepare(h))) return rc;
-            // Candidate chunks of k x (SMs x 128 candidates): whole waves of the persistent wgmma GEMM (one 128-candidate tile
-            // per CTA per wave); K*^T chunk <= 4 GiB.
-            int sms = 132;
-            LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-            const int64_t CH = 2 * LB_TILE, wave = (int64_t)(sms / 2) * CH;
-            const int64_t cap = std::max<int64_t>(CH, ((int64_t)4 << 30) / (4 * h->Np) / CH * CH);
-            int64_t Mc = (cap >= wave) ? cap / wave * wave : cap;
-            Mc = std::min((M + CH - 1) / CH * CH, Mc);
-            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
-            if ((rc = ensure(h, w.dKt, sizeof(float) * (size_t)Mc * h->Np))) return rc;
-            if ((rc = ensure(h, w.dNorm2, sizeof(double) * (size_t)Mc))) return rc; // Mc floats (split mode: Mc doubles)
-            if ((rc = ensure(h, w.dV, sizeof(double) * (size_t)(P + 1) * (h->Np / LB_TILE) * Mc))) return rc; // mean (+ bias) partials per training tile
-            if ((rc = ensure(h, w.dBias, sizeof(double) * Mc))) return rc;
-            double* dBiasUse = (h->precision == LB_PREC_FP16X3) ? nullptr : w.dBias.get(); // 22-bit operands: no rounding-bias term
-            if ((rc = w.dErr.reserve(h, sizeof(int)))) return rc;
-            LB_CUDA(cudaMemsetAsync(w.dErr.get(), 0, sizeof(int), st));
-            for (int64_t m0 = 0; m0 < M; m0 += Mc) {
-                const int64_t mc = std::min(Mc, M - m0);
-                const int64_t mcp = (mc + CH - 1) / CH * CH;
-                dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
-                h->launches++;
-                if ((rc = lb_launch_kstar_tf32(h, st, mc, w.dQs.get(), mcp, w.dKt.get(), w.dV.get(), w.dMu.get() + m0 * P, dBiasUse, &h->launches))) return rc;
-                if ((rc = lb_launch_sigma_tf32(h, st, mc, mcp, w.dKt.get(), w.dNorm2.get(), w.dErr.get(), dBiasUse, w.dS2.get() + m0, &h->launches))) return rc;
-            }
-        }
-        else if (M >= query_panel_min() && !h->force_unfused) {
-            // large batches: blocked solve over 2048-row super-blocks on the GEMM core (query.cu, namespace panel);
-            // candidate chunks bounded so that V (Np x Mc) stays <= ~6 GiB
-            const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)6 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
-            const int64_t Mc = std::min(Mp, maxcols);
-            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
-            if ((rc = ensure(h, w.dV, sizeof(double) * lb_query_panel_scratch_doubles(h, Mc)))) return rc;
-            for (int64_t m0 = 0; m0 < M; m0 += Mc) {
-                const int64_t mc = std::min(Mc, M - m0);
-                const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
-                dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-                pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
-                h->launches++;
-                if ((rc = lb_launch_query_panel(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, &h->launches))) return rc;
-            }
-        }
-        else if (lb_query_fused_supported(h) && !h->force_unfused) {
-            // fused persistent path: one CTA per candidate slab, private V scratch per CTA
-            int sms = 0;
-            LB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-            const int64_t ntiles = (M + 7) / 8;
-            const int grid = (int)std::min<int64_t>(sms, ntiles);
-            if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mp))) return rc;
-            if ((rc = ensure(h, w.dV, sizeof(double) * lb_query_fused_scratch_doubles(h, grid)))) return rc;
-            dim3 g1((unsigned)((Mp + 255) / 256), (unsigned)De);
-            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw, M, D, w.dQs.get(), Mp, h->kp, 1);
-            h->launches++;
-            if ((rc = lb_launch_query_fused(h, st, M, w.dQs.get(), Mp, w.dV.get(), grid, w.dMu.get(), w.dS2.get(), &h->launches))) return rc;
-        }
-        else {
-        // candidate chunks bounded so that V (Np x Mc) stays <= ~4 GiB
-        int64_t Mc = Mp;
-        const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)4 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
-        if (Mc > maxcols) Mc = maxcols;
-        if ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc))) return rc;
-        if ((rc = ensure(h, w.dV, sizeof(double) * h->Np * Mc))) return rc;
-        for (int64_t m0 = 0; m0 < M; m0 += Mc) {
-            const int64_t mc = std::min(Mc, M - m0);
-            const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
-            dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-            pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
-            h->launches++;
-            if ((rc = lb_launch_query(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, &h->launches))) return rc;
-        }
-        }
-    }
-    return LB_OK;
 }
 
 // A device copy of mean_at_q (M values) on h's stream, or mean_at_q itself when it already is a device pointer (or NULL)
@@ -927,10 +927,9 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
     std::lock_guard<std::mutex> lock(h->ex.qmutex);
     QueryWs& w = h->ex.ws;
     cudaStream_t st = h->stream;
-    const int De = h->kp.D, P = h->P > 0 ? h->P : 1;
+    const int De = h->kp.D, P = n_outputs(h);
     int rc;
-    const bool prior = (h->N == 0 || !h->fitted);
-    if (M == 1 && !prior && !xq_dev && !out_dev && !with_acq && h->precision == LB_PREC_FP64 && lb_query_fused_supported(h) && !h->force_unfused) {
+    if (query_path(h, M, !xq_dev && !out_dev && !with_acq) == QP_POINT) {
         // one launch, one synchronisation (query.cu: query_point_kernel)
         Extra& ex = h->ex;
         if (ex.point_cap < P + 1) {
@@ -1020,7 +1019,7 @@ static int grad_common(const lb_gp* hc, int64_t M, const double* Xq, bool dev, d
     lb_gp_full* h = full(hc);
     if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
     if (h->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
-    const int D = h->D, De = h->kp.D, P = h->P > 0 ? h->P : 1;
+    const int D = h->D, P = n_outputs(h);
     if (!dev)
         for (int64_t i = 0; i < M * D; ++i)
             if (!std::isfinite(Xq[i])) return LB_ERR_ARG;
@@ -1030,15 +1029,11 @@ static int grad_common(const lb_gp* hc, int64_t M, const double* Xq, bool dev, d
     cudaStream_t st = h->stream;
     const double p0 = acq_id >= 0 ? acq_params[0] : 0.0, p1 = acq_id == LB_ACQ_EI ? acq_params[1] : 0.0;
     const cudaMemcpyKind d2o = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    const bool prior = (h->N == 0 || !h->fitted);
+    const bool prior = query_path(h, M) == QP_PRIOR;
     if (prior && h->N != 0) return LB_ERR_STATE;
     int rc;
     const double* dQraw = Xq;
-    if (!dev && !prior) {
-        if ((rc = ensure(h, w.dQraw, sizeof(double) * M * D))) return rc;
-        LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
-        dQraw = w.dQraw.get();
-    }
+    if (!prior && (rc = candidates_on_device(h, Xq, M, dev, &dQraw))) return rc;
     if ((rc = ensure(h, w.dMu, sizeof(double) * M * P))) return rc;
     if ((rc = ensure(h, w.dS2, sizeof(double) * M))) return rc;
     StreamTemps tmp(h->device, st); // host mode: device copies of the outputs and of the means
@@ -1070,36 +1065,26 @@ static int grad_common(const lb_gp* hc, int64_t M, const double* Xq, bool dev, d
             dMeanGrad = p;
         }
     }
-    if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma^2 = k(v, v) + noise, both constant in v: zero gradients
-        out.mean = dMean;
-        out.mean_grad = dMeanGrad;
-        out.dmu = dptr[0];
-        out.ds2 = dptr[1];
-        out.acq = dptr[2];
-        out.grad = dptr[3];
-        if ((rc = lb_launch_prior_grad(st, M, D, P, h->kp.sf2 + h->kp.noise, out, w.dMu.get(), w.dS2.get()))) return rc;
-        h->launches++;
-    }
-    // candidate chunks as the panel path of query_fill: V (Np x Mc) <= ~6 GiB
-    const int64_t Mp = (M + LB_TILE - 1) / LB_TILE * LB_TILE;
-    const int64_t maxcols = std::max<int64_t>(LB_TILE, ((int64_t)6 << 30) / (8 * h->Np) / LB_TILE * LB_TILE);
-    const int64_t Mc = prior ? M : std::min(Mp, maxcols);
-    if (!prior && ((rc = ensure(h, w.dQs, sizeof(double) * De * Mc)) || (rc = ensure(h, w.dV, sizeof(double) * lb_query_panel_scratch_doubles(h, Mc)))))
-        return rc;
-    for (int64_t m0 = 0; m0 < M && !prior; m0 += Mc) {
-        const int64_t mc = std::min(Mc, M - m0);
-        const int64_t mcp = (mc + LB_TILE - 1) / LB_TILE * LB_TILE;
-        dim3 g1((unsigned)((mcp + 255) / 256), (unsigned)De);
-        pack_soa_kernel<<<g1, 256, 0, st>>>(dQraw + m0 * D, mc, D, w.dQs.get(), mcp, h->kp, 1);
-        h->launches++;
+    auto out_at = [&](int64_t m0) { // the outputs from candidate m0 on
         out.mean = dMean ? dMean + m0 : nullptr;
         out.mean_grad = dMeanGrad ? dMeanGrad + m0 * D : nullptr;
         out.dmu = dptr[0] ? dptr[0] + m0 * D : nullptr;
         out.ds2 = dptr[1] ? dptr[1] + m0 * D : nullptr;
         out.acq = dptr[2] ? dptr[2] + m0 : nullptr;
         out.grad = dptr[3] ? dptr[3] + m0 * D : nullptr;
-        if ((rc = lb_launch_query_grad(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, out, &h->launches)))
-            return rc;
+    };
+    if (prior) { // gp.hpp:161-163: mu = mean(v) (added by the caller), sigma^2 = k(v, v) + noise, both constant in v: zero gradients
+        out_at(0);
+        if ((rc = lb_launch_prior_grad(st, M, D, P, h->kp.sf2 + h->kp.noise, out, w.dMu.get(), w.dS2.get()))) return rc;
+        h->launches++;
+    }
+    else { // the chunks of query_fill's panel path
+        const int64_t Mc = panel_chunk(h, M);
+        rc = for_each_chunk(h, dQraw, M, Mc, LB_TILE, lb_query_panel_scratch_doubles(h, Mc), [&](int64_t m0, int64_t mc, int64_t mcp) {
+            out_at(m0);
+            return lb_launch_query_grad(h, st, mc, w.dQs.get(), mcp, w.dV.get(), w.dMu.get() + m0 * P, w.dS2.get() + m0, out, &h->launches);
+        });
+        if (rc) return rc;
     }
     if (mu_out) LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu.get(), sizeof(double) * M * P, d2o, st));
     if (s2_out) LB_CUDA(cudaMemcpyAsync(s2_out, w.dS2.get(), sizeof(double) * M, d2o, st));
@@ -1156,12 +1141,8 @@ static int pair_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq
     int rc;
     if ((rc = ensure_eci_events(o))) return rc;
     if (c && (rc = ensure_eci_events(c))) return rc;
-    const double* dXq = Xq;
-    if (!dev) { // one upload, read by both queries
-        if ((rc = ensure(o, w.dQraw, sizeof(double) * M * o->D))) return rc;
-        LB_CUDA(cudaMemcpyAsync(w.dQraw.get(), Xq, sizeof(double) * M * o->D, cudaMemcpyHostToDevice, st));
-        dXq = w.dQraw.get();
-    }
+    const double* dXq = nullptr; // one upload, read by both queries
+    if ((rc = candidates_on_device(o, Xq, M, dev, &dXq))) return rc;
     if (c) {
         LB_CUDA(cudaEventRecord(o->ex.ev_eci[0], st));
         LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[0], 0));
@@ -1229,7 +1210,7 @@ static int eci_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double jitter,
     lb_gp_full* cu = use_con ? c : nullptr;
     return pair_locked(o, cu, M, Xq, dev, obj_mean_at_q, con_mean_at_q, acq_out, best_val, best_idx, false,
         [&](const double* dMeanObj, const double* dMeanCon, double* dAcq, double* dBV, long long* dBI) {
-            const int Po = o->P > 0 ? o->P : 1, Pc = (use_con && c->P > 0) ? c->P : 1;
+            const int Po = n_outputs(o), Pc = use_con ? n_outputs(c) : 1;
             return lb_launch_eci_full(st, f_max, jitter, M, o->ex.ws.dMu.get(), Po, dMeanObj, obj_mean_const, o->ex.ws.dS2.get(),
                 use_con ? c->ex.ws.dMu.get() : nullptr, Pc, dMeanCon, con_mean_const, use_con ? c->ex.ws.dS2.get() : nullptr, dAcq,
                 o->ex.ws.am.blk_val.get(), o->ex.ws.am.blk_idx.get(), dBV, dBI, &o->launches);
@@ -1306,7 +1287,7 @@ static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point
                 if ((rc = ensure(a, w.dFront, sizeof(double) * 2 * k))) return rc;
                 LB_CUDA(cudaMemcpyAsync(w.dFront.get(), sorted.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
             }
-            const int Pa = a->P > 0 ? a->P : 1, Pb = b->P > 0 ? b->P : 1;
+            const int Pa = n_outputs(a), Pb = n_outputs(b);
             if ((rc = lb_launch_ehvi(st, ref_point[0], ref_point[1], k, w.dFront.get(), M, w.dMu.get(), Pa, dMean0, mean0_const, w.dS2.get(), b->ex.ws.dMu.get(), Pb,
                      dMean1, mean1_const, b->ex.ws.dS2.get(), dAcq, &a->launches)))
                 return rc;
@@ -1552,7 +1533,7 @@ int lb_get(lb_gp* h, int what, double* dst)
     int lower = 0;
     if (what == LB_GET_K) {
         if (!h->kernel_set) return LB_ERR_STATE;
-        if ((rc = make_unique(h, &h->dXs, sizeof(double) * (h->D + LB_MAX_LAMBDA) * Np, false))) return rc;
+        if ((rc = make_unique(h, &h->dXs, shared_bytes(h).Xs, false))) return rc;
         if ((rc = lb_launch_scale_x(h))) return rc;
         if ((rc = lb_launch_kbuild(h, dTmp))) return rc;
         src = dTmp;
@@ -1683,9 +1664,8 @@ int lb_dchol_adopt_begin(lb_gp* h, int64_t Nd)
     if (!h->kernel_set || h->N == 0 || h->Np == 0 || !h->dX) return LB_ERR_STATE;
     if (h->Np != Nd) return LB_ERR_UNSUPPORTED;
     LB_DEVICE(h);
-    int rc;
-    if ((rc = ensure_fit_buffers(h))) return rc;
-    if ((rc = lb_launch_scale_x(h))) return rc;
+    int rc = stage_fit(h);
+    if (rc) return rc;
     LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), h->stream));
     h->fitted = false;
     lb_factor_changed(h);

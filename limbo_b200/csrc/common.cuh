@@ -576,25 +576,78 @@ struct LbProfScope {
     ~LbProfScope() { if (h->prof) lb_prof_end(h, st, cls); }
 };
 
-// internal entry points (one per .cu)
+// internal entry points: what one .cu defines and another calls is declared here and nowhere else, under the file that defines it
+// (the pool, the profiler hooks and lb_set_last_cuda_error: above, ahead of the types that use them)
+// abi.cu
+int lb_ensure_scratch(lb_gp* h, size_t bytes);
+// kbuild.cu
 int lb_launch_scale_x(lb_gp* h);
 int lb_launch_kbuild(lb_gp* h, double* dK);
+// potrf.cu
 int lb_launch_potrf(lb_gp* h);
+int lb_launch_potf2_block(lb_gp* h, int k, int do_factor);
+int lb_debug_potf2_clocks(lb_gp* h, int k, long long* out_host, int n);
+// trsv.cu
 int lb_launch_solve_alpha(lb_gp* h);
 int lb_launch_trsv(lb_gp* h, double* dB, int nrhs, bool forward);
+// query.cu
+int lb_launch_trsm_lower(const lb_gp* h, cudaStream_t st, double* dV, int64_t Mp, int i_begin, long long* launches);
 int lb_launch_query(const lb_gp* h, cudaStream_t st, int64_t M, const double* dXq_soa /*D x Mp*/, int64_t Mp,
     double* dV /*Np x Mp*/, double* dMu /*Mp x P*/, double* dS2 /*Mp*/, long long* launches);
-int lb_launch_acq(const lb_gp* h, cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu0,
-    const double* dS2, double* dAcq, double* dBestVal, long long* dBestIdx, long long* launches);
+int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu, int mu_stride,
+    const double* dMeanAtQ, double mean_const, const double* dS2, double* dAcq, double* dBlkVal, long long* dBlkIdx,
+    double* dBestVal, long long* dBestIdx, long long* launches);
+int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
+    double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
+    const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches);
+int lb_launch_values_argmax(cudaStream_t st, int64_t M, const double* dVals, double* dBlkVal, long long* dBlkIdx, double* dBestVal,
+    long long* dBestIdx, long long* launches);
+size_t lb_query_panel_scratch_doubles(const lb_gp* h, int64_t Mp);
+double* lb_query_panel_tbuf(const lb_gp* h, double* dWork, int64_t Mp);
+double* lb_query_panel_norms(const lb_gp* h, double* dWork, int64_t Mp);
+int lb_query_panel_groups(lb_gp* h, cudaStream_t st, int ctiles, cudaStream_t sts[4], int gbeg[5]);
+int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
+    long long* launches);
+int64_t lb_linv_columns_width(const lb_gp* h, int G);
+size_t lb_linv_columns_scratch_doubles(const lb_gp* h, int G);
+int lb_launch_linv_columns(lb_gp* h, cudaStream_t st, int rank, int G, double* dWork, long long* launches);
+int lb_query_fused_supported(const lb_gp* h);
+size_t lb_query_fused_scratch_doubles(const lb_gp* h, int grid);
+int lb_launch_query_point(const lb_gp* h, cudaStream_t st, const double* x_host, double* dQs, double* dVscratch, double* dOutMapped,
+    long long* launches);
+int lb_launch_query_fused(const lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dVscratch,
+    int grid, double* dMu, double* dS2, long long* launches);
+// query_grad.cu
+int lb_launch_query_grad(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
+    const LbGradOut& out, long long* launches);
+int lb_launch_prior_grad(cudaStream_t st, int64_t M, int D, int P, double s2, const LbGradOut& out, double* dMu, double* dS2);
+// lml.cu
 int lb_launch_loglik(lb_gp* h, double* dOut /*3 doubles: a, logdet, loglik*/);
+int lb_launch_linv_levels(lb_gp* h, int want_tiles); // inverse of the diagonal blocks of `want_tiles` 128-tiles (power of two)
+int lb_launch_linv(lb_gp* h);
 int lb_launch_kinv(lb_gp* h);
-int lb_launch_linv_levels(lb_gp* h, int want_tiles); // lml.cu: inverse of the diagonal blocks of `want_tiles` 128-tiles (power of two)
+int lb_launch_symmetrize(lb_gp* h, double* dA);
 int lb_launch_grad(lb_gp* h, int optimize_noise, double* dGrad);
-int lb_ensure_scratch(lb_gp* h, size_t bytes);
+// loo.cu
+int lb_launch_loo_value(lb_gp* h, double* dOut);
+int lb_launch_loo_grad(lb_gp* h, int optimize_noise, double* dGrad);
+int lb_launch_grad_lambda(lb_gp* h, double* dGrad);
+int lb_launch_kinv_obs(lb_gp* h, double* dOut);
+// tf32_query.cu
 int lb_tf32_prepare(lb_gp* h);
-int lb_launch_tf32_gemm_norm(cudaStream_t st, const void* dA, int64_t lda, const void* dB, int64_t ldb, int64_t M, int64_t N, int64_t K,
-    int tri, float* dNorm2, float* dDout, int* dErr, int grid, int f16);
+size_t lb_dinv_chunk_bytes_impl(const lb_gp* h, int G);
+int lb_dinv_absmax(lb_gp* h, const double* dV, int G, double* out);
+int lb_dinv_pack_impl(lb_gp* h, const double* dV, int rank, int G, double absmax_all, void* dChunk);
+int lb_dinv_adopt_impl(lb_gp* h, int G, const void* dAll, double absmax_all);
 int lb_launch_kstar_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, const double* dQs, int64_t Mcp, float* dKt, double* dMuPart,
     double* dMu, double* dBias, long long* launches);
 int lb_launch_sigma_tf32(const lb_gp* h, cudaStream_t st, int64_t Mc, int64_t Mcp, const float* dKt, float* dNorm2, int* dErr,
     const double* dBias, double* dS2, long long* launches);
+// ehvi.cu
+int lb_launch_ehvi(cudaStream_t st, double r0, double r1, int64_t k, const double* dFront, int64_t M, const double* dMu0, int p0,
+    const double* dMean0, double mean0_const, const double* dS2_0, const double* dMu1, int p1, const double* dMean1, double mean1_const,
+    const double* dS2_1, double* dAcq, long long* launches);
+int lb_launch_pareto(cudaStream_t st, int64_t n, int K, const double* dObjs, int* dKeep, int* dErr, long long* launches);
+// sparsify.cu
+int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const double* dX, int64_t max_points, long long* dKept,
+    int64_t* n_kept, long long* dRemoved, double* dRemovedScore, long long* launches);

@@ -10,9 +10,6 @@
 //                                   (W = alpha alpha^T - K^-1 is never materialised)
 #include "gemm.cuh"
 
-int lb_launch_trsm_lower(const lb_gp* h, cudaStream_t st, double* dV, int64_t Mp, int i_begin, long long* launches);
-int lb_launch_grad_lambda(lb_gp* h, double* dGrad); // loo.cu
-
 namespace {
 
 constexpr int DCH = 16;

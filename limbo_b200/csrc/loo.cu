@@ -13,9 +13,6 @@
 //                                       gradient stays on the host, mean/mean.hpp:72-76)
 #include "gemm.cuh"
 
-int lb_launch_kinv(lb_gp* h);
-int lb_launch_symmetrize(lb_gp* h, double* dA);
-
 namespace {
 
 using Cfg = lbg::CfgWide;

@@ -11,13 +11,6 @@
 #include "gemm.cuh"
 #include <cfloat>
 
-size_t lb_query_panel_scratch_doubles(const lb_gp* h, int64_t Mp);
-double* lb_query_panel_tbuf(const lb_gp* h, double* dWork, int64_t Mp);
-double* lb_query_panel_norms(const lb_gp* h, double* dWork, int64_t Mp);
-int lb_query_panel_groups(lb_gp* h, cudaStream_t st, int ctiles, cudaStream_t sts[4], int gbeg[5]);
-int lb_launch_query_panel(lb_gp* h, cudaStream_t st, int64_t M, const double* dQs, int64_t Mp, double* dWork, double* dMu, double* dS2,
-    long long* launches);
-
 namespace {
 
 namespace panel_bwd {

@@ -26,12 +26,6 @@
 #include <mutex>
 #include <new>
 
-int lb_launch_linv(lb_gp* h);                  // lml.cu
-int lb_launch_symmetrize(lb_gp* h, double* dA); // lml.cu
-int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu, int mu_stride,
-    const double* dMeanAtQ, double mean_const, const double* dS2, double* dAcq, double* dBlkVal, long long* dBlkIdx,
-    double* dBestVal, long long* dBestIdx, long long* launches); // query.cu
-
 namespace {
 
 using GC = lbg::CfgDual;

@@ -748,9 +748,6 @@ sigma2_t32_kernel(const float* __restrict__ norm2, int64_t M, double kvv, double
 
 } // namespace tf32q
 
-int lb_launch_linv(lb_gp* h);
-
-
 // Prepare the row-major reduced-precision copy of L^-1 (rows padded with zeros to a multiple of the 256-row n-tile).
 // fp32 (tf32 MMA) stores L^-1 as is; fp16 stores L^-1 * 2^e with e chosen so that max |.| <= 2^14.
 int lb_tf32_prepare(lb_gp* h)
@@ -795,8 +792,6 @@ int lb_tf32_prepare(lb_gp* h)
 }
 
 // ---- the same copy assembled from the column chunks of G ranks (lb_dinv_* in abi.cu; limbo_b200/dist_inv.py) --------------------
-int64_t lb_linv_columns_width(const lb_gp* h, int G);
-
 static size_t dinv_plane_bytes(const lb_gp* h, int G)
 {
     const bool f16 = (h->precision == 2) || (h->precision == 3);
