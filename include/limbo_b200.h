@@ -273,6 +273,29 @@ int lb_kernel_grad_log_lik(lb_gp* h, int optimize_noise, double* grad);
 /* GP::compute_inv_kernel (gp.hpp:254-264) */
 int lb_compute_inv_kernel(lb_gp* h);
 
+/* Largest N lb_lml_grad_batch takes (LB_ERR_UNSUPPORTED above): the largest N at which one batched call of 10 vectors beat ten
+ * evaluations through lb_set_kernel / lb_fit / lb_log_lik / lb_kernel_grad_log_lik on an H100 (tools/bench_lml_batch.py,
+ * DESIGN.md §4.12). */
+#define LB_LML_BATCH_MAX_N 200
+/* GP::compute_log_lik and GP::compute_kernel_grad_log_lik (gp.hpp:267-311) of this handle's data and obs_mean, evaluated at R
+ * kernel states, as KernelLFOptimization (kernel_lf_opt.hpp:77-92) evaluates one:
+ *   log_hparams: R x n_hparams row-major, the kernel's own log-space parameters as lb_set_kernel takes them
+ *                (SE-ARD Lambda columns inferred from n_hparams as there);
+ *   noise:       R values of the signal noise;
+ *   lik:         R values;
+ *   grad:        R x (n_hparams + optimize_noise) row-major, laid out as lb_kernel_grad_log_lik's; may be NULL (no K^-1, no gradient);
+ *   info:        R values, 0 or the 1-based first non-positive pivot of that vector's factor (lik and grad NaN there); may be NULL.
+ * One launch; one CTA per vector.  A vector's results do not depend on R or on its place in the batch.  The handle's model state
+ * (factor, alpha, caches, kernel) is not touched.  Runs on the handle's stream and pool, under its query lock, in every precision
+ * mode (the likelihood is fp64 in all of them).  LB_ERR_STATE without data; LB_ERR_ARG for R <= 0, an unknown kernel id, a wrong
+ * n_hparams or a non-finite input; LB_ERR_UNSUPPORTED for N > LB_LML_BATCH_MAX_N or outside the kernels' existing bounds
+ * (D + k <= 64, Lambda k <= 4). */
+int lb_lml_grad_batch(lb_gp* h, int kernel_id, int64_t R, int n_hparams, const double* log_hparams, const double* noise,
+    int optimize_noise, double* lik, double* grad, int* info);
+/* same, device pointers (the inputs are read back to the host, where the per-vector kernel state is derived and checked) */
+int lb_lml_grad_batch_dev(lb_gp* h, int kernel_id, int64_t R, int n_hparams, const double* dLog_hparams, const double* dNoise,
+    int optimize_noise, double* dLik, double* dGrad, int* dInfo);
+
 /* GP::compute_log_loo_cv (gp.hpp:339-351): leave-one-out log predictive probability from diag(K^-1) and alpha */
 int lb_log_loo_cv(lb_gp* h, double* out);
 /* GP::compute_kernel_grad_log_loo_cv (gp.hpp:353-399), the gradient KernelLooOpt (model/gp/kernel_loo_opt.hpp:57-97)

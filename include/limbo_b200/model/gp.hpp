@@ -402,6 +402,37 @@ namespace limbo_b200 {
                 for (int i = 0; i < nh; ++i) grad(i) = g[(size_t)i];
                 return grad;
             }
+            // compute_log_lik and compute_kernel_grad_log_lik at R kernel states in one lb_lml_grad_batch call: what a copy of this GP
+            // returns after kernel_function().set_h_params(H.row(r)) and recompute(false), for every row of H (R x h_params_size(),
+            // the noise entry last when optimised: noise = exp(2 p), kernel.hpp:116-123).  The model is not changed.  grad (R x
+            // h_params_size()) and info may be null; info[r] > 0 is the first non-positive pivot of row r, where lik and grad are NaN.
+            // N above LB_LML_BATCH_MAX_N throws (LB_ERR_UNSUPPORTED).
+            void lml_grad_batch(const Eigen::MatrixXd& H, Eigen::VectorXd& lik, Eigen::MatrixXd* grad = nullptr,
+                std::vector<int>* info = nullptr) const
+            {
+                const long R = (long)H.rows();
+                const int nh = (int)H.cols();
+                const int on = Params::kernel::optimize_noise() ? 1 : 0;
+                assert(nh == (int)_kernel_function.h_params_size());
+                const int own = nh - on;
+                std::vector<double> hp((size_t)(R * own)), noise((size_t)R), g(grad ? (size_t)(R * nh) : 0), l((size_t)R);
+                std::vector<int> inf((size_t)R);
+                for (long r = 0; r < R; ++r) {
+                    for (int i = 0; i < own; ++i) hp[(size_t)(r * own + i)] = H(r, i);
+                    noise[(size_t)r] = on ? std::exp(2.0 * H(r, nh - 1)) : _kernel_function.noise();
+                }
+                lb_check(lb_lml_grad_batch(_h, kernel_traits<KernelFunction>::id, R, own, hp.data(), noise.data(), on, l.data(),
+                             grad ? g.data() : nullptr, inf.data()),
+                    "lb_lml_grad_batch");
+                lik.resize(R);
+                for (long r = 0; r < R; ++r) lik(r) = l[(size_t)r];
+                if (grad) {
+                    grad->resize(R, nh);
+                    for (long r = 0; r < R; ++r)
+                        for (int i = 0; i < nh; ++i) (*grad)(r, i) = g[(size_t)(r * nh + i)];
+                }
+                if (info) *info = inf;
+            }
             Eigen::VectorXd compute_mean_grad_log_lik() // gp.hpp:313-330; obs_mean^T K^-1 on the device, functor gradient on the host
             {
                 const long n = (long)_samples.size();

@@ -16,13 +16,14 @@ KERNEL_SQUARED_EXP_ARD, KERNEL_MATERN_FIVE_HALVES, KERNEL_MATERN_THREE_HALVES, K
 ACQ_UCB, ACQ_EI = 0, 1
 GET_K, GET_L, GET_ALPHA, GET_KINV = 0, 1, 2, 3
 EHVI_MAX_K, PARETO_MAX_K = 4096, 8  # LB_EHVI_MAX_K, LB_PARETO_MAX_K
+LML_BATCH_MAX_N = 200  # LB_LML_BATCH_MAX_N
 
 # every symbol include/limbo_b200.h declares
 DECLARED_SYMBOLS = [
     "lb_create", "lb_destroy", "lb_clone", "lb_set_stream", "lb_sync", "lb_launch_count", "lb_set_data",
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
     "lb_acq_argmax", "lb_acq_argmax_dev", "lb_query_grad", "lb_query_grad_dev", "lb_acq_grad", "lb_acq_grad_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_eci_grad", "lb_eci_grad_dev", "lb_ehvi_argmax", "lb_ehvi_argmax_dev",
-    "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_compute_inv_kernel", "lb_log_loo_cv",
+    "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_lml_grad_batch", "lb_lml_grad_batch_dev", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
     "lb_nb_samples", "lb_strerror", "lb_last_cuda_error", "lb_spgp_create", "lb_spgp_destroy", "lb_spgp_set_data", "lb_spgp_lik",
     "lb_spgp_compute", "lb_spgp_query", "lb_spgp_acq_argmax", "lb_spgp_launch_count",
@@ -100,6 +101,8 @@ def load() -> C.CDLL:
         "lb_pareto_set_dev": ([p, i64, i32, dp, dp, dp], i32),
         "lb_log_lik": ([p, dp], i32),
         "lb_kernel_grad_log_lik": ([p, i32, dp], i32),
+        "lb_lml_grad_batch": ([p, i32, i64, i32, dp, dp, i32, dp, dp, dp], i32),
+        "lb_lml_grad_batch_dev": ([p, i32, i64, i32, dp, dp, i32, dp, dp, dp], i32),
         "lb_compute_inv_kernel": ([p], i32),
         "lb_log_loo_cv": ([p, dp], i32),
         "lb_kernel_grad_log_loo_cv": ([p, i32, dp], i32),

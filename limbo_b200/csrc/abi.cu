@@ -1733,6 +1733,106 @@ int lb_kernel_grad_log_lik(lb_gp* hh, int optimize_noise, double* grad)
     return LB_OK;
 }
 
+// GP::compute_log_lik and compute_kernel_grad_log_lik at R kernel states of this handle's data (lml_batch.cu), under the query
+// lock.  The per-vector kernel state is derived on the host exactly as lb_set_kernel derives it (same std::exp, same reciprocals),
+// so a vector sees the K the single path builds.
+static int lml_grad_batch_common(lb_gp* hh, int kernel_id, int64_t R, int n_hparams, const double* log_hparams, const double* noise,
+    int optimize_noise, double* lik, double* grad, int* info, bool dev)
+{
+    if (!hh) return LB_ERR_ARG;
+    if (hh->D <= 0 || hh->N == 0 || !hh->dX) return LB_ERR_STATE;
+    if (R <= 0 || R > INT32_MAX || !log_hparams || !noise || !lik) return LB_ERR_ARG;
+    if (kernel_id < 0 || kernel_id > 3) return LB_ERR_ARG;
+    const int Draw = hh->D;
+    int klam = 0;
+    if (kernel_id == LB_K_SE_ARD) {
+        const int rest = n_hparams - 1 - Draw;
+        if (rest < 0 || rest % Draw != 0) return LB_ERR_ARG;
+        klam = rest / Draw;
+        if (klam > LB_MAX_LAMBDA || Draw + klam > LB_MAX_D) return LB_ERR_UNSUPPORTED;
+    }
+    else if (n_hparams != 2)
+        return LB_ERR_ARG;
+    if (hh->N > LB_LML_BATCH_MAX_N) return LB_ERR_UNSUPPORTED;
+    lb_gp_full* h = full(hh);
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex);
+    cudaStream_t st = h->stream;
+    std::vector<double> hp_dev, no_dev;
+    const double* hp = log_hparams;
+    const double* no = noise;
+    if (dev) { // the kernel state is derived on the host: fetch the vectors
+        hp_dev.resize((size_t)(R * n_hparams));
+        no_dev.resize((size_t)R);
+        LB_CUDA(cudaMemcpyAsync(hp_dev.data(), log_hparams, sizeof(double) * hp_dev.size(), cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(no_dev.data(), noise, sizeof(double) * R, cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaStreamSynchronize(st));
+        hp = hp_dev.data();
+        no = no_dev.data();
+    }
+    for (int64_t i = 0; i < R * n_hparams; ++i)
+        if (!std::isfinite(hp[i])) return LB_ERR_ARG;
+    for (int64_t r = 0; r < R; ++r)
+        if (!std::isfinite(no[r])) return LB_ERR_ARG;
+    // per vector: sf2, l, c1, c2, noise, 0, 0, 0, 1/ell (Draw), Lambda (Draw x klam) - lb_set_kernel's arithmetic
+    const int stride = kernel_id == LB_K_SE_ARD ? 8 + Draw * (1 + klam) : 8;
+    std::vector<double> prm((size_t)(R * stride), 0.0);
+    for (int64_t r = 0; r < R; ++r) {
+        const double* p = hp + r * n_hparams;
+        double* o = prm.data() + r * stride;
+        if (kernel_id == LB_K_SE_ARD) {
+            o[0] = std::exp(2.0 * p[n_hparams - 1]);
+            o[1] = 1.0;
+            for (int d = 0; d < Draw; ++d) o[8 + d] = 1.0 / std::exp(p[d]);
+            std::memcpy(o + 8 + Draw, p + Draw, sizeof(double) * Draw * klam);
+        }
+        else {
+            const double l = std::exp(p[0]);
+            o[0] = std::exp(2.0 * p[1]);
+            o[1] = l;
+            if (kernel_id == LB_K_MATERN52) { o[2] = std::sqrt(5.0) / l; o[3] = 5.0 / (3.0 * (l * l)); }
+            else if (kernel_id == LB_K_MATERN32) o[2] = std::sqrt(3.0) / l;
+            else o[2] = 1.0 / (l * l);
+        }
+        o[4] = no[r];
+    }
+    const int nh = n_hparams + (optimize_noise ? 1 : 0);
+    int rc;
+    {
+        StreamTemps tmp(h->device, st);
+        double *dPrm = nullptr, *dLik = lik, *dGrad = grad;
+        int* dInfo = info;
+        if ((rc = tmp.alloc(sizeof(double) * prm.size(), &dPrm))) return rc;
+        if (!dev) {
+            if ((rc = tmp.alloc(sizeof(double) * R, &dLik)) || (grad && (rc = tmp.alloc(sizeof(double) * R * nh, &dGrad)))
+                || (info && (rc = tmp.alloc(sizeof(int) * R, &dInfo))))
+                return rc;
+        }
+        LB_CUDA(cudaMemcpyAsync(dPrm, prm.data(), sizeof(double) * prm.size(), cudaMemcpyHostToDevice, st));
+        if ((rc = lb_launch_lml_batch(st, tmp, kernel_id, h->dX, h->Np, h->dY, (int)h->N, Draw, klam, h->P, dPrm, stride, (int)R, nh,
+                 optimize_noise ? 1 : 0, dLik, dGrad, dInfo, &h->launches)))
+            return rc;
+        if (!dev) {
+            LB_CUDA(cudaMemcpyAsync(lik, dLik, sizeof(double) * R, cudaMemcpyDeviceToHost, st));
+            if (grad) LB_CUDA(cudaMemcpyAsync(grad, dGrad, sizeof(double) * R * nh, cudaMemcpyDeviceToHost, st));
+            if (info) LB_CUDA(cudaMemcpyAsync(info, dInfo, sizeof(int) * R, cudaMemcpyDeviceToHost, st));
+        }
+        LB_CUDA(cudaStreamSynchronize(st));
+    }
+    return LB_OK;
+}
+
+int lb_lml_grad_batch(lb_gp* h, int kernel_id, int64_t R, int n_hparams, const double* log_hparams, const double* noise,
+    int optimize_noise, double* lik, double* grad, int* info)
+{
+    return lml_grad_batch_common(h, kernel_id, R, n_hparams, log_hparams, noise, optimize_noise, lik, grad, info, false);
+}
+int lb_lml_grad_batch_dev(lb_gp* h, int kernel_id, int64_t R, int n_hparams, const double* dLog_hparams, const double* dNoise,
+    int optimize_noise, double* dLik, double* dGrad, int* dInfo)
+{
+    return lml_grad_batch_common(h, kernel_id, R, n_hparams, dLog_hparams, dNoise, optimize_noise, dLik, dGrad, dInfo, true);
+}
+
 int lb_log_loo_cv(lb_gp* hh, double* out)
 {
     if (!hh || !out) return LB_ERR_ARG;

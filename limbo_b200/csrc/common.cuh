@@ -187,6 +187,41 @@ __device__ __forceinline__ double lb_unit_kernel_from_z(double z, const KernPara
     return lb_exp_nonpos(-0.5 * (z * kp.c1));
 }
 
+// The pair derivatives the likelihood gradient weights (lml.cu grad_kernel, lml_batch.cu), from the (scaled) squared distance:
+//   SE-ARD   g0 = k (the ell / Lambda entries multiply it by their pair factor), g1 = dk / dlog sigma_f = 2k  squared_exp_ard.hpp:127-135
+//   others   g0 = dk / dlog l, g1 = dk / dlog sigma_f      matern_five_halves.hpp:115-133, matern_three_halves.hpp:110-124, exp.hpp:101-110
+// with the branch-free lb_exp_nonpos (<= 3e-16 relative, inside the 1e-9 bar of the gradient).
+template <int KID>
+__device__ __forceinline__ void lb_kernel_grad_pair(double zz, const KernParams& kp, double& g0, double& g1)
+{
+    if (KID == LB_K_SE_ARD) {
+        const double k = kp.sf2 * lb_exp_nonpos(-0.5 * zz);
+        g0 = k;
+        g1 = 2.0 * k;
+    }
+    else if (KID == LB_K_MATERN52) {
+        const double d = sqrt(zz), d_sq = d * d, l_sq = kp.l * kp.l;
+        const double term1 = sqrt(5.0) * d / kp.l;
+        const double term2 = 5. * d_sq / (3. * l_sq);
+        const double r = lb_exp_nonpos(-term1);
+        g0 = kp.sf2 * (r * term1 * (1 + term1 + term2) + (-term1 - 2. * term2) * r);
+        g1 = 2 * kp.sf2 * (1 + term1 + term2) * r;
+    }
+    else if (KID == LB_K_MATERN32) {
+        const double d = sqrt(zz);
+        const double term = sqrt(3.0) * d / kp.l;
+        const double r = lb_exp_nonpos(-term);
+        g0 = kp.sf2 * (-term * r + (1 + term) * term * r);
+        g1 = 2 * kp.sf2 * (1 + term) * r;
+    }
+    else {
+        const double r = zz / (kp.l * kp.l);
+        const double k = kp.sf2 * lb_exp_nonpos(-0.5 * r);
+        g0 = r * k;
+        g1 = 2 * k;
+    }
+}
+
 // expected improvement of mu over f_max + jitter, 0 when sigma < 1e-10: ei.hpp:92-115, and the factor eci.hpp:86-106 weights
 __device__ __forceinline__ double lb_ei_factor(double mu, double s2, double f_max, double jitter)
 {
@@ -642,6 +677,10 @@ int lb_launch_linv(lb_gp* h);
 int lb_launch_kinv(lb_gp* h);
 int lb_launch_symmetrize(lb_gp* h, double* dA);
 int lb_launch_grad(lb_gp* h, int optimize_noise, double* dGrad);
+// lml_batch.cu: one launch; dPrm is R x stride (lb_lml_grad_batch's per-vector kernel state), dGrad NULL = likelihood only
+int lb_launch_lml_batch(cudaStream_t st, StreamTemps& tmp, int kernel_id, const double* dX, int64_t ldx, const double* dY, int N,
+    int Draw, int klam, int P, const double* dPrm, int stride, int R, int nh, int optimize_noise, double* dLik, double* dGrad,
+    int* dInfo, long long* launches);
 // loo.cu
 int lb_launch_loo_value(lb_gp* h, double* dOut);
 int lb_launch_loo_grad(lb_gp* h, int optimize_noise, double* dGrad);

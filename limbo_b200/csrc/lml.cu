@@ -258,36 +258,14 @@ __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const d
                     w *= f;
                     if (ii == jj) g_noise = fma(w, 2.0 * kp.noise, g_noise); // kernel.hpp:90-93
                 }
-                const double zz = z[c][e];
-                if (ard) { // squared_exp_ard.hpp:127-135
-                    const double k = kp.sf2 * lb_exp_nonpos(-0.5 * zz);
-                    wk[c][e] = w * k;
-                    g_sf = fma(w, 2.0 * k, g_sf);
+                double g0, g1; // common.cuh lb_kernel_grad_pair
+                lb_kernel_grad_pair<KID>(z[c][e], kp, g0, g1);
+                if (ard) {
+                    wk[c][e] = w * g0;
+                    g_sf = fma(w, g1, g_sf);
                 }
                 else {
                     wk[c][e] = 0.0;
-                    double g0, g1;
-                    if (KID == LB_K_MATERN52) { // matern_five_halves.hpp:115-133
-                        const double d = sqrt(zz), d_sq = d * d, l_sq = kp.l * kp.l;
-                        const double term1 = sqrt(5.0) * d / kp.l;
-                        const double term2 = 5. * d_sq / (3. * l_sq);
-                        const double r = lb_exp_nonpos(-term1);
-                        g0 = kp.sf2 * (r * term1 * (1 + term1 + term2) + (-term1 - 2. * term2) * r);
-                        g1 = 2 * kp.sf2 * (1 + term1 + term2) * r;
-                    }
-                    else if (KID == LB_K_MATERN32) { // matern_three_halves.hpp:110-124
-                        const double d = sqrt(zz);
-                        const double term = sqrt(3.0) * d / kp.l;
-                        const double r = lb_exp_nonpos(-term);
-                        g0 = kp.sf2 * (-term * r + (1 + term) * term * r);
-                        g1 = 2 * kp.sf2 * (1 + term) * r;
-                    }
-                    else { // exp.hpp:101-110
-                        const double r = zz / (kp.l * kp.l);
-                        const double k = kp.sf2 * lb_exp_nonpos(-0.5 * r);
-                        g0 = r * k;
-                        g1 = 2 * k;
-                    }
                     g_l = fma(w, g0, g_l);
                     g_sf = fma(w, g1, g_sf);
                 }

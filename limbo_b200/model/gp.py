@@ -8,6 +8,7 @@ one-point-at-a-time reference lacks are suffixed ``_batch``.
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 
@@ -413,6 +414,29 @@ class GP:
         _lib.check(self._lib.lb_kernel_grad_log_lik(self._h, int(k.optimize_noise()), _ptr(g)), "lb_kernel_grad_log_lik")
         self._inv_kernel_updated = True
         return g
+
+    # ---- gp.hpp:267-311 at R kernel states in one call (lb_lml_grad_batch); the model is not changed ----
+    def lml_grad_batch(self, H, compute_grad: bool = True):
+        """compute_log_lik and compute_kernel_grad_log_lik as a copy of this GP would return them after
+        kernel_function().set_h_params(H[r]) and recompute(False), for every row r of H (R x h_params_size(), the noise
+        entry last when optimize_noise: noise = exp(2 p), kernel.hpp).  Returns (lik (R,), grad (R x h_params_size()) or None,
+        info (R,)): info[r] > 0 is the 1-based first non-positive pivot of that row's factor, where lik and grad are NaN."""
+        k = self._kernel_function
+        H = np.ascontiguousarray(np.atleast_2d(np.asarray(H, dtype=np.float64)))
+        R, nh = H.shape
+        assert nh == k.h_params_size()
+        nk = k.params_size()
+        own = np.ascontiguousarray(H[:, :nk])
+        if k.optimize_noise():  # kernel.hpp:116-123, the same exp the kernel functor takes
+            noise = np.array([math.exp(2.0 * float(p)) for p in H[:, nk]], dtype=np.float64)
+        else:
+            noise = np.full(R, k.noise(), dtype=np.float64)
+        lik = np.empty(R)
+        grad = np.empty((R, nh)) if compute_grad else None
+        info = np.empty(R, dtype=np.int32)
+        _lib.check(self._lib.lb_lml_grad_batch(self._h, k.kernel_id, R, nk, _ptr(own), _ptr(noise), int(k.optimize_noise()), _ptr(lik),
+                                               _ptr(grad) if grad is not None else None, _ptr(info)), "lb_lml_grad_batch")
+        return lik, grad, info
 
     # ---- gp.hpp:313-330: obs_mean^T K^-1 on the device (lb_kinv_obs_mean); the mean functor's gradient is host code ----
     def compute_mean_grad_log_lik(self) -> np.ndarray:

@@ -5,6 +5,7 @@ import sys
 
 import numpy as np
 
+from .. import _lib
 from .. import opt as _opt
 
 
@@ -34,6 +35,14 @@ class KernelLFOpt(HPOpt):
         gp.compute_log_lik()
 
 
+def batch_pays(n: int, rows: int) -> bool:
+    """Whether one lb_lml_grad_batch call of `rows` vectors at n samples beats `rows` evaluations of the single path: n within
+    LB_LML_BATCH_MAX_N, and rows at least (n / 90)^2, the crossover measured on an H100 (DESIGN.md §4.12: one call costs about as
+    much as 1 single evaluation at n = 50, 1.5 at n = 100 and 5 at n = 200), so a lone lane left running after eps_stop stopped
+    the others goes back to the single path."""
+    return n <= _lib.LML_BATCH_MAX_N and rows * 8100 >= n * n
+
+
 class _KernelLFOptimization:
     def __init__(self, gp):
         self._original_gp = gp
@@ -50,6 +59,16 @@ class _KernelLFOptimization:
         if not compute_grad:
             return _opt.no_grad(lik)
         return lik, gp.compute_kernel_grad_log_lik()
+
+    def batch(self, X, compute_grad: bool):
+        """The R rows of X at once (opt.BatchedRprop, opt.BatchedParallelRepeater): one lb_lml_grad_batch call where it pays
+        (batch_pays), otherwise row by row through __call__."""
+        X = np.ascontiguousarray(np.atleast_2d(np.asarray(X, dtype=np.float64)))
+        if batch_pays(self._original_gp.nb_samples(), X.shape[0]):
+            lik, grad, _ = self._original_gp.lml_grad_batch(X, compute_grad)
+            return lik, grad
+        rows = [self(x, compute_grad) for x in X]
+        return np.array([r[0] for r in rows]), (np.stack([r[1] for r in rows]) if compute_grad else None)
 
 
 class KernelLooOpt(HPOpt):
