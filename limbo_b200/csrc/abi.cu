@@ -80,7 +80,7 @@ struct Extra {
     double* hPoint = nullptr;  // pinned, mapped host buffer for the one-point query (mu[P], sigma^2)
     double* dPoint = nullptr;  // its device alias
     int point_cap = 0;
-    cudaEvent_t ev_eci[2] = {}; // lb_eci_argmax's fork / join events, created on first use (the events of h->ev belong to the fit)
+    cudaEvent_t ev_pair[2] = {}; // pair_locked's fork / join events, created on first use (the events of h->ev belong to the fit)
 };
 
 } // namespace
@@ -311,6 +311,107 @@ int for_each_chunk(lb_gp_full* h, const double* dQraw, int64_t M, int64_t Mc, in
     return LB_OK;
 }
 
+// The host ends of one call on one stream.  Host mode: in() gives a device copy of a host array, out() a device temporary whose
+// contents finish() copies back to the caller's array before it synchronises the stream once.  Device mode: the caller's pointers
+// pass through, and finish() neither copies nor waits.  NULL stays NULL.
+class Staging {
+public:
+    StreamTemps tmp;
+    Staging(int device, cudaStream_t st, bool dev) : tmp(device, st), st_(st), dev_(dev) {}
+    template <typename T>
+    int in(const T* src, size_t n, const T** out)
+    {
+        *out = src;
+        if (!src || dev_) return LB_OK;
+        T* p = nullptr;
+        int rc = tmp.alloc(sizeof(T) * n, &p);
+        if (rc) return rc;
+        LB_CUDA(cudaMemcpyAsync(p, src, sizeof(T) * n, cudaMemcpyHostToDevice, st_));
+        *out = p;
+        return LB_OK;
+    }
+    template <typename T>
+    int out(T* dst, size_t n, T** out)
+    {
+        *out = dst;
+        if (!dst || dev_) return LB_OK;
+        int rc = tmp.alloc(sizeof(T) * n, out);
+        if (rc) return rc;
+        back_.push_back({dst, *out, sizeof(T) * n});
+        return LB_OK;
+    }
+    int finish()
+    {
+        if (dev_) return LB_OK;
+        for (const Back& b : back_) LB_CUDA(cudaMemcpyAsync(b.dst, b.src, b.bytes, cudaMemcpyDeviceToHost, st_));
+        LB_CUDA(cudaStreamSynchronize(st_));
+        return LB_OK;
+    }
+
+private:
+    struct Back { void* dst; const void* src; size_t bytes; };
+    cudaStream_t st_;
+    bool dev_;
+    std::vector<Back> back_;
+};
+
+// false for a non-finite coordinate of the M x D host candidates; device candidates are not read
+bool coordinates_finite(const double* Xq, int64_t M, int D, bool dev)
+{
+    if (!dev)
+        for (int64_t i = 0; i < M * D; ++i)
+            if (!std::isfinite(Xq[i])) return false;
+    return true;
+}
+
+// n zeros into dst (NULL: nothing), on st when dst is a device array
+template <typename T>
+int zero_fill(T* dst, int64_t n, bool dev, cudaStream_t st)
+{
+    if (!dst) return LB_OK;
+    if (dev) LB_CUDA(cudaMemsetAsync(dst, 0, sizeof(T) * n, st));
+    else std::fill(dst, dst + n, T(0));
+    return LB_OK;
+}
+
+// The layout of n_hparams log-hyper-parameters of kernel kernel_id (0 to 3) over Draw inputs: the number of SE-ARD Lambda columns
+// (0 for the other kernels), or LB_ERR_ARG for a count that fits no layout, LB_ERR_UNSUPPORTED beyond LB_MAX_LAMBDA / LB_MAX_D.
+int hparam_klam(int kernel_id, int Draw, int n_hparams)
+{
+    if (kernel_id != LB_K_SE_ARD) return n_hparams == 2 ? 0 : LB_ERR_ARG;
+    const int rest = n_hparams - 1 - Draw; // [log ell (D), A columns (D each, k of them), log sigma_f]  squared_exp_ard.hpp:91,96-105
+    if (rest < 0 || rest % Draw != 0) return LB_ERR_ARG;
+    const int klam = rest / Draw;
+    if (klam > LB_MAX_LAMBDA || Draw + klam > LB_MAX_D) return LB_ERR_UNSUPPORTED;
+    return klam;
+}
+
+// The kernel state of the log-hyper-parameters p (layout from hparam_klam) and the noise, written over kp.  kp.lambda is left NULL:
+// the Lambda columns, p[Draw ..] column-major, stay with the caller.  Every kernel build reads what this derives, so the single path
+// (lb_set_kernel) and the batched likelihood (lb_lml_grad_batch) see the same K.
+void kernel_state(KernParams& kp, int kernel_id, int Draw, int klam, const double* p, int n_hparams, double noise)
+{
+    kp.id = kernel_id;
+    kp.Draw = Draw;
+    kp.klam = klam;
+    kp.D = Draw + klam;
+    kp.lambda = nullptr;
+    kp.noise = noise;
+    if (kernel_id == LB_K_SE_ARD) {
+        for (int d = 0; d < Draw; ++d) kp.inv_ell[d] = 1.0 / std::exp(p[d]);
+        kp.sf2 = std::exp(2.0 * p[n_hparams - 1]);
+        kp.l = 1.0;
+    }
+    else { // matern_five_halves.hpp:97-102 and siblings
+        kp.l = std::exp(p[0]);
+        kp.sf2 = std::exp(2.0 * p[1]);
+    }
+    kp.c1 = kp.c2 = 0.0;
+    if (kernel_id == LB_K_MATERN52) { kp.c1 = std::sqrt(5.0) / kp.l; kp.c2 = 5.0 / (3.0 * (kp.l * kp.l)); }
+    else if (kernel_id == LB_K_MATERN32) kp.c1 = std::sqrt(3.0) / kp.l;
+    else if (kernel_id == LB_K_EXP) kp.c1 = 1.0 / (kp.l * kp.l);
+}
+
 } // namespace
 
 int lb_ensure_scratch(lb_gp* h, size_t bytes)
@@ -383,7 +484,7 @@ int lb_destroy(lb_gp* hh)
     free_model(h);
     h->ex.ws = QueryWs{}; // the remaining private buffers go back with the handle (delete h)
     if (h->ex.hPoint) cudaFreeHost(h->ex.hPoint);
-    for (cudaEvent_t e : h->ex.ev_eci) if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : h->ex.ev_pair) if (e) cudaEventDestroy(e);
     for (cudaStream_t& s : h->group)
         if (s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); s = nullptr; }
     Shell sh;
@@ -519,50 +620,25 @@ int lb_set_kernel(lb_gp* h, int kernel_id, const double* p, int n_hparams, doubl
     if (!h || !p) return LB_ERR_ARG;
     if (kernel_id < 0 || kernel_id > 3) return LB_ERR_UNSUPPORTED;
     if (h->D <= 0) return LB_ERR_STATE; // need the input dimension first (lb_set_data)
-    int klam = 0;
-    if (kernel_id == LB_K_SE_ARD) { // [log ell (D), A columns (D each, k of them), log sigma_f]  squared_exp_ard.hpp:91,96-105
-        const int rest = n_hparams - 1 - h->D;
-        if (rest < 0 || rest % h->D != 0) return LB_ERR_ARG;
-        klam = rest / h->D;
-        if (klam > LB_MAX_LAMBDA || h->D + klam > LB_MAX_D) return LB_ERR_UNSUPPORTED;
-    }
-    else if (n_hparams != 2)
-        return LB_ERR_ARG;
+    const int klam = hparam_klam(kernel_id, h->D, n_hparams);
+    if (klam < 0) return klam;
     LB_DEVICE(h);
     bool lambda_same = true;
     const KernParams old = h->kp;
     const bool was_set = h->kernel_set;
     const int old_nh = h->n_hparams;
     KernParams& kp = h->kp;
-    kp.id = kernel_id;
-    kp.Draw = h->D;
-    kp.klam = klam;
-    kp.D = h->D + klam;
-    kp.lambda = nullptr;
-    kp.noise = noise;
-    if (kernel_id == LB_K_SE_ARD) {
-        for (int d = 0; d < h->D; ++d) kp.inv_ell[d] = 1.0 / std::exp(p[d]);
-        kp.sf2 = std::exp(2.0 * p[n_hparams - 1]);
-        kp.l = 1.0;
-        if (klam > 0) { // _A(i, j) = p((j + 1) * D + i): already column-major
-            int rc = h->dLambda.reserve(h, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA);
-            if (rc) return rc;
-            double* lh = full(h)->ex.lambda_host;
-            lambda_same = (old.klam == klam) && std::memcmp(lh, p + h->D, sizeof(double) * h->D * klam) == 0;
-            std::memcpy(lh, p + h->D, sizeof(double) * h->D * klam);
-            LB_CUDA(cudaMemcpyAsync(h->dLambda.get(), p + h->D, sizeof(double) * h->D * klam, cudaMemcpyHostToDevice, h->stream));
-            LB_CUDA(cudaStreamSynchronize(h->stream));
-            kp.lambda = h->dLambda.get();
-        }
+    kernel_state(kp, kernel_id, h->D, klam, p, n_hparams, noise);
+    if (klam > 0) { // _A(i, j) = p((j + 1) * D + i): already column-major
+        int rc = h->dLambda.reserve(h, sizeof(double) * LB_MAX_D * LB_MAX_LAMBDA);
+        if (rc) return rc;
+        double* lh = full(h)->ex.lambda_host;
+        lambda_same = (old.klam == klam) && std::memcmp(lh, p + h->D, sizeof(double) * h->D * klam) == 0;
+        std::memcpy(lh, p + h->D, sizeof(double) * h->D * klam);
+        LB_CUDA(cudaMemcpyAsync(h->dLambda.get(), p + h->D, sizeof(double) * h->D * klam, cudaMemcpyHostToDevice, h->stream));
+        LB_CUDA(cudaStreamSynchronize(h->stream));
+        kp.lambda = h->dLambda.get();
     }
-    else { // matern_five_halves.hpp:97-102 and siblings
-        kp.l = std::exp(p[0]);
-        kp.sf2 = std::exp(2.0 * p[1]);
-    }
-    kp.c1 = kp.c2 = 0.0;
-    if (kernel_id == LB_K_MATERN52) { kp.c1 = std::sqrt(5.0) / kp.l; kp.c2 = 5.0 / (3.0 * (kp.l * kp.l)); }
-    else if (kernel_id == LB_K_MATERN32) kp.c1 = std::sqrt(3.0) / kp.l;
-    else if (kernel_id == LB_K_EXP) kp.c1 = 1.0 / (kp.l * kp.l);
     h->n_hparams = n_hparams;
     h->kernel_set = true;
     // The same functor state again (add_sample pushes the kernel before every lb_append, gp.hpp:126-152 never touches
@@ -1054,62 +1130,32 @@ static int grad_common(const lb_gp* hc, int64_t M, const double* Xq, bool dev, d
     if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
     if (h->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
     const int D = h->D, P = n_outputs(h);
-    if (!dev)
-        for (int64_t i = 0; i < M * D; ++i)
-            if (!std::isfinite(Xq[i])) return LB_ERR_ARG;
+    if (!coordinates_finite(Xq, M, D, dev)) return LB_ERR_ARG;
     LB_DEVICE(h);
     std::lock_guard<std::mutex> lock(h->ex.qmutex);
     QueryWs& w = h->ex.ws;
     cudaStream_t st = h->stream;
-    const double p0 = acq_id >= 0 ? acq_params[0] : 0.0, p1 = acq_id == LB_ACQ_EI ? acq_params[1] : 0.0;
-    const cudaMemcpyKind d2o = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     const bool prior = query_path(h, M) == QP_PRIOR;
     if (prior && h->N != 0) return LB_ERR_STATE;
     int rc;
     const double* dQraw = Xq;
     if (!prior && (rc = candidates_on_device(h, Xq, M, dev, &dQraw))) return rc;
-    StreamTemps tmp(h->device, st); // host mode: device copies of the outputs and of the means
+    Staging io(h->device, st, dev); // the means (acquisitions only) and the gradient outputs
     LbGradOut out{};
     out.acq_id = acq_id;
-    out.p0 = p0;
-    out.p1 = p1;
+    out.p0 = acq_id >= 0 ? acq_params[0] : 0.0;
+    out.p1 = acq_id == LB_ACQ_EI ? acq_params[1] : 0.0;
     out.mean_const = mean_const;
-    double* douts[4] = {dmu_out, ds2_out, acq_out, grad_out};
-    const size_t ncols[4] = {(size_t)D, (size_t)D, 1, (size_t)D};
-    double* dptr[4] = {};
-    for (int k = 0; k < 4; ++k) {
-        if (!douts[k] || (acq_id < 0 && k >= 2)) continue;
-        if (dev) dptr[k] = douts[k];
-        else if ((rc = tmp.alloc(sizeof(double) * M * ncols[k], &dptr[k]))) return rc;
-    }
-    const double* dMean = mean_at_q;
-    const double* dMeanGrad = mean_grad;
-    if (acq_id >= 0 && !dev) {
-        double* p;
-        if (mean_at_q) {
-            if ((rc = tmp.alloc(sizeof(double) * M, &p))) return rc;
-            LB_CUDA(cudaMemcpyAsync(p, mean_at_q, sizeof(double) * M, cudaMemcpyHostToDevice, st));
-            dMean = p;
-        }
-        if (mean_grad) {
-            if ((rc = tmp.alloc(sizeof(double) * M * D, &p))) return rc;
-            LB_CUDA(cudaMemcpyAsync(p, mean_grad, sizeof(double) * M * D, cudaMemcpyHostToDevice, st));
-            dMeanGrad = p;
-        }
-    }
-    out.mean = dMean;
-    out.mean_grad = dMeanGrad;
-    out.dmu = dptr[0];
-    out.ds2 = dptr[1];
-    out.acq = dptr[2];
-    out.grad = dptr[3];
+    if ((rc = io.in(mean_at_q, M, &out.mean)) || (rc = io.in(mean_grad, (size_t)M * D, &out.mean_grad))
+        || (rc = io.out(dmu_out, (size_t)M * D, &out.dmu)) || (rc = io.out(ds2_out, (size_t)M * D, &out.ds2))
+        || (rc = io.out(acq_out, M, &out.acq)) || (rc = io.out(grad_out, (size_t)M * D, &out.grad)))
+        return rc;
     if ((rc = grad_fill(h, M, dQraw, out))) return rc;
+    const cudaMemcpyKind d2o = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (mu_out) LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu.get(), sizeof(double) * M * P, d2o, st));
     if (s2_out) LB_CUDA(cudaMemcpyAsync(s2_out, w.dS2.get(), sizeof(double) * M, d2o, st));
-    if (!dev)
-        for (int k = 0; k < 4; ++k)
-            if (dptr[k]) LB_CUDA(cudaMemcpyAsync(douts[k], dptr[k], sizeof(double) * M * ncols[k], cudaMemcpyDeviceToHost, st));
-    LB_CUDA(cudaStreamSynchronize(st));
+    if ((rc = io.finish())) return rc;
+    if (dev) LB_CUDA(cudaStreamSynchronize(st)); // the device outputs are complete on return too
     LB_CUDA(cudaGetLastError());
     return LB_OK;
 }
@@ -1137,67 +1183,116 @@ int lb_acq_grad_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_
         dAcq_out, dGrad_out);
 }
 
-static int ensure_eci_events(lb_gp_full* h)
+static int ensure_pair_events(lb_gp_full* h)
 {
-    for (cudaEvent_t& e : h->ex.ev_eci)
+    for (cudaEvent_t& e : h->ex.ev_pair)
         if (!e) LB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     return LB_OK;
 }
 
-// What an acquisition over two handles shares (ECI, EHVI): both handles' qmutex are held.  The candidates are uploaded once; o's
-// query runs on o's stream and c's (c may be NULL) on c's stream, so they may overlap; o's stream then waits for c, and
-// epilogue(dMean_o, dMean_c, dAcq, dBestVal, dBestIdx) launches the fused scoring on o's stream.  c's stream waits for the
-// epilogue before the locks are released.  dev: every pointer is a device pointer and the call does not synchronise.
-// acq_ws: give the epilogue a value buffer even when the caller asked for none.
+// f() under o's query lock, and under c's too when c is not NULL
 extern "C++" {
-template <typename Epilogue>
-static int pair_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq, bool dev, const double* o_mean_at_q,
-    const double* c_mean_at_q, double* acq_out, double* best_val, int64_t* best_idx, bool acq_ws, Epilogue&& epilogue)
+template <typename F>
+static int with_query_locks(lb_gp_full* o, lb_gp_full* c, F&& f)
+{
+    if (!c) {
+        std::lock_guard<std::mutex> lock(o->ex.qmutex);
+        return f();
+    }
+    std::scoped_lock lock(o->ex.qmutex, c->ex.qmutex); // deadlock-free whatever order other callers pass the pair in
+    return f();
+}
+
+// What a call over two handles shares (ECI, EHVI; values and gradients): both handles' qmutex are held.  The candidates are
+// uploaded once; pass(h, dXq) runs o's pass on o's stream and then, when that succeeded, c's (c may be NULL) on c's stream, so
+// that the two may overlap.  o's stream then waits for c's, and epilogue() enqueues the work over both passes on o's stream.
+// c's stream waits for the epilogue before the locks are released: a later call on c must not overwrite what it reads.
+// dev: Xq is a device pointer.
+template <typename Pass, typename Epilogue>
+static int pair_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq, bool dev, Pass&& pass, Epilogue&& epilogue)
 {
     cudaStream_t st = o->stream;
-    QueryWs& w = o->ex.ws;
     int rc;
-    if ((rc = ensure_eci_events(o))) return rc;
-    if (c && (rc = ensure_eci_events(c))) return rc;
-    const double* dXq = nullptr; // one upload, read by both queries
+    if ((rc = ensure_pair_events(o)) || (c && (rc = ensure_pair_events(c)))) return rc;
+    const double* dXq = nullptr; // one upload, read by both passes
     if ((rc = candidates_on_device(o, Xq, M, dev, &dXq))) return rc;
     if (c) {
-        LB_CUDA(cudaEventRecord(o->ex.ev_eci[0], st));
-        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[0], 0));
+        LB_CUDA(cudaEventRecord(o->ex.ev_pair[0], st));
+        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_pair[0], 0));
     }
-    rc = query_fill(o, M, dXq, true);
-    int rc_con = (rc == LB_OK && c) ? query_fill(c, M, dXq, true) : LB_OK;
-    if (c) { // o's stream waits for c's mu / sigma^2 (and for c's last read of o's candidate buffer)
-        LB_CUDA(cudaEventRecord(c->ex.ev_eci[0], c->stream));
-        LB_CUDA(cudaStreamWaitEvent(st, c->ex.ev_eci[0], 0));
-    }
-    if (rc) return rc;
-    if (rc_con) return rc_con;
-    if (!dev) {
-        if ((rc = query_timed_out(o))) return rc;
-        if (c && (rc = query_timed_out(c))) return rc;
-    }
-    if ((rc = w.am.reserve(o->device, st, M))) return rc;
-    const double* dMeanO = nullptr;
-    const double* dMeanC = nullptr;
-    if ((rc = mean_on_device(o, st, o_mean_at_q, M, dev, &dMeanO))) return rc;
-    if (c && (rc = mean_on_device(c, st, c_mean_at_q, M, dev, &dMeanC))) return rc;
-    double* dAcq = acq_out;
-    if ((acq_out && !dev) || (!acq_out && acq_ws)) {
-        if ((rc = ensure(o, w.am.vals, sizeof(double) * M))) return rc;
-        dAcq = w.am.vals.get();
-    }
-    double* dBV = dev ? best_val : w.am.best_val.get();
-    long long* dBI = dev ? (long long*)best_idx : w.am.best_idx.get();
-    rc = epilogue(dMeanO, dMeanC, dAcq, dBV, dBI);
-    if (c) { // a later call on c must not overwrite the buffers the epilogue reads before it has run
-        LB_CUDA(cudaEventRecord(o->ex.ev_eci[1], st));
-        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[1], 0));
+    rc = pass(o, dXq);
+    const int rc_c = (rc == LB_OK && c) ? pass(c, dXq) : LB_OK;
+    if (c) { // o's stream waits for c's pass (and for c's last read of o's candidate buffer)
+        LB_CUDA(cudaEventRecord(c->ex.ev_pair[0], c->stream));
+        LB_CUDA(cudaStreamWaitEvent(st, c->ex.ev_pair[0], 0));
     }
     if (rc) return rc;
-    if (!dev && (rc = w.am.read_best(st, best_val, best_idx, acq_out, M))) return rc;
+    if (rc_c) return rc_c;
+    rc = epilogue();
+    if (c) {
+        LB_CUDA(cudaEventRecord(o->ex.ev_pair[1], st));
+        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_pair[1], 0));
+    }
+    if (rc) return rc;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
+}
+
+// pair_locked for an argmax: each pass is query_fill, and score(dMean_o, dMean_c, dAcq, dBestVal, dBestIdx) launches the fused
+// scoring on o's stream.  dev: every pointer is a device pointer and the call does not synchronise.  acq_ws: give score a value
+// buffer even when the caller asked for none.  After a timed-out reduced-precision pass, pair_locked still records the release
+// of c's stream: it only orders c's later work after what o's stream already holds, as on every other path.
+template <typename Score>
+static int pair_argmax_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq, bool dev, const double* o_mean_at_q,
+    const double* c_mean_at_q, double* acq_out, double* best_val, int64_t* best_idx, bool acq_ws, Score&& score)
+{
+    cudaStream_t st = o->stream;
+    ArgmaxWs& am = o->ex.ws.am;
+    auto pass = [&](lb_gp_full* h, const double* dXq) { return query_fill(h, M, dXq, true); };
+    return pair_locked(o, c, M, Xq, dev, pass, [&] {
+        int rc;
+        if (!dev && ((rc = query_timed_out(o)) || (c && (rc = query_timed_out(c))))) return rc;
+        if ((rc = am.reserve(o->device, st, M))) return rc;
+        const double* dMeanO = nullptr;
+        const double* dMeanC = nullptr;
+        if ((rc = mean_on_device(o, st, o_mean_at_q, M, dev, &dMeanO))) return rc;
+        if (c && (rc = mean_on_device(c, st, c_mean_at_q, M, dev, &dMeanC))) return rc;
+        double* dAcq = acq_out;
+        if ((acq_out && !dev) || (!acq_out && acq_ws)) {
+            if ((rc = ensure(o, am.vals, sizeof(double) * M))) return rc;
+            dAcq = am.vals.get();
+        }
+        double* dBV = dev ? best_val : am.best_val.get();
+        long long* dBI = dev ? (long long*)best_idx : am.best_idx.get();
+        if ((rc = score(dMeanO, dMeanC, dAcq, dBV, dBI))) return rc;
+        return dev ? LB_OK : am.read_best(st, best_val, best_idx, acq_out, M);
+    });
+}
+
+// pair_locked for a gradient: each pass is the handle's gradient pass (grad_fill, no acquisition) in its own chunk widths, into its
+// own workspace (mu, sigma^2 and dGrad), and epilogue(mo, mc) gets mo / mc with those outputs filled in.
+template <typename Epilogue>
+static int pair_grad_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq, bool dev, LbPairModel mo, LbPairModel mc,
+    Epilogue&& epilogue)
+{
+    for (lb_gp_full* h : {o, c})
+        if (h && query_path(h, M) == QP_PRIOR && h->N != 0) return LB_ERR_STATE;
+    auto pass = [&](lb_gp_full* h, const double* dXq) {
+        LbPairModel& pm = h == o ? mo : mc;
+        const size_t nd = (size_t)M * h->D;
+        int rc = ensure(h, h->ex.ws.dGrad, sizeof(double) * 2 * nd);
+        if (rc) return rc;
+        LbGradOut out{};
+        out.acq_id = -1; // mu, sigma^2 and their gradients only
+        pm.dmu = out.dmu = h->ex.ws.dGrad.get();
+        pm.ds2 = out.ds2 = h->ex.ws.dGrad.get() + nd;
+        if ((rc = grad_fill(h, M, dXq, out))) return rc;
+        pm.mu = h->ex.ws.dMu.get(); // sized by grad_fill
+        pm.p = n_outputs(h);
+        pm.s2 = h->ex.ws.dS2.get();
+        return LB_OK;
+    };
+    return pair_locked(o, c, M, Xq, dev, pass, [&] { return epilogue(mo, mc); });
 }
 } // extern "C++"
 
@@ -1209,24 +1304,16 @@ static int eci_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double jitter,
 {
     cudaStream_t st = o->stream;
     if (o->N == 0) { // eci.hpp:86: no objective samples, every value is 0 and the first candidate wins
-        if (dev) {
-            if (acq_out) LB_CUDA(cudaMemsetAsync(acq_out, 0, sizeof(double) * M, st));
-            LB_CUDA(cudaMemsetAsync(best_val, 0, sizeof(double), st));
-            LB_CUDA(cudaMemsetAsync(best_idx, 0, sizeof(int64_t), st));
-        }
-        else {
-            if (acq_out) std::fill(acq_out, acq_out + M, 0.0);
-            *best_val = 0.0;
-            *best_idx = 0;
-        }
-        return LB_OK;
+        int rc;
+        if ((rc = zero_fill(acq_out, M, dev, st)) || (rc = zero_fill(best_val, 1, dev, st))) return rc;
+        return zero_fill(best_idx, 1, dev, st);
     }
     if (o->D <= 0 || !o->kernel_set) return LB_ERR_STATE;
     const bool use_con = c && c->N > 0; // eci.hpp:124: Pf = 1 without constraint samples
     if (use_con && c->D != o->D) return LB_ERR_ARG;
     if (use_con && !c->kernel_set) return LB_ERR_STATE;
     lb_gp_full* cu = use_con ? c : nullptr;
-    return pair_locked(o, cu, M, Xq, dev, obj_mean_at_q, con_mean_at_q, acq_out, best_val, best_idx, false,
+    return pair_argmax_locked(o, cu, M, Xq, dev, obj_mean_at_q, con_mean_at_q, acq_out, best_val, best_idx, false,
         [&](const double* dMeanObj, const double* dMeanCon, double* dAcq, double* dBV, long long* dBI) {
             const int Po = n_outputs(o), Pc = use_con ? n_outputs(c) : 1;
             return lb_launch_eci_full(st, f_max, jitter, M, o->ex.ws.dMu.get(), Po, dMeanObj, obj_mean_const, o->ex.ws.dS2.get(),
@@ -1244,14 +1331,10 @@ static int eci_common(const lb_gp* obj, const lb_gp* con, const double* eci_para
     lb_gp_full* o = full(obj);
     lb_gp_full* c = con ? full(con) : nullptr;
     LB_DEVICE(o);
-    if (!c) {
-        std::lock_guard<std::mutex> lock(o->ex.qmutex);
-        return eci_locked(o, nullptr, eci_params[0], eci_params[1], M, Xq, dev, obj_mean_at_q, obj_mean_const, nullptr, 0.0, acq_out,
-            best_val, best_idx);
-    }
-    std::scoped_lock lock(o->ex.qmutex, c->ex.qmutex); // deadlock-free whatever order other callers pass the pair in
-    return eci_locked(o, c, eci_params[0], eci_params[1], M, Xq, dev, obj_mean_at_q, obj_mean_const, con_mean_at_q, con_mean_const,
-        acq_out, best_val, best_idx);
+    return with_query_locks(o, c, [&] {
+        return eci_locked(o, c, eci_params[0], eci_params[1], M, Xq, dev, obj_mean_at_q, obj_mean_const, con_mean_at_q, con_mean_const,
+            acq_out, best_val, best_idx);
+    });
 }
 
 int lb_eci_argmax(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq_rowmajor,
@@ -1269,12 +1352,17 @@ int lb_eci_argmax_dev(const lb_gp* obj, const lb_gp* con, const double* eci_para
         dAcq_out, dBest_val, dBest_idx);
 }
 
-// The k x 2 front sorted by f[0], stably by input index (ehvi2d's std::sort gives the same sum for a mutually non-dominated front);
-// false for a non-finite value
-static bool sorted_front(const double* front, int64_t k, std::vector<double>* sorted)
+// The argument checks of lb_ehvi_argmax / lb_ehvi_grad that need no lock, and the k x 2 front sorted by f[0], stably by input index
+// (ehvi2d's std::sort gives the same sum for a mutually non-dominated front)
+static int ehvi_front(const lb_gp* m0, const lb_gp* m1, const double* ref_point, int64_t k, const double* front, int64_t M,
+    const double* Xq, std::vector<double>* sorted)
 {
+    if (!m0 || !m1 || m0 == m1 || !ref_point || k < 0 || (k > 0 && !front) || M <= 0 || !Xq) return LB_ERR_ARG;
+    if (m0->device != m1->device) return LB_ERR_ARG;
+    if (!std::isfinite(ref_point[0]) || !std::isfinite(ref_point[1])) return LB_ERR_ARG;
+    if (k > LB_EHVI_MAX_K) return LB_ERR_UNSUPPORTED; // before the front is read
     for (int64_t i = 0; i < 2 * k; ++i)
-        if (!std::isfinite(front[i])) return false;
+        if (!std::isfinite(front[i])) return LB_ERR_ARG;
     std::vector<int64_t> ord((size_t)k);
     for (int64_t i = 0; i < k; ++i) ord[(size_t)i] = i;
     std::stable_sort(ord.begin(), ord.end(), [&](int64_t a, int64_t b) { return front[2 * a] < front[2 * b]; });
@@ -1283,21 +1371,30 @@ static bool sorted_front(const double* front, int64_t k, std::vector<double>* so
         (*sorted)[(size_t)(2 * i)] = front[2 * ord[(size_t)i]];
         (*sorted)[(size_t)(2 * i + 1)] = front[2 * ord[(size_t)i] + 1];
     }
-    return true;
+    return LB_OK;
+}
+
+// ehvi_front's sorted front into a's dFront, on a's stream
+static int upload_front(lb_gp_full* a, const std::vector<double>& sorted)
+{
+    if (sorted.empty()) return LB_OK;
+    const size_t bytes = sizeof(double) * sorted.size();
+    int rc = ensure(a, a->ex.ws.dFront, bytes);
+    if (rc) return rc;
+    LB_CUDA(cudaMemcpyAsync(a->ex.ws.dFront.get(), sorted.data(), bytes, cudaMemcpyHostToDevice, a->stream));
+    return LB_OK;
 }
 
 // experimental/acqui/ehvi.hpp:70-79 over the models m0 and m1 (ehvi.cu: ehvi_kernel), the front and the reference point on the
-// host.  The front is sorted by f[0] once (sorted_front).
+// host.  The front is sorted by f[0] once (ehvi_front).
 static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point, int64_t k, const double* front, int64_t M,
     const double* Xq, bool dev, const double* mean0_at_q, double mean0_const, const double* mean1_at_q, double mean1_const,
     double* acq_out, double* best_val, int64_t* best_idx)
 {
-    if (!m0 || !m1 || m0 == m1 || !ref_point || k < 0 || (k > 0 && !front) || M <= 0 || !Xq || !best_val || !best_idx) return LB_ERR_ARG;
-    if (m0->device != m1->device) return LB_ERR_ARG;
-    if (!std::isfinite(ref_point[0]) || !std::isfinite(ref_point[1])) return LB_ERR_ARG;
-    if (k > LB_EHVI_MAX_K) return LB_ERR_UNSUPPORTED; // before the front is read
+    if (!best_val || !best_idx) return LB_ERR_ARG;
     std::vector<double> sorted;
-    if (!sorted_front(front, k, &sorted)) return LB_ERR_ARG;
+    int rc = ehvi_front(m0, m1, ref_point, k, front, M, Xq, &sorted);
+    if (rc) return rc;
     lb_gp_full* a = full(m0);
     lb_gp_full* b = full(m1);
     LB_DEVICE(a);
@@ -1305,14 +1402,11 @@ static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point
     if (a->D <= 0 || !a->kernel_set || b->D <= 0 || !b->kernel_set) return LB_ERR_STATE;
     if (a->D != b->D) return LB_ERR_ARG;
     cudaStream_t st = a->stream;
-    return pair_locked(a, b, M, Xq, dev, mean0_at_q, mean1_at_q, acq_out, best_val, best_idx, true,
+    return pair_argmax_locked(a, b, M, Xq, dev, mean0_at_q, mean1_at_q, acq_out, best_val, best_idx, true,
         [&](const double* dMean0, const double* dMean1, double* dAcq, double* dBV, long long* dBI) {
             QueryWs& w = a->ex.ws;
             int rc;
-            if (k > 0) {
-                if ((rc = ensure(a, w.dFront, sizeof(double) * 2 * k))) return rc;
-                LB_CUDA(cudaMemcpyAsync(w.dFront.get(), sorted.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
-            }
+            if ((rc = upload_front(a, sorted))) return rc;
             const int Pa = n_outputs(a), Pb = n_outputs(b);
             if ((rc = lb_launch_ehvi(st, ref_point[0], ref_point[1], k, w.dFront.get(), M, w.dMu.get(), Pa, dMean0, mean0_const, w.dS2.get(), b->ex.ws.dMu.get(), Pb,
                      dMean1, mean1_const, b->ex.ws.dS2.get(), dAcq, &a->launches)))
@@ -1338,105 +1432,6 @@ int lb_ehvi_argmax_dev(const lb_gp* m0, const lb_gp* m1, const double* ref_point
 
 // ---- gradients of the two-model acquisitions (lb_eci_grad, lb_ehvi_grad) -------------------------------------------------------
 
-// What a gradient over two handles shares, in the manner of pair_locked: both handles' qmutex are held.  The candidates are uploaded
-// once; each handle's gradient pass (grad_fill, no acquisition) runs on its own stream, in its own chunk widths, into its own
-// workspace (mu, sigma^2 and dGrad), so that the two may overlap.  o's stream then waits for c's (c may be NULL), and
-// epilogue(mo, mc) runs over all M candidates on o's stream, mo / mc being mo_in / mc_in with the pass's outputs filled in.
-// c's stream waits for the epilogue before the locks are released: a later call on c may reallocate what the epilogue reads.
-extern "C++" {
-template <typename Epilogue>
-static int pair_grad_locked(lb_gp_full* o, lb_gp_full* c, int64_t M, const double* Xq, bool dev, const LbPairModel& mo_in,
-    const LbPairModel& mc_in, Epilogue&& epilogue)
-{
-    cudaStream_t st = o->stream;
-    int rc;
-    lb_gp_full* hs[2] = {o, c};
-    LbPairModel pm[2] = {mo_in, mc_in};
-    LbGradOut outs[2] = {};
-    for (int i = 0; i < 2; ++i) {
-        lb_gp_full* h = hs[i];
-        if (!h) continue;
-        if (query_path(h, M) == QP_PRIOR && h->N != 0) return LB_ERR_STATE;
-        if ((rc = ensure_eci_events(h))) return rc;
-        const size_t nd = (size_t)M * h->D;
-        if ((rc = ensure(h, h->ex.ws.dGrad, sizeof(double) * 2 * nd))) return rc;
-        outs[i].acq_id = -1; // mu, sigma^2 and their gradients only
-        pm[i].dmu = outs[i].dmu = h->ex.ws.dGrad.get();
-        pm[i].ds2 = outs[i].ds2 = h->ex.ws.dGrad.get() + nd;
-    }
-    const double* dXq = nullptr; // one upload, read by both passes
-    if ((rc = candidates_on_device(o, Xq, M, dev, &dXq))) return rc;
-    if (c) {
-        LB_CUDA(cudaEventRecord(o->ex.ev_eci[0], st));
-        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[0], 0));
-    }
-    int rcs[2] = {LB_OK, LB_OK};
-    for (int i = 0; i < 2 && hs[i] && rcs[0] == LB_OK; ++i) rcs[i] = grad_fill(hs[i], M, dXq, outs[i]);
-    if (c) { // o's stream waits for c's pass (and for c's last read of o's candidate buffer)
-        LB_CUDA(cudaEventRecord(c->ex.ev_eci[0], c->stream));
-        LB_CUDA(cudaStreamWaitEvent(st, c->ex.ev_eci[0], 0));
-    }
-    if (rcs[0]) return rcs[0];
-    if (rcs[1]) return rcs[1];
-    for (int i = 0; i < 2; ++i) {
-        if (!hs[i]) continue;
-        pm[i].mu = hs[i]->ex.ws.dMu.get();
-        pm[i].p = n_outputs(hs[i]);
-        pm[i].s2 = hs[i]->ex.ws.dS2.get();
-    }
-    rc = epilogue(pm[0], pm[1]);
-    if (c) {
-        LB_CUDA(cudaEventRecord(o->ex.ev_eci[1], st));
-        LB_CUDA(cudaStreamWaitEvent(c->stream, o->ex.ev_eci[1], 0));
-    }
-    if (rc) return rc;
-    LB_CUDA(cudaGetLastError());
-    return LB_OK;
-}
-} // extern "C++"
-
-// The host ends of a two-model gradient call: in host mode, device copies of the means and their gradients (NULL stays NULL) and
-// device outputs in `tmp` on o's stream; the outputs back to the host and one synchronisation at the end.  dev: the pointers as
-// they are, no synchronisation.
-struct PairGradIo {
-    StreamTemps tmp;
-    cudaStream_t st;
-    bool dev;
-    PairGradIo(int device, cudaStream_t s, bool d) : tmp(device, s), st(s), dev(d) {}
-    int in(const double* src, size_t n, const double** out)
-    {
-        *out = src;
-        if (!src || dev) return LB_OK;
-        double* p = nullptr;
-        int rc = tmp.alloc(sizeof(double) * n, &p);
-        if (rc) return rc;
-        LB_CUDA(cudaMemcpyAsync(p, src, sizeof(double) * n, cudaMemcpyHostToDevice, st));
-        *out = p;
-        return LB_OK;
-    }
-    int out(double* dst, size_t n, double** out)
-    {
-        *out = dst;
-        return (!dst || dev) ? LB_OK : tmp.alloc(sizeof(double) * n, out);
-    }
-    int finish(double* acq_host, const double* dAcq, int64_t M, double* grad_host, const double* dGrad, int D)
-    {
-        if (dev) return LB_OK;
-        if (acq_host) LB_CUDA(cudaMemcpyAsync(acq_host, dAcq, sizeof(double) * M, cudaMemcpyDeviceToHost, st));
-        if (grad_host) LB_CUDA(cudaMemcpyAsync(grad_host, dGrad, sizeof(double) * M * D, cudaMemcpyDeviceToHost, st));
-        LB_CUDA(cudaStreamSynchronize(st));
-        return LB_OK;
-    }
-};
-
-static bool coordinates_finite(const double* Xq, int64_t M, int D, bool dev)
-{
-    if (!dev)
-        for (int64_t i = 0; i < M * D; ++i)
-            if (!std::isfinite(Xq[i])) return false;
-    return true;
-}
-
 // lb_eci_grad(_dev) under the locks: eci_locked's cases (no objective samples: 0 everywhere; a constraint without samples: Pf = 1),
 // with query.cu's eci_grad_kernel as the epilogue
 static int eci_grad_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double jitter, int64_t M, const double* Xq, bool dev,
@@ -1448,24 +1443,17 @@ static int eci_grad_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double ji
     if (c && c->D > 0 && c->D != D) return LB_ERR_ARG;
     if (!coordinates_finite(Xq, M, D, dev)) return LB_ERR_ARG;
     cudaStream_t st = o->stream;
+    int rc;
     if (o->N == 0) { // eci.hpp:86: no objective samples, every value and gradient is 0 (before the kernel is consulted, as eci_locked)
-        if (dev) {
-            if (acq_out) LB_CUDA(cudaMemsetAsync(acq_out, 0, sizeof(double) * M, st));
-            if (grad_out) LB_CUDA(cudaMemsetAsync(grad_out, 0, sizeof(double) * M * D, st));
-        }
-        else {
-            if (acq_out) std::fill(acq_out, acq_out + M, 0.0);
-            if (grad_out) std::fill(grad_out, grad_out + M * D, 0.0);
-        }
-        return LB_OK;
+        if ((rc = zero_fill(acq_out, M, dev, st))) return rc;
+        return zero_fill(grad_out, M * D, dev, st);
     }
     if (!o->kernel_set) return LB_ERR_STATE;
     const bool use_con = c && c->N > 0; // eci.hpp:124: Pf = 1 without constraint samples
     if (use_con && !c->kernel_set) return LB_ERR_STATE;
-    PairGradIo io(o->device, st, dev);
+    Staging io(o->device, st, dev);
     LbPairModel mo{}, mc{};
     double *dAcq = nullptr, *dGrad = nullptr;
-    int rc;
     mo.mean_const = obj_mean_const;
     mc.mean_const = con_mean_const;
     if ((rc = io.in(obj_mean, M, &mo.mean)) || (rc = io.in(obj_mean_grad, (size_t)M * D, &mo.mean_grad))) return rc;
@@ -1474,8 +1462,7 @@ static int eci_grad_locked(lb_gp_full* o, lb_gp_full* c, double f_max, double ji
     rc = pair_grad_locked(o, use_con ? c : nullptr, M, Xq, dev, mo, mc, [&](const LbPairModel& a, const LbPairModel& b) {
         return lb_launch_eci_grad(st, f_max, jitter, M, D, a, b, dAcq, dGrad, &o->launches);
     });
-    if (rc) return rc;
-    return io.finish(acq_out, dAcq, M, grad_out, dGrad, D);
+    return rc ? rc : io.finish();
 }
 
 static int eci_grad_common(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq, bool dev,
@@ -1488,14 +1475,10 @@ static int eci_grad_common(const lb_gp* obj, const lb_gp* con, const double* eci
     lb_gp_full* o = full(obj);
     lb_gp_full* c = con ? full(con) : nullptr;
     LB_DEVICE(o);
-    if (!c) {
-        std::lock_guard<std::mutex> lock(o->ex.qmutex);
-        return eci_grad_locked(o, nullptr, eci_params[0], eci_params[1], M, Xq, dev, obj_mean, obj_mean_const, obj_mean_grad, nullptr,
-            0.0, nullptr, acq_out, grad_out);
-    }
-    std::scoped_lock lock(o->ex.qmutex, c->ex.qmutex);
-    return eci_grad_locked(o, c, eci_params[0], eci_params[1], M, Xq, dev, obj_mean, obj_mean_const, obj_mean_grad, con_mean,
-        con_mean_const, con_mean_grad, acq_out, grad_out);
+    return with_query_locks(o, c, [&] {
+        return eci_grad_locked(o, c, eci_params[0], eci_params[1], M, Xq, dev, obj_mean, obj_mean_const, obj_mean_grad, con_mean,
+            con_mean_const, con_mean_grad, acq_out, grad_out);
+    });
 }
 
 int lb_eci_grad(const lb_gp* obj, const lb_gp* con, const double* eci_params, int64_t M, const double* Xq_rowmajor,
@@ -1518,12 +1501,9 @@ static int ehvi_grad_common(const lb_gp* m0, const lb_gp* m1, const double* ref_
     const double* Xq, bool dev, const double* mean0, double mean0_const, const double* mean0_grad, const double* mean1,
     double mean1_const, const double* mean1_grad, double* acq_out, double* grad_out)
 {
-    if (!m0 || !m1 || m0 == m1 || !ref_point || k < 0 || (k > 0 && !front) || M <= 0 || !Xq) return LB_ERR_ARG;
-    if (m0->device != m1->device) return LB_ERR_ARG;
-    if (!std::isfinite(ref_point[0]) || !std::isfinite(ref_point[1])) return LB_ERR_ARG;
-    if (k > LB_EHVI_MAX_K) return LB_ERR_UNSUPPORTED; // before the front is read
     std::vector<double> sorted;
-    if (!sorted_front(front, k, &sorted)) return LB_ERR_ARG;
+    int rc = ehvi_front(m0, m1, ref_point, k, front, M, Xq, &sorted);
+    if (rc) return rc;
     if (m0->precision != LB_PREC_FP64 || m1->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
     lb_gp_full* a = full(m0);
     lb_gp_full* b = full(m1);
@@ -1534,10 +1514,9 @@ static int ehvi_grad_common(const lb_gp* m0, const lb_gp* m1, const double* ref_
     const int D = a->D;
     if (!coordinates_finite(Xq, M, D, dev)) return LB_ERR_ARG;
     cudaStream_t st = a->stream;
-    PairGradIo io(a->device, st, dev);
+    Staging io(a->device, st, dev);
     LbPairModel g0{}, g1{};
     double *dAcq = nullptr, *dGrad = nullptr;
-    int rc;
     g0.mean_const = mean0_const;
     g1.mean_const = mean1_const;
     if ((rc = io.in(mean0, M, &g0.mean)) || (rc = io.in(mean0_grad, (size_t)M * D, &g0.mean_grad)) || (rc = io.in(mean1, M, &g1.mean))
@@ -1545,16 +1524,11 @@ static int ehvi_grad_common(const lb_gp* m0, const lb_gp* m1, const double* ref_
         return rc;
     if ((rc = io.out(acq_out, M, &dAcq)) || (rc = io.out(grad_out, (size_t)M * D, &dGrad))) return rc;
     rc = pair_grad_locked(a, b, M, Xq, dev, g0, g1, [&](const LbPairModel& p0, const LbPairModel& p1) {
-        QueryWs& w = a->ex.ws;
-        if (k > 0) {
-            const int r = ensure(a, w.dFront, sizeof(double) * 2 * k);
-            if (r) return r;
-            LB_CUDA(cudaMemcpyAsync(w.dFront.get(), sorted.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
-        }
-        return lb_launch_ehvi_grad(st, ref_point[0], ref_point[1], k, w.dFront.get(), M, D, p0, p1, dAcq, dGrad, &a->launches);
+        const int r = upload_front(a, sorted);
+        if (r) return r;
+        return lb_launch_ehvi_grad(st, ref_point[0], ref_point[1], k, a->ex.ws.dFront.get(), M, D, p0, p1, dAcq, dGrad, &a->launches);
     });
-    if (rc) return rc;
-    return io.finish(acq_out, dAcq, M, grad_out, dGrad, D);
+    return rc ? rc : io.finish();
 }
 
 int lb_ehvi_grad(const lb_gp* m0, const lb_gp* m1, const double* ref_point, int64_t k, const double* front_rowmajor, int64_t M,
@@ -1590,16 +1564,10 @@ static int pareto_common(const lb_gp* hc, int64_t n, int K, const double* objs, 
     int herr = 0;
     int rc;
     {
-        StreamTemps tmp(h->device, st);
+        Staging io(h->device, st, dev);
         int* dKeep = nullptr;
-        const double* dO = objs;
-        if ((rc = tmp.alloc(sizeof(int) * (n + 1), &dKeep))) return rc;
-        if (!dev) {
-            double* dObj = nullptr;
-            if ((rc = tmp.alloc(sizeof(double) * n * K, &dObj))) return rc;
-            LB_CUDA(cudaMemcpyAsync(dObj, objs, sizeof(double) * n * K, cudaMemcpyHostToDevice, st));
-            dO = dObj;
-        }
+        const double* dO = nullptr;
+        if ((rc = io.tmp.alloc(sizeof(int) * (n + 1), &dKeep)) || (rc = io.in(objs, (size_t)(n * K), &dO))) return rc;
         LB_CUDA(cudaMemsetAsync(dKeep + n, 0, sizeof(int), st));
         if ((rc = lb_launch_pareto(st, n, K, dO, dKeep, dKeep + n, &h->launches))) return rc;
         LB_CUDA(cudaMemcpyAsync(keep.data(), dKeep, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
@@ -1664,15 +1632,15 @@ static int sparsify_common(const lb_gp* hc, int64_t N, int D, const double* X, i
         return LB_OK;
     }
     if (dev) return lb_run_sparsify(h, st, N, D, X, max_points, (long long*)kept, n_kept, (long long*)removed, removed_score, &h->launches);
-    StreamTemps tmp(h->device, st);
-    double* dX = nullptr;
+    Staging io(h->device, st, false); // the outputs' lengths are known after the run: their copies back stay here
+    const double* dX = nullptr;
     long long *dKept = nullptr, *dRm = nullptr;
     double* dRs = nullptr;
     int rc;
-    if ((rc = tmp.alloc(sizeof(double) * N * D, &dX)) || (rc = tmp.alloc(sizeof(long long) * N, &dKept))
-        || (removed && (rc = tmp.alloc(sizeof(long long) * N, &dRm))) || (removed_score && (rc = tmp.alloc(sizeof(double) * N, &dRs))))
+    if ((rc = io.in(X, (size_t)(N * D), &dX)) || (rc = io.tmp.alloc(sizeof(long long) * N, &dKept))
+        || (removed && (rc = io.tmp.alloc(sizeof(long long) * N, &dRm)))
+        || (removed_score && (rc = io.tmp.alloc(sizeof(double) * N, &dRs))))
         return rc;
-    LB_CUDA(cudaMemcpyAsync(dX, X, sizeof(double) * N * D, cudaMemcpyHostToDevice, st));
     if ((rc = lb_run_sparsify(h, st, N, D, dX, max_points, dKept, n_kept, dRm, dRs, &h->launches))) return rc;
     const int64_t nr = N - *n_kept;
     LB_CUDA(cudaMemcpyAsync(kept, dKept, sizeof(int64_t) * *n_kept, cudaMemcpyDeviceToHost, st));
@@ -1734,8 +1702,8 @@ int lb_kernel_grad_log_lik(lb_gp* hh, int optimize_noise, double* grad)
 }
 
 // GP::compute_log_lik and compute_kernel_grad_log_lik at R kernel states of this handle's data (lml_batch.cu), under the query
-// lock.  The per-vector kernel state is derived on the host exactly as lb_set_kernel derives it (same std::exp, same reciprocals),
-// so a vector sees the K the single path builds.
+// lock.  The per-vector kernel state is derived on the host by lb_set_kernel's kernel_state, so a vector sees the K the single
+// path builds.
 static int lml_grad_batch_common(lb_gp* hh, int kernel_id, int64_t R, int n_hparams, const double* log_hparams, const double* noise,
     int optimize_noise, double* lik, double* grad, int* info, bool dev)
 {
@@ -1744,15 +1712,8 @@ static int lml_grad_batch_common(lb_gp* hh, int kernel_id, int64_t R, int n_hpar
     if (R <= 0 || R > INT32_MAX || !log_hparams || !noise || !lik) return LB_ERR_ARG;
     if (kernel_id < 0 || kernel_id > 3) return LB_ERR_ARG;
     const int Draw = hh->D;
-    int klam = 0;
-    if (kernel_id == LB_K_SE_ARD) {
-        const int rest = n_hparams - 1 - Draw;
-        if (rest < 0 || rest % Draw != 0) return LB_ERR_ARG;
-        klam = rest / Draw;
-        if (klam > LB_MAX_LAMBDA || Draw + klam > LB_MAX_D) return LB_ERR_UNSUPPORTED;
-    }
-    else if (n_hparams != 2)
-        return LB_ERR_ARG;
+    const int klam = hparam_klam(kernel_id, Draw, n_hparams);
+    if (klam < 0) return klam;
     if (hh->N > LB_LML_BATCH_MAX_N) return LB_ERR_UNSUPPORTED;
     lb_gp_full* h = full(hh);
     LB_DEVICE(h);
@@ -1774,51 +1735,20 @@ static int lml_grad_batch_common(lb_gp* hh, int kernel_id, int64_t R, int n_hpar
         if (!std::isfinite(hp[i])) return LB_ERR_ARG;
     for (int64_t r = 0; r < R; ++r)
         if (!std::isfinite(no[r])) return LB_ERR_ARG;
-    // per vector: sf2, l, c1, c2, noise, 0, 0, 0, 1/ell (Draw), Lambda (Draw x klam) - lb_set_kernel's arithmetic
-    const int stride = kernel_id == LB_K_SE_ARD ? 8 + Draw * (1 + klam) : 8;
-    std::vector<double> prm((size_t)(R * stride), 0.0);
-    for (int64_t r = 0; r < R; ++r) {
-        const double* p = hp + r * n_hparams;
-        double* o = prm.data() + r * stride;
-        if (kernel_id == LB_K_SE_ARD) {
-            o[0] = std::exp(2.0 * p[n_hparams - 1]);
-            o[1] = 1.0;
-            for (int d = 0; d < Draw; ++d) o[8 + d] = 1.0 / std::exp(p[d]);
-            std::memcpy(o + 8 + Draw, p + Draw, sizeof(double) * Draw * klam);
-        }
-        else {
-            const double l = std::exp(p[0]);
-            o[0] = std::exp(2.0 * p[1]);
-            o[1] = l;
-            if (kernel_id == LB_K_MATERN52) { o[2] = std::sqrt(5.0) / l; o[3] = 5.0 / (3.0 * (l * l)); }
-            else if (kernel_id == LB_K_MATERN32) o[2] = std::sqrt(3.0) / l;
-            else o[2] = 1.0 / (l * l);
-        }
-        o[4] = no[r];
-    }
+    std::vector<KernParams> kps((size_t)R);
+    for (int64_t r = 0; r < R; ++r) kernel_state(kps[(size_t)r], kernel_id, Draw, klam, hp + r * n_hparams, n_hparams, no[r]);
     const int nh = n_hparams + (optimize_noise ? 1 : 0);
+    Staging io(h->device, st, dev);
+    double *dLik = nullptr, *dGrad = nullptr;
+    int* dInfo = nullptr;
     int rc;
-    {
-        StreamTemps tmp(h->device, st);
-        double *dPrm = nullptr, *dLik = lik, *dGrad = grad;
-        int* dInfo = info;
-        if ((rc = tmp.alloc(sizeof(double) * prm.size(), &dPrm))) return rc;
-        if (!dev) {
-            if ((rc = tmp.alloc(sizeof(double) * R, &dLik)) || (grad && (rc = tmp.alloc(sizeof(double) * R * nh, &dGrad)))
-                || (info && (rc = tmp.alloc(sizeof(int) * R, &dInfo))))
-                return rc;
-        }
-        LB_CUDA(cudaMemcpyAsync(dPrm, prm.data(), sizeof(double) * prm.size(), cudaMemcpyHostToDevice, st));
-        if ((rc = lb_launch_lml_batch(st, tmp, kernel_id, h->dX, h->Np, h->dY, (int)h->N, Draw, klam, h->P, dPrm, stride, (int)R, nh,
-                 optimize_noise ? 1 : 0, dLik, dGrad, dInfo, &h->launches)))
-            return rc;
-        if (!dev) {
-            LB_CUDA(cudaMemcpyAsync(lik, dLik, sizeof(double) * R, cudaMemcpyDeviceToHost, st));
-            if (grad) LB_CUDA(cudaMemcpyAsync(grad, dGrad, sizeof(double) * R * nh, cudaMemcpyDeviceToHost, st));
-            if (info) LB_CUDA(cudaMemcpyAsync(info, dInfo, sizeof(int) * R, cudaMemcpyDeviceToHost, st));
-        }
-        LB_CUDA(cudaStreamSynchronize(st));
-    }
+    if ((rc = io.out(lik, (size_t)R, &dLik)) || (rc = io.out(grad, (size_t)(R * nh), &dGrad)) || (rc = io.out(info, (size_t)R, &dInfo)))
+        return rc;
+    if ((rc = lb_launch_lml_batch(st, io.tmp, kps.data(), hp, n_hparams, (int)R, h->dX, h->Np, h->dY, (int)h->N, h->P, nh,
+             optimize_noise ? 1 : 0, dLik, dGrad, dInfo, &h->launches)))
+        return rc;
+    if ((rc = io.finish())) return rc;
+    if (dev) LB_CUDA(cudaStreamSynchronize(st)); // the device outputs are complete on return too
     return LB_OK;
 }
 

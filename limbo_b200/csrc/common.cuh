@@ -677,10 +677,11 @@ int lb_launch_linv(lb_gp* h);
 int lb_launch_kinv(lb_gp* h);
 int lb_launch_symmetrize(lb_gp* h, double* dA);
 int lb_launch_grad(lb_gp* h, int optimize_noise, double* dGrad);
-// lml_batch.cu: one launch; dPrm is R x stride (lb_lml_grad_batch's per-vector kernel state), dGrad NULL = likelihood only
-int lb_launch_lml_batch(cudaStream_t st, StreamTemps& tmp, int kernel_id, const double* dX, int64_t ldx, const double* dY, int N,
-    int Draw, int klam, int P, const double* dPrm, int stride, int R, int nh, int optimize_noise, double* dLik, double* dGrad,
-    int* dInfo, long long* launches);
+// lml_batch.cu: one launch over the R kernel states kps (one kernel and layout; lambda unset) with the Lambda columns of the host
+// rows hparams (R x n_hparams, lb_lml_grad_batch's); dGrad NULL = likelihood only
+int lb_launch_lml_batch(cudaStream_t st, StreamTemps& tmp, const KernParams* kps, const double* hparams, int n_hparams, int R,
+    const double* dX, int64_t ldx, const double* dY, int N, int P, int nh, int optimize_noise, double* dLik, double* dGrad, int* dInfo,
+    long long* launches);
 // loo.cu
 int lb_launch_loo_value(lb_gp* h, double* dOut);
 int lb_launch_loo_grad(lb_gp* h, int optimize_noise, double* dGrad);

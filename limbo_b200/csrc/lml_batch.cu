@@ -17,6 +17,7 @@
 // measured); the code is the same, through generic pointers.  Every reduction runs in a fixed
 // order over a thread assignment that depends on N only, so a vector's result does not depend on R or on its place in the batch.
 #include "common.cuh"
+#include <cstring>
 #include <math_constants.h>
 
 namespace {
@@ -319,12 +320,32 @@ int launch(const LmlBatchArgs& a0, StreamTemps& tmp, cudaStream_t st, long long*
 
 } // namespace
 
-int lb_launch_lml_batch(cudaStream_t st, StreamTemps& tmp, int kernel_id, const double* dX, int64_t ldx, const double* dY, int N,
-    int Draw, int klam, int P, const double* dPrm, int stride, int R, int nh, int optimize_noise, double* dLik, double* dGrad,
-    int* dInfo, long long* launches)
+int lb_launch_lml_batch(cudaStream_t st, StreamTemps& tmp, const KernParams* kps, const double* hparams, int n_hparams, int R,
+    const double* dX, int64_t ldx, const double* dY, int N, int P, int nh, int optimize_noise, double* dLik, double* dGrad, int* dInfo,
+    long long* launches)
 {
     int rc = set_attrs();
     if (rc) return rc;
+    const int kernel_id = kps[0].id, Draw = kps[0].Draw, klam = kps[0].klam;
+    // the rows of LmlBatchArgs::prm
+    const int stride = kernel_id == LB_K_SE_ARD ? 8 + Draw * (1 + klam) : 8;
+    std::vector<double> prm((size_t)R * stride, 0.0);
+    for (int r = 0; r < R; ++r) {
+        const KernParams& kp = kps[r];
+        double* o = prm.data() + (size_t)r * stride;
+        o[0] = kp.sf2;
+        o[1] = kp.l;
+        o[2] = kp.c1;
+        o[3] = kp.c2;
+        o[4] = kp.noise;
+        if (kernel_id == LB_K_SE_ARD) {
+            std::memcpy(o + 8, kp.inv_ell, sizeof(double) * Draw);
+            std::memcpy(o + 8 + Draw, hparams + (size_t)r * n_hparams + Draw, sizeof(double) * Draw * klam);
+        }
+    }
+    double* dPrm = nullptr;
+    if ((rc = tmp.alloc(sizeof(double) * prm.size(), &dPrm))) return rc;
+    LB_CUDA(cudaMemcpyAsync(dPrm, prm.data(), sizeof(double) * prm.size(), cudaMemcpyHostToDevice, st));
     LmlBatchArgs a{};
     a.X = dX; a.ldx = ldx; a.Y = dY; a.N = N; a.Draw = Draw; a.klam = klam; a.De = Draw + klam; a.P = P;
     a.prm = dPrm; a.stride = stride; a.R = R; a.nh = nh; a.optimize_noise = optimize_noise; a.want_grad = dGrad != nullptr;

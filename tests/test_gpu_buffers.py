@@ -42,6 +42,21 @@ def _gp_round(lib):
     con.compute(list(X), list(Y[:, 1:]))
     gp.eci_argmax_batch(con, float(Y[:, 0].max()), 0.0, Xq, return_values=True)
     gp.ehvi_argmax_batch(con, [-3.0, -3.0], np.array([[1.0, 0.5], [0.5, 1.0]]), Xq, return_values=True)
+    gp.query_grad_batch(Xq[:50])
+    gp.acq_grad_batch(1, [0.0, float(Y[:, 0].max())], Xq[:50])
+    gp.eci_grad_batch(con, float(Y[:, 0].max()), 0.0, Xq[:50])
+    gp.ehvi_grad_batch(con, [-3.0, -3.0], np.array([[1.0, 0.5], [0.5, 1.0]]), Xq[:50])
+    k = gp.kernel_function()
+    gp.lml_grad_batch(np.tile(k.h_params(), (5, 1)) + rng.uniform(-0.5, 0.5, (5, k.h_params_size())))
+    dXq = torch.from_numpy(Xq[:50]).cuda()
+    dMu, dS2, dDmu, dDs2, dAcq, dGrad = (torch.zeros(n, dtype=torch.float64, device="cuda") for n in (50, 50, 50 * D, 50 * D, 50, 50 * D))
+    ep = np.array([float(Y[:, 0].max()), 0.0])
+    torch.cuda.synchronize()
+    assert lib.lb_query_grad_dev(gp._h, 50, dXq.data_ptr(), dMu.data_ptr(), dS2.data_ptr(), dDmu.data_ptr(), dDs2.data_ptr()) == 0
+    assert lib.lb_eci_grad_dev(gp._h, con._h, ep.ctypes.data, 50, dXq.data_ptr(), None, 0.0, None, None, 0.0, None, dAcq.data_ptr(),
+                               dGrad.data_ptr()) == 0
+    torch.cuda.synchronize()
+    del dXq, dMu, dS2, dDmu, dDs2, dAcq, dGrad
     gp.kernel_matrix(); gp.matrixL(); gp.inv_kernel()
     gp.compute_kernel_grad_log_loo_cv()
     gp.compute_mean_grad_log_lik()  # lb_kinv_obs_mean
