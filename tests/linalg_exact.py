@@ -1,6 +1,7 @@
-"""Matrices with an exactly known Cholesky factor, numpy restatements of the kernel derivatives, and first-order
-rounding-error bounds for the fp64 factorisation, inverse, solves and query (tests/test_linalg_exact_host.py,
-tests/test_gpu_linalg_exact.py).
+"""Matrices with an exactly known Cholesky factor, numpy restatements of the kernel derivatives (SE-ARD with its Lambda
+columns included), and first-order rounding-error bounds for the fp64 factorisation, inverse, solves and query, the
+likelihood and LOO-CV objectives and their gradients, K^-1 obs_mean, and the batched likelihood of a K built from X
+(tests/test_linalg_exact_host.py, tests/test_gpu_linalg_exact.py, tests/test_gpu_objectives_exact.py).
 
 K = L0 L0^T with L0 integer lower-triangular: a diagonal in [2^11, 2^12], strictly-lower entries in [-8, 8].  Every
 entry of K is an integer below 2^53, so any fp64 BLAS forms it exactly and its Cholesky factor is exactly L0.  The
@@ -159,88 +160,141 @@ def exact_shapes():
     return out
 
 
+
+EXACT_KLAM = (0, 1, 2, 4)
+
+
+def exact_objective(i: int, N: int):
+    """(kernel id, D, Lambda columns, optimize_noise) of the i-th exact shape: the kernels cycle through the four, SE-ARD
+    carries k = 0, 1, 2, 4 Lambda columns in turn, the noise entry alternates, and D = 20 at N = 1151 (two 16-dimension passes
+    of the gradient kernels, and dk_build's loop over 24 staged dimensions)."""
+    kid = KERNELS[i % 4]
+    klam = EXACT_KLAM[(i // 4) % 4] if kid == 0 else 0
+    D = 20 if (kid == 0 and N == 1151) else 2
+    return kid, D, klam, bool((i // 4) % 2)
+
+
+def exact_objective_params(kid, D, klam, rng) -> np.ndarray:
+    """kernel_params, with the D = 20 case's longer length scales (ell in e^[0.3, 0.8], sigma_f = e^0.1)."""
+    if D == 20:
+        lam = rng.normal(0.0, 0.5 / math.sqrt(D), D * klam) if klam else np.zeros(0)
+        return np.concatenate([rng.uniform(0.3, 0.8, D), lam, [0.1]])
+    return kernel_params(kid, D, rng, klam)
+
 # ---------------------------------------------------------------------------------------------------------------------
 # kernels: values and derivatives (the formulas of oracle/limbo_oracle.hpp, vectorised)
 # ---------------------------------------------------------------------------------------------------------------------
-def kernel_params(kid: int, D: int, rng) -> np.ndarray:
+def kernel_params(kid: int, D: int, rng, klam: int = 0) -> np.ndarray:
+    """Log-space hyper-parameters; SE-ARD with klam Lambda columns of entries N(0, 0.25 / D) (A(i, j) = p[(j + 1) D + i])."""
     if kid == 0:
-        return np.concatenate([rng.uniform(-0.7, 0.3, D), [rng.uniform(-0.3, 0.3)]])
+        ell = rng.uniform(-0.7, 0.3, D)
+        lam = rng.normal(0.0, 0.5 / math.sqrt(D), D * klam) if klam else np.zeros(0)
+        return np.concatenate([ell, lam, [rng.uniform(-0.3, 0.3)]])
     return np.array([rng.uniform(-1.0, 0.0), rng.uniform(-0.3, 0.3)])
+
+
+def ard_split(p, D):
+    """SE-ARD's (klam, 1/ell, Lambda (D x klam), sf2) from its log-space parameters, in p's dtype."""
+    klam = (p.size - 1 - D) // D
+    assert p.size == D + D * klam + 1, (p.size, D)
+    return klam, np.exp(-p[:D]), p[D:D + D * klam].reshape(klam, D).T, np.exp(2 * p[-1])
 
 
 def _sqdist(X1, X2, scale=None):
     """Squared distances from the coordinate differences (no Gram-matrix trick, which cancels for close points)."""
     A = X1 if scale is None else X1 * scale
     B = X2 if scale is None else X2 * scale
-    z = np.zeros((X1.shape[0], X2.shape[0]))
+    z = np.zeros((X1.shape[0], X2.shape[0]), dtype=A.dtype)
     for d in range(A.shape[1]):
         q = A[:, d, None] - B[None, :, d]
         z += q * q
     return z
 
 
+def _ard_z(p, X1, X2):
+    """SE-ARD's squared distance in the staged coordinates [x / ell, x^T Lambda] and its parts."""
+    klam, inv, A, sf2 = ard_split(p, X1.shape[1])
+    z = _sqdist(X1, X2, inv)
+    U1, U2 = X1 @ A, X2 @ A
+    if klam:
+        z = z + _sqdist(U1, U2)
+    return z, inv, U1, U2, sf2
+
+
 def kernel_matrix(kid: int, p: np.ndarray, X1: np.ndarray, X2: np.ndarray) -> np.ndarray:
-    """k(x1, x2) without noise, as in Kernel::kernel of each functor."""
+    """k(x1, x2) without noise, as in Kernel::kernel of each functor (in the inputs' dtype)."""
+    c = X1.dtype.type
     if kid == 0:
-        D = X1.shape[1]
-        sf2 = math.exp(2 * p[D])
-        return sf2 * np.exp(-0.5 * _sqdist(X1, X2, np.exp(-p[:D])))
-    l, sf2 = math.exp(p[0]), math.exp(2 * p[1])
+        z, _, _, _, sf2 = _ard_z(p, X1, X2)
+        return sf2 * np.exp(-z / 2)
+    l, sf2 = np.exp(p[0]), np.exp(2 * p[1])
     s = _sqdist(X1, X2)
     if kid == 3:
-        return sf2 * np.exp(-0.5 * s / (l * l))
+        return sf2 * np.exp(-s / (2 * l * l))
     r = np.sqrt(s)
     if kid == 1:
-        t1 = math.sqrt(5.0) * r / l
-        t2 = 5.0 * s / (3.0 * l * l)
-        return sf2 * (1.0 + t1 + t2) * np.exp(-t1)
-    t = math.sqrt(3.0) * r / l
-    return sf2 * (1.0 + t) * np.exp(-t)
+        t1 = np.sqrt(c(5)) * r / l
+        t2 = 5 * s / (3 * l * l)
+        return sf2 * (1 + t1 + t2) * np.exp(-t1)
+    t = np.sqrt(c(3)) * r / l
+    return sf2 * (1 + t) * np.exp(-t)
 
 
 def kernel_grads(kid: int, p: np.ndarray, X1: np.ndarray, X2: np.ndarray):
-    """Yields dk(x1, x2) / d theta_q for every hyper-parameter q (log ell_d / log l, then log sigma_f), as matrices."""
+    """Yields dk(x1, x2) / d theta_q for every hyper-parameter q as matrices, in the order of the functor's parameters: SE-ARD
+    log ell_d, then Lambda entry A(i, j) at q = (j + 1) D + i (squared_exp_ard.hpp:119-122: -k (x1 - x2)^T A(:, j) (x1 - x2)_i),
+    then log sigma_f; the isotropic kernels log l, then log sigma_f.  In the inputs' dtype (long double for the host checks)."""
+    c = X1.dtype.type
     if kid == 0:
         D = X1.shape[1]
-        sf2 = math.exp(2 * p[D])
-        inv = np.exp(-p[:D])
-        k = sf2 * np.exp(-0.5 * _sqdist(X1, X2, inv))
+        z, inv, U1, U2, sf2 = _ard_z(p, X1, X2)
+        k = sf2 * np.exp(-z / 2)
         for d in range(D):
             q = (X1[:, d, None] - X2[None, :, d]) * inv[d]
             yield q * q * k
-        yield 2.0 * k
+        for j in range(U1.shape[1]):
+            proj = U1[:, j, None] - U2[None, :, j]
+            for i in range(D):
+                yield -(proj * (X1[:, i, None] - X2[None, :, i])) * k
+        yield 2 * k
         return
-    l, sf2 = math.exp(p[0]), math.exp(2 * p[1])
+    l, sf2 = np.exp(p[0]), np.exp(2 * p[1])
     s = _sqdist(X1, X2)
     if kid == 3:
         r = s / (l * l)
-        k = sf2 * np.exp(-0.5 * r)
+        k = sf2 * np.exp(-r / 2)
         yield r * k
-        yield 2.0 * k
+        yield 2 * k
         return
     d = np.sqrt(s)
     if kid == 1:
-        t1 = math.sqrt(5.0) * d / l
-        t2 = 5.0 * s / (3.0 * l * l)
+        t1 = np.sqrt(c(5)) * d / l
+        t2 = 5 * s / (3 * l * l)
         e = np.exp(-t1)
-        yield sf2 * (e * t1 * (1.0 + t1 + t2) + (-t1 - 2.0 * t2) * e)
-        yield 2.0 * sf2 * (1.0 + t1 + t2) * e
+        yield sf2 * (e * t1 * (1 + t1 + t2) + (-t1 - 2 * t2) * e)
+        yield 2 * sf2 * (1 + t1 + t2) * e
         return
-    t = math.sqrt(3.0) * d / l
+    t = np.sqrt(c(3)) * d / l
     e = np.exp(-t)
-    yield sf2 * (-t * e + (1.0 + t) * t * e)
-    yield 2.0 * sf2 * (1.0 + t) * e
+    yield sf2 * (-t * e + (1 + t) * t * e)
+    yield 2 * sf2 * (1 + t) * e
 
 
 def kernel_eval_err(kid: int, p: np.ndarray, xmax: float, D: int) -> float:
     """Absolute bound on the fp64 evaluation error of one kernel value or derivative, inputs in [-xmax, xmax]^D.
     Every formula is sf^2 * (polynomial of degree <= 3 in rho) * exp(-rho) of the squared distance z, Lipschitz in z
-    with constant <= sf^2 (1 + a^2)(1 + rho)^2 (a: the scale of z inside rho); z itself is a sum of D squared differences
-    of (pre-scaled) coordinates, so |dz| <= gamma_{D+3} zb with zb the largest sum of (|x_d| + |y_d|)^2 / scale_d^2."""
+    with constant <= sf^2 (1 + a^2)(1 + rho)^2 (a: the scale of z inside rho); z itself is a sum of De squared differences
+    of staged coordinates u = x J, so |dz| <= gamma_{D+3} zb with zb the largest sum over e of (2 xmax sum_d |J_de|)^2.
+    SE-ARD's Lambda entries -k proj raw (proj = (x1 - x2)^T A(:, j), raw = (x1 - x2)_i, |proj| <= sqrt(zb), |raw| <= 2 xmax)
+    add sf^2 (|d proj| |raw| + |proj| |d raw| + |proj raw| |dk| / sf^2) <= sf^2 2 xmax sqrt(zb) (2 + zb) gamma_{D+3}."""
+    lam = 0.0
     if kid == 0:
-        sf2 = math.exp(2 * p[D])
-        zb = float(((2.0 * xmax * np.exp(-p[:D])) ** 2).sum())
+        klam, inv, A, sf2 = ard_split(np.asarray(p, dtype=np.float64), D)
+        J = np.hstack([np.diag(inv), A])
+        zb = float(((2.0 * xmax * np.abs(J).sum(0)) ** 2).sum())
         a2, rho = 1.0, 0.5 * zb
+        if klam:
+            lam = sf2 * 2.0 * xmax * math.sqrt(zb) * (2.0 + zb) * gamma(D + 3)
     else:
         l, sf2 = math.exp(p[0]), math.exp(2 * p[1])
         zb = D * (2.0 * xmax) ** 2
@@ -250,7 +304,7 @@ def kernel_eval_err(kid: int, p: np.ndarray, xmax: float, D: int) -> float:
         else:
             a2 = (5.0 if kid == 1 else 3.0) / (l * l)
             rho = math.sqrt(a2 * zb)
-    return sf2 * ((1.0 + a2) * (1.0 + rho) ** 2 * gamma(D + 3) * zb + gamma(32) * (1.0 + rho) ** 3 * (1.0 + zb))
+    return sf2 * ((1.0 + a2) * (1.0 + rho) ** 2 * gamma(D + 3) * zb + gamma(32) * (1.0 + rho) ** 3 * (1.0 + zb)) + lam
 
 
 def grad_reference(kid, p, X, alpha, kinv, noise, optimize_noise):
@@ -281,6 +335,164 @@ def bound_grad(case: ExactCase, kid, p, X, absum, fro, da_bound, dkinv_bound) ->
     wsum = float(np.abs(W).sum())
     ev = kernel_eval_err(kid, p, float(np.abs(X).max()), X.shape[1])
     return 0.5 * dW * fro + 2.0 * gamma(n * n + case.P + 8) * absum + 0.5 * ev * wsum
+
+
+def dk_matrices(kid, p, X, noise, optimize_noise):
+    """dK / d theta_q for every hyper-parameter (kernel_grads), then 2 noise I when the noise is optimised (kernel.hpp:90-93)."""
+    out = list(kernel_grads(kid, p, X, X))
+    if optimize_noise:
+        out.append(2 * noise * np.eye(X.shape[0], dtype=X.dtype))
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# leave-one-out cross-validation (gp.hpp:339-399) and K^-1 obs_mean (gp.hpp:313-330)
+# ---------------------------------------------------------------------------------------------------------------------
+def loo_value(alpha, kinv) -> float:
+    """sum_i,p -1/2 alpha_ip^2 / c_i - 1/2 log(1 / c_i) - 1/2 log(2 pi), c = diag(K^-1) (gp.hpp:339-351)."""
+    ic = 1 / np.diag(kinv)
+    dt = ic.dtype.type
+    return (-alpha * alpha * ic[:, None] / 2 - np.log(ic)[:, None] / 2 - np.log(2 * dt(np.pi)) / 2).sum()
+
+
+def loo_terms(alpha, kinv, dk, cols=None):
+    """(alpha Z alpha - 1/2 (1 + alpha^2 / c) diag(Z K^-1)) / c per row and output, Z = K^-1 dK (gp.hpp:353-399); cols: the
+    columns n of Z alpha and of diag(Z K^-1) = sum_n Z_in K^-1_ni to sum (the device's 128-column tiles), all by default."""
+    ic = 1 / np.diag(kinv)
+    Z = kinv @ dk
+    if cols is None:
+        za, zk = Z @ alpha, (Z * kinv).sum(1)
+    else:
+        za, zk = Z[:, cols] @ alpha[cols], (Z[:, cols] * kinv[:, cols]).sum(1)
+    return Z, za, zk, (alpha * za - (1 + alpha * alpha * ic[:, None]) * zk[:, None] / 2) * ic[:, None]
+
+
+def loo_reference(kid, p, X, alpha, kinv, noise, optimize_noise):
+    """LOO value and gradient in the dtype of the inputs (np.longdouble for the host checks)."""
+    g = [loo_terms(alpha, kinv, dk)[3].sum() for dk in dk_matrices(kid, p, X, noise, optimize_noise)]
+    return loo_value(alpha, kinv), np.array(g)
+
+
+def bound_loo(case: ExactCase, da_bound, dkinv_bound) -> float:
+    """|v^ - v| for the LOO value from K^-1 and alpha with ||d alpha_p|| <= da_bound[p] and ||dK^-1||_F <= dkinv_bound
+    (device and reference together): the derivatives -alpha / c (alpha) and 1/2 (alpha^2 / c^2 + 1 / c) (c_i = K^-1_ii) by
+    Cauchy-Schwarz, then the terms (a division, a log, four products and sums: 10 roundings each) and the sum of N P of them,
+    on the device and on the host."""
+    kinv, a = case.ref()["kinv"], case.A0
+    ic = 1.0 / np.diag(kinv)
+    w = 0.5 * (a * a * (ic * ic)[:, None] + ic[:, None]).sum(1)
+    first = float((np.linalg.norm(a * ic[:, None], axis=0) * da_bound).sum() + np.linalg.norm(w) * dkinv_bound)
+    terms = float((0.5 * a * a * ic[:, None] + 0.5 * np.abs(np.log(ic))[:, None] + 0.5 * math.log(2 * math.pi)).sum())
+    return first + 2.0 * gamma(case.N * case.P + 10) * terms
+
+
+def bound_loo_grad(case: ExactCase, kid, p, X, noise, optimize_noise, da_bound, dkinv_bound) -> np.ndarray:
+    """|g^ - g| per hyper-parameter of the LOO gradient, from K^-1 (X, ||dX||_F <= dkinv_bound), alpha (a, ||da_p|| <=
+    da_bound[p]) and dK (evaluation error ev per entry, kernel_eval_err; the noise entry's 2 noise I is exact), first order:
+      alpha:    t_ip = (a Za - 1/2 (1 + a^2/c) zk) / c moves by ic (da Za + a (Z da) - a da ic zk): by ||.||_2 per output;
+      X in Z:   Za by dX dK a (sum_ip |a ic| |dX dK a| <= ||a ic|| ||dX|| ||dK a||), zk = diag(X dK X) by (dX M)_ii + (M^T dX)_ii
+                with M = dK X: sum_i v_i ||dX_i,:|| ||M_:,i|| <= ||dX||_F ||v ||M_:,i|| ||, twice (v_i = sum_p (1 + a^2 ic) ic / 2);
+      c = diag(X): d t / d c_i = (-a Za + zk / 2 + a^2 zk ic) ic^2, by ||.||_2;
+      Z product (DMMA on the device, BLAS on the host): |dZ| <= gamma_N |X||dK| = gamma_N G; the epilogue's sums over the N
+                columns (per 128-column tile, then over the T tiles) add gamma_{N+T} |Z||a| <= G|a| and |Z||X| <= G|X|:
+                |dZa| <= 2 gamma_{N+T+2} G|a|, |dzk_i| <= 2 gamma_{N+T+2} (G|X|)_ii;
+      ev:       |dZa_ip| <= ev (|X| 1)_i sum |a_p|, |dzk_i| <= ev (|X| 1)_i^2;
+      the terms and the final sum: gamma_{NP+10} sum |t|.
+    The rounding and evaluation terms are counted twice (device and host)."""
+    n, P = case.N, case.P
+    Xk, a = case.ref()["kinv"], case.A0
+    ic = 1.0 / np.diag(Xk)
+    absX = np.abs(Xk)
+    r1 = absX.sum(1)
+    v = 0.5 * ((1.0 + a * a * ic[:, None]) * ic[:, None]).sum(1)
+    T = max(1, -(-n // TILE))
+    gz = gamma(n + T + 2)
+    ev = kernel_eval_err(kid, p, float(np.abs(X).max()), X.shape[1])
+    dks = dk_matrices(kid, p, X, noise, optimize_noise)
+    out = []
+    for q, dk in enumerate(dks):
+        is_noise = optimize_noise and q == len(dks) - 1
+        Z, za, zk, t = loo_terms(a, Xk, dk)
+        aic = a * ic[:, None]
+        b = 0.0
+        for pp in range(P):
+            b += da_bound[pp] * (np.linalg.norm(ic * za[:, pp]) + np.linalg.norm(Z.T @ aic[:, pp])
+                                 + np.linalg.norm(ic * ic * a[:, pp] * zk))
+        M = dk @ Xk
+        b += dkinv_bound * (float(np.linalg.norm(aic, axis=0) @ np.linalg.norm(dk @ a, axis=0))
+                            + 2.0 * np.linalg.norm(v * np.linalg.norm(M, axis=0)))
+        s = ((-a * za + 0.5 * zk[:, None] + a * a * zk[:, None] * ic[:, None]) * (ic * ic)[:, None]).sum(1)
+        b += dkinv_bound * np.linalg.norm(s)
+        G = absX @ np.abs(dk)
+        rnd = float((np.abs(aic) * (2.0 * gz * (G @ np.abs(a)))).sum() + (v * 2.0 * gz * (G * absX).sum(1)).sum())
+        evt = 0.0 if is_noise else ev * float((np.abs(aic) * (r1[:, None] * np.abs(a).sum(0)[None, :])).sum() + (v * r1 * r1).sum())
+        fin = gamma(n * P + 10) * float((np.abs(a * za * ic[:, None]) + 0.5 * (1.0 + a * a * ic[:, None]) * np.abs(zk)[:, None]
+                                         * ic[:, None]).sum())
+        out.append(b + 2.0 * (rnd + evt + fin))
+    return np.array(out)
+
+
+def bound_kinv_obs(case: ExactCase, dkinv_bound) -> np.ndarray:
+    """2-norm bound per column on (K^-1 Y)^ - A0 (Y = K A0 exactly): ||dX||_2 ||y_p|| from the K^-1 bound, and the dot products
+    over 32 slices of N and the sum of the 32 partials, gamma_{N+32} || |X| |y_p| ||_2."""
+    Xk, Y = case.ref()["kinv"], case.Y
+    return dkinv_bound * np.linalg.norm(Y, axis=0) + gamma(case.N + 32) * np.linalg.norm(np.abs(Xk) @ np.abs(Y), axis=0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the log-likelihood and its gradient of a K built from X (lb_lml_grad_batch)
+# ---------------------------------------------------------------------------------------------------------------------
+JITTER = 1e-8  # kernel.hpp:83, on the diagonal of every K
+
+
+class LmlCase:
+    """GP::compute_log_lik and compute_kernel_grad_log_lik (gp.hpp:267-311) at one kernel state, in fp64 through LAPACK, with
+    the quantities of its first-order bound (bound())."""
+
+    def __init__(self, kid, p, noise, X, Y, optimize_noise):
+        import scipy.linalg as sl
+        self.kid, self.p, self.noise, self.X, self.Y, self.on = kid, np.asarray(p, dtype=np.float64), noise, X, Y, optimize_noise
+        n = X.shape[0]
+        K = kernel_matrix(kid, self.p, X, X)
+        K[np.diag_indices(n)] += noise + JITTER
+        ev = sl.eigh(K, eigvals_only=True)
+        self.K, self.lmin, self.lmax = K, float(ev[0]), float(ev[-1])
+        self.kappa = self.lmax / self.lmin
+        L = np.linalg.cholesky(K)
+        self.L = L
+        self.alpha = sl.cho_solve((L, True), Y)
+        Li = sl.solve_triangular(L, np.eye(n), lower=True)
+        self.kinv = Li.T @ Li
+        self.logdet = 2.0 * float(np.log(np.diag(L)).sum())
+        ya = float((Y * self.alpha).sum())
+        self.lik = -0.5 * ya - 0.5 * self.logdet - 0.5 * n * math.log(2 * math.pi)
+        self.grad, self.absum, self.fro = grad_reference(kid, self.p, X, self.alpha, self.kinv, noise, optimize_noise)
+
+    def bound(self):
+        """(likelihood bound, gradient bound per entry) of ONE fp64 evaluation from X (the device's or this reference's):
+          K:        |dK_ij| <= ev (kernel_eval_err) and 2u K_ii on the diagonal (noise and jitter added): ||dK_b||_F;
+          factor:   backward error gamma_{3N+1} || |L||L^T| ||_F of the Cholesky factorisation and both solves (Thm 10.3/10.4),
+                    added to dK_b: dK;
+          alpha:    ||d alpha_p|| <= ||K^-1||_2 dK ||alpha_p||;  K^-1: ||dX||_F <= ||K^-1||_2^2 dK sqrt(N) (section 14.2);
+          log det:  |tr(K^-1 dK)| <= ||K^-1||_F dK, and gamma_{N+4} sum |2 log L_ii| for the logs and their sum;
+          y^T alpha: sum_p ||y_p|| ||d alpha_p|| + gamma_{NP+2} sum |y||alpha|; the likelihood's three terms: 4 roundings;
+          gradient: bound_grad's terms from d alpha and dX, ev sum |W| / 2 and gamma_{N^2+P+8} sum |W||dk|."""
+        n = self.X.shape[0]
+        ev = kernel_eval_err(self.kid, self.p, float(np.abs(self.X).max()), self.X.shape[1])
+        absL = np.abs(self.L)
+        dKb = math.sqrt(n * (n - 1)) * ev + math.sqrt(n) * (ev + 2.0 * U * float(np.diag(self.K).max()))
+        dK = dKb + gamma(3 * n + 1) * float(np.linalg.norm(absL @ absL.T))
+        nki = 1.0 / self.lmin
+        da = nki * dK * np.linalg.norm(self.alpha, axis=0)
+        dX = nki * nki * dK * math.sqrt(n)
+        dld = math.sqrt(n) * nki * dK + gamma(n + 4) * float(np.abs(2.0 * np.log(np.diag(self.L))).sum())
+        ya = float((self.Y * self.alpha).sum())
+        dya = float((np.linalg.norm(self.Y, axis=0) * da).sum()) + gamma(n * self.Y.shape[1] + 2) * float(np.abs(self.Y * self.alpha).sum())
+        blik = 0.5 * (dya + dld) + gamma(4) * (0.5 * abs(ya) + 0.5 * abs(self.logdet) + 0.5 * n * math.log(2 * math.pi))
+        W = self.alpha @ self.alpha.T - self.kinv
+        dW = float(2.0 * (da * np.linalg.norm(self.alpha, axis=0)).sum() + dX)
+        bgrad = 0.5 * dW * self.fro + 2.0 * gamma(n * n + self.Y.shape[1] + 8) * self.absum + 0.5 * ev * float(np.abs(W).sum())
+        return blik, bgrad
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -664,6 +876,41 @@ class Handle:
                                                self.C.addressof(best), self.C.addressof(idx)), "lb_acq_argmax")
         return v, best.value, idx.value
 
+
+    def loo_cv(self) -> float:
+        v = self.C.c_double()
+        self._lib.check(self.lib.lb_log_loo_cv(self.h, self.C.addressof(v)), "lb_log_loo_cv")
+        return v.value
+
+    def loo_grad(self, optimize_noise: bool):
+        g = np.empty(self.nh + (1 if optimize_noise else 0))
+        self._lib.check(self.lib.lb_kernel_grad_log_loo_cv(self.h, int(optimize_noise), g.ctypes.data), "lb_kernel_grad_log_loo_cv")
+        return g
+
+    def kinv_obs(self):
+        """lb_kinv_obs_mean: K^-1 obs_mean (N x P)."""
+        out = np.empty((self.N, self.P), order="F")
+        self._lib.check(self.lib.lb_kinv_obs_mean(self.h, out.ctypes.data), "lb_kinv_obs_mean")
+        return out
+
+    def append(self, x, Yall):
+        """lb_append: one sample x (D) and the refreshed (N + 1) x P obs_mean."""
+        x = np.ascontiguousarray(x, dtype=np.float64)
+        Yall = np.asfortranarray(Yall, dtype=np.float64)
+        self._lib.check(self.lib.lb_append(self.h, x.ctypes.data, Yall.ctypes.data), "lb_append")
+        self.N += 1
+        self._keep = (self._keep[0], Yall)
+
+    def lml_grad_batch(self, kid, H, noise, optimize_noise: bool):
+        """lb_lml_grad_batch at the rows of H (R x n_hparams) and noise (R): (lik, grad, info)."""
+        H = np.ascontiguousarray(H, dtype=np.float64)
+        noise = np.ascontiguousarray(noise, dtype=np.float64)
+        R, nh = H.shape
+        lik, grad = np.empty(R), np.empty((R, nh + (1 if optimize_noise else 0)))
+        info = np.empty(R, dtype=np.int32)
+        self._lib.check(self.lib.lb_lml_grad_batch(self.h, kid, R, nh, H.ctypes.data, noise.ctypes.data, int(optimize_noise),
+                                                   lik.ctypes.data, grad.ctypes.data, info.ctypes.data), "lb_lml_grad_batch")
+        return lik, grad, info
 
 def factor_outputs(h: Handle, case: ExactCase, X) -> dict:
     """L, alpha and K^-1 of an exact case on handle h (data, kernel, factor, alpha)."""

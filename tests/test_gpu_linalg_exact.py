@@ -61,6 +61,16 @@ def _check_factor(h, case, tag=""):
     return L, alpha, Ki
 
 
+def test_lambda_gradient_shapes_are_covered():
+    """The Lambda entries of the likelihood gradient (dk_build over 1024 column slices of wdot) are checked against the
+    reference at N > 1024 (a second pass of the slice loop) on at least two shapes, and with k = 4 (LB_MAX_LAMBDA)."""
+    lam = [(N, E.exact_objective(i, N)[2]) for i, (N, _, _) in enumerate(EXACT) if E.exact_objective(i, N)[2] > 0]
+    checked = [(N, k) for N, k in lam if N <= 2200 or N == 4223]
+    assert sum(N > 1024 for N, _ in checked) >= 2, checked
+    assert any(k == 4 for _, k in checked), checked
+    assert {k for _, k in lam} == {1, 2, 4}, lam
+
+
 @pytest.mark.parametrize("N,P,seed", EXACT, ids=[f"N{n}_P{p}" for n, p, _ in EXACT])
 def test_exact_factor_solve_inverse_logdet_grad(handle, N, P, seed):
     h = handle
@@ -68,12 +78,10 @@ def test_exact_factor_solve_inverse_logdet_grad(handle, N, P, seed):
     assert case.ref()["kappa"] < 16.0
     rng = np.random.default_rng(seed + 1)
     i = EXACT.index((N, P, seed))
-    kid = E.KERNELS[i % 4]
-    D = 20 if (kid == 0 and N == 1151) else 2  # two 16-dimension passes of the gradient kernel
+    kid, D, klam, optimize_noise = E.exact_objective(i, N)  # SE-ARD with k Lambda columns: lb_launch_grad_lambda
     X = rng.uniform(0.0, 1.0, size=(N, D))
-    p = np.concatenate([rng.uniform(0.3, 0.8, D), [0.1]]) if D == 20 else E.kernel_params(kid, D, rng)
+    p = E.exact_objective_params(kid, D, klam, rng)
     noise = 0.01
-    optimize_noise = bool((i // 4) % 2)
     h.set_data(X, case.Y)
     h.set_kernel(kid, p, noise)
     assert h.factor(case.K) == 0
@@ -86,9 +94,11 @@ def test_exact_factor_solve_inverse_logdet_grad(handle, N, P, seed):
         gr, absum, fro = E.grad_reference(kid, p, X, case.A0, case.ref()["kinv"], noise, optimize_noise)
         bg = E.bound_grad(case, kid, p, X, absum, fro, E.bound_alpha(case), E.bound_kinv(case))
         eg = np.abs(g - gr)
-        print(f"  grad {E.KERNEL_NAMES[kid]} D={D} noise={optimize_noise} ratio={np.max(eg / bg):.2e}")
+        print(f"  grad {E.KERNEL_NAMES[kid]} D={D} k={klam} noise={optimize_noise} ratio={np.max(eg / bg):.2e}")
         assert np.all(eg <= bg), (g, gr, bg)
         _ratio("grad", eg, bg)
+        if klam:
+            _ratio("grad_lambda", eg[D:D * (1 + klam)], bg[D:D * (1 + klam)])
 
     # log det: with alpha = 0, loglik = -0.5 log det K - 0.5 N log(2 pi)
     h.refit_alpha(np.zeros((N, P)))

@@ -235,3 +235,174 @@ def test_acq_bounds_hold_for_long_double():
         rv_, rg_ = float(np.max(np.abs(v - rv).astype(np.float64) / bv)), float(np.max(np.abs(g - rg).astype(np.float64) / bg))
         print(f"acq={acq_id} {params} ratio value={rv_:.2e} grad={rg_:.2e}")
         assert rv_ <= 1.0 and rg_ <= 1.0
+
+
+# ---- SE-ARD Lambda columns, LOO-CV, K^-1 obs_mean and the batched likelihood ------------------------------------------
+@pytest.mark.parametrize("klam", [1, 2, 4])
+@pytest.mark.parametrize("D", [1, 3, 20])
+def test_lambda_derivatives_match_oracle(oracle_mod, D, klam):
+    """SE-ARD with klam Lambda columns (A(i, j) at (j + 1) D + i): kernel_matrix against the oracle's K, and the likelihood
+    gradient built from every kernel_grads entry against OracleGP.grad, which sums the functor's own gradient
+    (squared_exp_ard.hpp:119-122) over the pairs."""
+    O = oracle_mod
+    rng = np.random.default_rng(700 + 10 * D + klam)
+    for N, P in [(7, 1), (60, 2)]:
+        p = E.kernel_params(0, D, rng, klam)
+        assert p.size == D * (1 + klam) + 1
+        X = rng.uniform(0.0, 1.0, size=(N, D))
+        Y = rng.normal(size=(N, P))
+        og = O.OracleGP()
+        og.set_data(X, Y)
+        og.set_kernel(0, p, 0.01)
+        assert og.fit() == -1
+        K = E.kernel_matrix(0, p, X, X)
+        K[np.diag_indices(N)] += 0.01 + E.JITTER
+        ev = E.kernel_eval_err(0, p, 1.0, D)
+        assert np.abs(K - og.get(0)).max() <= 2 * ev + 4 * E.U
+        G = list(E.kernel_grads(0, p, X, X))
+        assert len(G) == p.size
+        for q in range(D, p.size - 2):  # neighbouring Lambda slots differ (a slot written one entry off would show)
+            assert np.abs(G[q] - G[q + 1]).max() > 2 * ev, q
+        alpha, kinv = og.get(2), og.get(3)
+        g, absum, _ = E.grad_reference(0, p, X, alpha, kinv, 0.01, True)
+        go = og.grad(True)
+        assert np.all(np.abs(g - go) <= 1e-12 * (absum + np.abs(go).max())), (N, g, go)
+
+
+@pytest.mark.parametrize("kid,klam", [(0, 0), (0, 2), (1, 0), (2, 0), (3, 0)])
+def test_loo_formula_matches_oracle_gp(oracle_mod, kid, klam):
+    """loo_reference (value and gradient, noise optimised) against OracleGP.loo_cv / loo_grad on kernel-matrix problems."""
+    O = oracle_mod
+    rng = np.random.default_rng(800 + 10 * kid + klam)
+    for N, D, P in [(5, 1, 1), (40, 3, 2), (130, 3, 1)]:
+        X = rng.uniform(0.0, 1.0, size=(N, D))
+        Y = rng.normal(size=(N, P))
+        p = E.kernel_params(kid, D, rng, klam)
+        og = O.OracleGP()
+        og.set_data(X, Y)
+        og.set_kernel(kid, p, 0.01)
+        assert og.fit() == -1
+        v, g = E.loo_reference(kid, p, X, og.get(2), og.get(3), 0.01, True)
+        vo, go = og.loo_cv(), og.loo_grad(True)
+        assert abs(v - vo) <= 1e-10 * abs(vo), (N, v, vo)
+        assert np.all(np.abs(g - go) <= 1e-9 * np.abs(go).max()), (N, g, go)
+
+
+def _inv_lower_ld(L):
+    """L^-1 of a lower-triangular matrix by substitution in long double."""
+    n = L.shape[0]
+    Lq = L.astype(np.longdouble)
+    Li = np.zeros((n, n), dtype=np.longdouble)
+    for i in range(n):
+        Li[i, i] = 1 / Lq[i, i]
+        Li[i, :i] = -(Lq[i, :i] @ Li[:i, :i]) / Lq[i, i]
+    return Li
+
+
+def _tiles(N):
+    return [slice(t, min(t + 128, N)) for t in range(0, N, 128)]
+
+
+LOO_CASES = [(127, 1, 0, 2, True), (130, 3, 1, 0, False), (256, 5, 0, 4, True), (300, 2, 3, 0, True)]
+
+
+@pytest.mark.parametrize("N,P,kid,klam,on", LOO_CASES)
+def test_loo_and_kinv_obs_bounds_hold_for_long_double(N, P, kid, klam, on):
+    """The fp64 LOO value and gradient (LAPACK K^-1 of the exact factor, alpha = A0) and K^-1 Y stay inside bound_loo,
+    bound_loo_grad and bound_kinv_obs against the same formulas in long double.  Scaling the value's rows of any one
+    128-row tile by 1 + 2^-30 leaves its bound; dropping any one tile's contribution to K^-1 Y (the K^-1 bound grows as N^2 u
+    and is of the order of a 2^-30 slip there from N = 256 on), or its partials of Z alpha and diag(Z K^-1) from the gradient (its bound carries the evaluation error of dK, kernel_eval_err's
+    worst case over the whole input box, which is far above the rounding of the products)."""
+    c = E.ExactCase(N, P, 1200 + N)
+    rng = np.random.default_rng(N)
+    X = rng.uniform(0.0, 1.0, size=(N, 2))
+    p = E.kernel_params(kid, 2, rng, klam)
+    noise = 0.01
+    kinv = c.ref()["kinv"]
+    ba, bk = E.bound_alpha(c), E.bound_kinv(c)
+    v64, g64 = E.loo_reference(kid, p, X, c.A0, kinv, noise, on)
+    Li = _inv_lower_ld(c.L0)
+    kld = Li.T @ Li
+    ld = np.longdouble
+    vld, gld = E.loo_reference(kid, p.astype(ld), X.astype(ld), c.A0.astype(ld), kld, ld(noise), on)
+    bv, bg = E.bound_loo(c, ba, bk), E.bound_loo_grad(c, kid, p, X, noise, on, ba, bk)
+    rv, rg = float(abs(v64 - vld) / bv), np.abs(g64 - gld).astype(np.float64) / bg
+    ko64 = kinv @ c.Y
+    bko = E.bound_kinv_obs(c, bk)
+    rko = np.linalg.norm(ko64 - c.A0, axis=0) / bko
+    print(f"N={N} kid={kid} klam={klam} ratios loo={rv:.2e} loo_grad={rg.max():.2e} kinv_obs={rko.max():.2e}")
+    assert rv <= 1.0 and np.all(rg <= 1.0) and np.all(rko <= 1.0)
+    # one tile's contribution scaled by 1 + 2^-30 (value) or dropped (K^-1 Y, gradient) exceeds the bound, for every tile
+    eps = 2.0 ** -30
+    ic = 1.0 / np.diag(kinv)
+    rows = -c.A0 * c.A0 * ic[:, None] / 2 - np.log(ic)[:, None] / 2 - math.log(2 * math.pi) / 2
+    dks = E.dk_matrices(kid, p, X, noise, on)
+    for t in _tiles(N):
+        assert abs(eps * rows[t].sum()) > bv, ("value", t)
+        assert np.all(np.linalg.norm(kinv[:, t] @ c.Y[t], axis=0) > bko), ("kinv_obs", t)
+        gt = np.array([E.loo_terms(c.A0, kinv, dk, t)[3].sum() for dk in dks])
+        assert np.all(np.abs(gt) > bg), ("grad", t, np.abs(gt) / bg)
+
+
+def _chol_ld(K):
+    n = K.shape[0]
+    L = np.zeros_like(K)
+    for j in range(n):
+        d = K[j, j] - L[j, :j] @ L[j, :j]
+        L[j, j] = np.sqrt(d)
+        L[j + 1:, j] = (K[j + 1:, j] - L[j + 1:, :j] @ L[j, :j]) / L[j, j]
+    return L
+
+
+def lml_ld(case: E.LmlCase):
+    """The likelihood and gradient of an LmlCase in long double throughout (kernel, Cholesky, solves, inverse, gradient)."""
+    ld = np.longdouble
+    X, p, Y = case.X.astype(ld), case.p.astype(ld), case.Y.astype(ld)
+    n = X.shape[0]
+    K = E.kernel_matrix(case.kid, p, X, X)
+    K[np.diag_indices(n)] += ld(case.noise) + ld(E.JITTER)
+    L = _chol_ld(K)
+    Li = _inv_lower_ld(L)
+    kinv = Li.T @ Li
+    alpha = kinv @ Y
+    lik = -(Y * alpha).sum() / 2 - np.log(np.diag(L)).sum() - n * np.log(2 * ld(np.pi)) / 2
+    W = alpha @ alpha.T - kinv
+    g = [(W * dk).sum() / 2 for dk in E.dk_matrices(case.kid, p, X, ld(case.noise), case.on)]
+    return lik, np.array(g)
+
+
+GCH = 8  # lml_batch.cu: SE-ARD ell / Lambda gradient entries per sweep
+
+
+@pytest.mark.parametrize("kid,N,D,klam,P,on", [(0, 33, 3, 2, 2, True), (0, 128, 4, 4, 1, False), (1, 200, 3, 0, 2, True),
+                                               (3, 127, 5, 0, 1, True)])
+def test_lml_bounds_hold_for_long_double(kid, N, D, klam, P, on):
+    """LmlCase's fp64 likelihood and gradient stay inside its bound against long double, kappa_2(K) <= 1e4; for SE-ARD,
+    swapping two neighbouring ell / Lambda entries (across the first GCH sweep boundary and the ell / Lambda boundary) or
+    dropping the last sweep's entries exceeds twice the bound (the device-against-reference bar)."""
+    rng = np.random.default_rng(1300 + N)
+    X = rng.uniform(0.0, 1.0, size=(N, D))
+    Y = rng.normal(size=(N, P))
+    p = E.grad_params(kid, D, klam, rng)
+    noise = lml_noise(p, N)
+    c = E.LmlCase(kid, p, noise, X, Y, on)
+    assert c.kappa <= 1e4, c.kappa
+    bl, bg = c.bound()
+    lik, g = lml_ld(c)
+    rl, rg = float(abs(c.lik - lik) / bl), np.abs(c.grad - g).astype(np.float64) / bg
+    print(f"kid={kid} N={N} kappa={c.kappa:.1f} ratios lik={rl:.2e} grad={rg.max():.2e}")
+    assert rl <= 1.0 and np.all(rg <= 1.0)
+    if kid == 0:
+        nent = D * (1 + klam)
+        for a_, b_ in {(D - 1, D), (GCH - 1, GCH)}:
+            if b_ < nent:
+                gs = c.grad.copy()
+                gs[[a_, b_]] = gs[[b_, a_]]
+                assert np.any(np.abs(gs - c.grad) > 2 * bg), ("swap", a_, b_)
+        last = (nent - 1) // GCH * GCH
+        assert np.any(np.abs(c.grad[last:nent]) > 2 * bg[last:nent]), "drop the last sweep"
+
+
+def lml_noise(p, N):
+    """A noise that keeps kappa_2(K) <= 1e4: lambda_max <= N sf2 + noise, lambda_min >= noise."""
+    return 0.01 + N * math.exp(2 * p[-1]) / 8000.0
