@@ -1,5 +1,5 @@
-// limbo_b200/csrc/potrf.cu — blocked right-looking Cholesky, trailing update on
-// fp64 tensor cores (DMMA).
+// limbo_b200/csrc/potrf.cu — blocked Cholesky with deferred trailing updates, trailing
+// update on fp64 tensor cores (DMMA).
 //
 // Replaces `_matrixL = Eigen::LLT<Eigen::MatrixXd>(_kernel).matrixL()`
 // (model/gp.hpp:565).  Per 128-column panel k:
@@ -8,7 +8,8 @@
 //                         form its inverse (kept in invD for every later
 //                         triangular solve);
 //   2. trsm_panel_kernel: L[i,k] = A[i,k] * inv(L[k,k])^T   (DMMA GEMM)
-//   3. syrk_kernel      : A[i,j] -= L[i,k] * L[j,k]^T, k < j <= i (DMMA GEMM)
+//   3. syrk_kernel      : A[i,j] -= L[i,k] * L[j,k]^T, k < j <= i (DMMA GEMM), several
+//                         panels per pass (potrf_plan below decides which and when)
 // A non-positive pivot is reported LAPACK-style through info (the reference
 // never checks Eigen's info(), SURVEY.md §5).
 #include "gemm.cuh"
@@ -248,29 +249,35 @@ trsm_panel_kernel(double* __restrict__ L, int64_t ld, int k, const double* __res
     lbg::store_acc<C>(acc, A, ld);
 }
 
-// Trailing update with the panel block columns [kb, kb + kd):
-//   A[i,j] -= L[i, kb:kb+kd] L[j, kb:kb+kd]^T   for j in [j0, j0 + nc), j <= i < T
-// (kd = 1: one 128-column panel, K = 128; kd = 2: two panels at once, K = 256 —
-// half the C traffic and half the tile prologues per flop).  C is preloaded into
-// the accumulators so its latency overlaps the operand pipeline's prologue.
-// Cfg = CfgDual: 128 x 64 tiles, 128 threads, two CTAs per SM (one CTA's C-tile prologue / store epilogue
-// hides under the other's DMMA stream).
+// The block columns of one trailing-update pass: column j0 + c takes the panel block columns [kb[c], kend), c < nc.
+constexpr int SYRK_MAX_COLS = 64;
+struct SyrkCols {
+    int j0, nc, kend;
+    int kb[SYRK_MAX_COLS];
+};
+
+// Trailing update of block column j = j0 + c with its panel block columns [kb[c], kend):
+//   A[i,j] -= L[i, kb[c]:kend] L[j, kb[c]:kend]^T   for c < nc, j <= i < T
+// C is preloaded into the accumulators so its latency overlaps the operand pipeline's prologue.  The grid walks the columns
+// from the right: the planner never gives a column a later kb than the columns left of it, so the longest-K tiles start first
+// and the short ones fill the last wave.  Cfg = CfgDual: 128 x 64 tiles, 128 threads, two CTAs per SM (one CTA's C-tile
+// prologue / store epilogue hides under the other's DMMA stream).
 template <typename C>
 __global__ void __launch_bounds__(C::THREADS, C::CTAS_PER_SM)
-syrk_kernel(double* __restrict__ L, int64_t ld, int kb, int kd, int j0, int nc, int T)
+syrk_kernel(double* __restrict__ L, int64_t ld, const __grid_constant__ SyrkCols cols, int T)
 {
     extern __shared__ __align__(16) double smem[];
     constexpr int SPLIT = LB_TILE / C::BN; // column sub-tiles per 128-block
-    int idx = blockIdx.x / SPLIT, c = 0;
+    int idx = blockIdx.x / SPLIT, c = cols.nc - 1;
     const int h = blockIdx.x - idx * SPLIT;
-    while (c < nc && idx >= T - j0 - c) { idx -= T - j0 - c; ++c; }
-    const int j = j0 + c, i = j + idx;
+    while (c > 0 && idx >= T - cols.j0 - c) { idx -= T - cols.j0 - c; --c; }
+    const int j = cols.j0 + c, i = j + idx, kb = cols.kb[c];
     const double* A = L + (int64_t)i * LB_TILE + (int64_t)kb * LB_TILE * ld;
     const double* B = L + (int64_t)j * LB_TILE + h * C::BN + (int64_t)kb * LB_TILE * ld;
     double* Cg = L + (int64_t)i * LB_TILE + ((int64_t)j * LB_TILE + h * C::BN) * ld;
     lbg::Acc<C> acc;
     lbg::load_acc<C>(acc, Cg, ld);
-    lbg::mainloop<C, false, false, true>(acc, A, ld, B, ld, kd * LB_TILE, smem);
+    lbg::mainloop<C, false, false, true>(acc, A, ld, B, ld, (cols.kend - kb) * LB_TILE, smem);
     lbg::store_acc<C>(acc, Cg, ld);
 }
 
@@ -322,10 +329,17 @@ static inline int syrk_tiles(int T, int j0, int nc)
     return n;
 }
 
-// syrk_kernel over the block columns [j0, j0 + nc) with the panel block columns [kb, kb + kd)
+static void launch_syrk(cudaStream_t st, double* L, int64_t ld, const SyrkCols& cols, int T)
+{
+    syrk_kernel<SyrkCfg><<<syrk_tiles(T, cols.j0, cols.nc) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, st>>>(L, ld, cols, T);
+}
+
+// syrk_kernel over the block columns [j0, j0 + nc), each with the panel block columns [kb, kb + kd)
 static void launch_syrk(cudaStream_t st, double* L, int64_t ld, int kb, int kd, int j0, int nc, int T)
 {
-    syrk_kernel<SyrkCfg><<<syrk_tiles(T, j0, nc) * SYRK_SPLIT, SyrkCfg::THREADS, SyrkCfg::PIPE_BYTES, st>>>(L, ld, kb, kd, j0, nc, T);
+    SyrkCols cols{j0, nc, kb + kd, {}};
+    for (int c = 0; c < nc; ++c) cols.kb[c] = kb;
+    launch_syrk(st, L, ld, cols, T);
 }
 
 // Pair panel (k, k + 1): potf2(k) trsm(k) syrk[k -> col k+1] (K = 128) potf2(k+1), and trsm(k+1) when k + 2 < T.  L, invD and
@@ -361,17 +375,80 @@ static int launch_pair_panel(lb_gp* h, cudaStream_t st, double* L, double* invD,
     return LB_OK;
 }
 
-// Right-looking factorisation with look-ahead, panels in QUADS of 128-column block columns (two pairs):
+// Blocked factorisation with look-ahead, panels in QUADS of four 128-column block columns (two pairs), and trailing updates
+// deferred into long-K passes.  applied[j] counts the panels already subtracted from block column j; every update of column j
+// takes the panels [applied[j], kend) in one pass, so each tile's accumulator runs through the same ascending sequence of DMMAs
+// whatever the passes are (a store and a reload in between do not round), and the factor is bit-identical to the right-looking
+// and the pair-wise distributed factorisations (tests/test_gpu_dist_fit.py, tests/test_gpu_multirank.py).  Per quad q (k = 4q):
 //   side stream : pair(k)  = potf2(k) trsm(k) syrk[k -> col k+1] potf2(k+1) trsm(k+1)
-//                 a_in     = K=256 update of block columns k+2, k+3 with pair(k)            (inside the quad)
+//                 K = 256 update of block columns k+2, k+3 with pair(k)                    (inside the quad)
 //                 pair(k+2)
-//   main stream : a(q)     = K=512 update of the NEXT quad's four block columns with all four panels of this quad
-//                 b(q)     = K=512 update of everything right of them
-// quad(q+1) only needs a(q), so the latency-bound panel chain runs under b(q).  With K=512 every trailing tile is loaded /
-// stored half as often per flop as with K=256 (the C-tile prologue and store epilogue are what keeps a short-K GEMM below the
-// long-K kernels of this library: 0.76-0.84 against 0.90-0.92).  A tile's accumulator runs through the same sequence of DMMAs
-// as with two K=256 passes (the store / load in between does not round), so the factor is bit-identical to the pair-wise
-// distributed factorisation below (tests/test_gpu_dist_fit.py, tests/test_gpu_multirank.py).
+//   main stream : a(q)     = K = 512 update of the next quad's four block columns with this quad's panels
+//                 LL(q)    = quad q+2's block columns with every panel not yet applied to them (up to k+4), then further
+//                            columns to the right, each with its own [applied, k+4), until the pass holds POTRF_FILL_WAVES
+//                            waves of CTAs
+// quad q+1's chain only needs a(q), so it runs under LL(q).  A column is loaded and stored once per pass instead of once per
+// quad, and most trailing flops run at K in the thousands.  The fill bound keeps the late passes, whose deferred columns hold
+// few tiles of long K, from ending in a sliver wave (DESIGN.md §4.2).
+namespace {
+
+constexpr int POTRF_FILL_WAVES = 8;
+
+enum { PLAN_MAIN = 0, PLAN_SIDE = 1 };
+enum { POP_PAIR = 0, POP_UPDATE, POP_RECORD, POP_WAIT };
+
+struct PotrfOp {
+    int op;        // POP_*
+    int stream;    // PLAN_MAIN / PLAN_SIDE
+    int arg;       // POP_PAIR: first block column of the pair; POP_RECORD / POP_WAIT: index into lb_gp::ev
+    SyrkCols cols; // POP_UPDATE
+};
+
+// The factorisation of a T x T block matrix as one list of operations in issue order, for `sms` SMs.  Streams order their own
+// operations; POP_WAIT orders its stream behind the latest POP_RECORD of the same event issued before it.
+std::vector<PotrfOp> potrf_plan(int T, int sms)
+{
+    std::vector<PotrfOp> ops;
+    std::vector<int> applied(T > 0 ? T : 0, 0);
+    const int64_t fill = (int64_t)POTRF_FILL_WAVES * sms * SyrkCfg::CTAS_PER_SM;
+    auto sync = [&](int from, int to, int ev) {
+        ops.push_back({POP_RECORD, from, ev, {}});
+        ops.push_back({POP_WAIT, to, ev, {}});
+    };
+    auto pair = [&](int k) {
+        ops.push_back({POP_PAIR, PLAN_SIDE, k, {}});
+        if (k + 1 < T) applied[k + 1] = k + 1;
+    };
+    // the columns [j0, j1) up to panel kend, then more columns while the pass is short of `want` CTAs
+    auto update = [&](int st, int j0, int j1, int kend, int64_t want) {
+        PotrfOp o{POP_UPDATE, st, 0, {j0, 0, kend, {}}};
+        int64_t ctas = 0;
+        for (int j = j0; j < T && o.cols.nc < SYRK_MAX_COLS && (j < j1 || ctas < want); ++j) {
+            o.cols.kb[o.cols.nc++] = applied[j];
+            applied[j] = kend;
+            ctas += (int64_t)(T - j) * SYRK_SPLIT;
+        }
+        if (o.cols.nc > 0) ops.push_back(o);
+    };
+    sync(PLAN_MAIN, PLAN_SIDE, 0); // inputs (K) ready
+    for (int k = 0, q = 0; k < T; k += 4, ++q) {
+        pair(k);
+        if (k + 2 < T) {
+            update(PLAN_SIDE, k + 2, k + 4, k + 2, 0);
+            pair(k + 2);
+        }
+        if (k + 4 >= T) break;
+        sync(PLAN_SIDE, PLAN_MAIN, 1 + (q & 1));
+        update(PLAN_MAIN, k + 4, k + 8, k + 4, 0); // a(q)
+        sync(PLAN_MAIN, PLAN_SIDE, 3 + (q & 1));
+        update(PLAN_MAIN, k + 8, k + 12, k + 4, fill); // LL(q)
+    }
+    sync(PLAN_SIDE, PLAN_MAIN, 5); // join
+    return ops;
+}
+
+} // namespace
+
 int lb_launch_potrf(lb_gp* h)
 {
     int rc = set_attrs();
@@ -379,55 +456,48 @@ int lb_launch_potrf(lb_gp* h)
     const int T = (int)(h->Np / LB_TILE);
     const int64_t ld = h->Np;
     cudaStream_t main = h->stream, side = h->side ? h->side : h->stream;
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     LB_CUDA(cudaMemsetAsync(h->dInfo.get(), 0, 2 * sizeof(int), main));
-    if (side != main) {
-        LB_CUDA(cudaEventRecord(h->ev[0], main)); // inputs (K) ready
-        LB_CUDA(cudaStreamWaitEvent(side, h->ev[0], 0));
-    }
-    int q = 0;
-    for (int k = 0; k < T; k += 4, ++q) {
-        // ---- quad(q) on the side stream ----
-        if ((rc = launch_pair_panel(h, side, h->dL, h->dInvD, h->dInfo.get(), ld, k, T))) return rc;
-        if (k + 2 < T) {
-            const int nc2 = (T - (k + 2) < 2) ? (T - (k + 2)) : 2;
-            {
-                LbProfScope ps(h, side, LB_PC_SYRK_COL);
-                launch_syrk(side, h->dL, ld, k, 2, k + 2, nc2, T);
-            }
+    for (const PotrfOp& o : potrf_plan(T, sms)) {
+        cudaStream_t st = o.stream == PLAN_SIDE ? side : main;
+        switch (o.op) {
+        case POP_PAIR:
+            if ((rc = launch_pair_panel(h, st, h->dL, h->dInvD, h->dInfo.get(), ld, o.arg, T))) return rc;
+            break;
+        case POP_UPDATE: {
+            LbProfScope ps(h, st, o.stream == PLAN_SIDE ? LB_PC_SYRK_COL : LB_PC_SYRK);
+            launch_syrk(st, h->dL, ld, o.cols, T);
             h->launches++;
-            if ((rc = launch_pair_panel(h, side, h->dL, h->dInvD, h->dInfo.get(), ld, k + 2, T))) return rc;
+            break;
         }
-        if (k + 4 >= T) break;
-        if (side != main) {
-            LB_CUDA(cudaEventRecord(h->ev[1 + (q & 1)], side));
-            LB_CUDA(cudaStreamWaitEvent(main, h->ev[1 + (q & 1)], 0));
+        case POP_RECORD:
+            if (side != main) LB_CUDA(cudaEventRecord(h->ev[o.arg], st));
+            break;
+        case POP_WAIT:
+            if (side != main) LB_CUDA(cudaStreamWaitEvent(st, h->ev[o.arg], 0));
+            break;
         }
-        // ---- a(q): the next quad's block columns, K = 512 ----
-        const int j0 = k + 4;
-        const int nca = (T - j0 < 4) ? (T - j0) : 4;
-        {
-            LbProfScope ps(h, main, LB_PC_SYRK);
-            launch_syrk(main, h->dL, ld, k, 4, j0, nca, T);
-        }
-        h->launches++;
-        if (side != main) {
-            LB_CUDA(cudaEventRecord(h->ev[3 + (q & 1)], main));
-            LB_CUDA(cudaStreamWaitEvent(side, h->ev[3 + (q & 1)], 0));
-        }
-        // ---- b(q): the rest of the trailing matrix, K = 512 ----
-        const int ncb = T - j0 - nca;
-        if (ncb > 0) {
-            LbProfScope ps(h, main, LB_PC_SYRK);
-            launch_syrk(main, h->dL, ld, k, 4, j0 + nca, ncb, T);
-            h->launches++;
-        }
-    }
-    if (side != main) { // join
-        LB_CUDA(cudaEventRecord(h->ev[5], side));
-        LB_CUDA(cudaStreamWaitEvent(main, h->ev[5], 0));
     }
     LB_CUDA(cudaGetLastError());
     return LB_OK;
+}
+
+// The plan lb_launch_potrf walks, for host-side checks: one record of 6 + SYRK_MAX_COLS ints per operation, {op, stream, arg,
+// j0, nc, kend, kb[0 .. SYRK_MAX_COLS)}, at most `cap` records written.  Returns the number of operations.
+extern "C" int lb_debug_potrf_plan(int T, int sms, int* out, int cap)
+{
+    if (T < 1 || sms < 1) return LB_ERR_ARG;
+    const std::vector<PotrfOp> ops = potrf_plan(T, sms);
+    constexpr int W = 6 + SYRK_MAX_COLS;
+    for (int n = 0; n < (int)ops.size() && n < cap; ++n) {
+        const PotrfOp& o = ops[n];
+        int* r = out + (int64_t)n * W;
+        r[0] = o.op; r[1] = o.stream; r[2] = o.arg;
+        r[3] = o.cols.j0; r[4] = o.cols.nc; r[5] = o.cols.kend;
+        for (int c = 0; c < SYRK_MAX_COLS; ++c) r[6 + c] = o.cols.kb[c];
+    }
+    return (int)ops.size();
 }
 
 // =====================================================================================================================
