@@ -264,8 +264,8 @@ int lb_sparsify_dev(const lb_gp* h, int64_t N, int D, const double* dX_rowmajor,
     int64_t* n_kept, int64_t* dRemoved, double* dRemovedScore);
 
 /* experimental::model::SPGP (experimental/model/spgp.hpp): Snelson and Ghahramani's sparse GP with M pseudo-inputs, single
- * output, SE-ARD.  Same conventions as lb_gp; lb_spgp_query and lb_spgp_acq_argmax may be called from several threads, the other
- * calls need exclusive access.  w is the reference's parameter vector (HyperParams, spgp.hpp:94-101) of n_w = (M+1) D + 2
+ * output, SE-ARD.  Same conventions as lb_gp; lb_spgp_query, lb_spgp_acq_argmax, lb_spgp_query_grad and lb_spgp_acq_grad may be
+ * called from several threads, the other calls need exclusive access.  w is the reference's parameter vector (HyperParams, spgp.hpp:94-101) of n_w = (M+1) D + 2
  * entries: [xb (M x D, column-major), log b (D; b = inverse squared length scales), log c (signal variance), log sig (noise
  * variance)].  lb_spgp_lik and lb_spgp_compute return LB_ERR_ARG for M < 1, M > N, n_w != (M+1) D + 2 or a non-finite w, and
  * the 1-based index (> 0) of the first non-positive pivot of Q = K(xb, xb) + jitter I, or else of A = sig I + V V^T. */
@@ -286,6 +286,25 @@ int lb_spgp_query(const lb_spgp* s, int64_t Mq, const double* Xq_rowmajor, int o
 /* lb_acq_argmax over lb_spgp_query's mu and sigma^2 (ties to the lowest index). */
 int lb_spgp_acq_argmax(const lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* Xq_rowmajor, int optimized,
     const double* mean_at_q, double mean_const, double* acq_out, double* best_val, int64_t* best_idx);
+/* Candidate gradients for Mq candidates (row-major Mq x D), extending lb_spgp_query as lb_query_grad extends lb_query:
+ * mu_minus_mean and sigma2 are bit-identical to lb_spgp_query's on the same batch; dmu (Mq x D row-major) is the gradient of
+ * mu_minus_mean, dsigma2 (Mq x D) that of sigma2.  With b the inverse squared length scales, x~ = x o sqrt(b), k_m the kernel
+ * value at pseudo-input m and x~b_m = xb_m o sqrt(b) (k(x, x) = c does not depend on x):
+ *   grad mu = -sqrt(b) o sum_m b1_m k_m (x~ - x~b_m),  b1 = L^-T Lm^-T bet,
+ *   grad sigma2 = 2 sqrt(b) o sum_m u_m k_m (x~ - x~b_m),  u = L^-T (L^-1 k - sig Lm^-T Lm^-1 L^-1 k).
+ * optimized adds sig to sigma2 and nothing to its gradient.  Any output may be NULL.  LB_ERR_ARG for a NULL handle or Xq_rowmajor,
+ * Mq < 1 or a non-finite coordinate; LB_ERR_STATE before lb_spgp_compute.  May be called from several threads, as lb_spgp_query. */
+int lb_spgp_query_grad(const lb_spgp* s, int64_t Mq, const double* Xq_rowmajor, int optimized, double* mu_minus_mean, double* sigma2,
+    double* dmu, double* dsigma2);
+/* Acquisition value (Mq) and gradient (Mq x D row-major) with the FirstElem aggregator, extending lb_spgp_acq_argmax (same acq_id,
+ * acq_params, mean_at_q and mean_const; the values are bit-identical to its acq_out) with lb_acq_grad's formulas over
+ * lb_spgp_query_grad's gradients: UCB / GP_UCB grad = grad mu + params[0] grad sigma2 / (2 sqrt(sigma2)); EI grad = Phi(Z) grad mu +
+ * phi(Z) grad sigma with f_max and the jitter fixed, value and gradient 0 where sigma < 1e-10.  mean_grad_at_q: Mq x D gradient of
+ * mean(v)'s first component, added to grad mu, or NULL when the mean does not depend on v.  Either output may be NULL.  LB_ERR_ARG
+ * for a NULL handle, acq_params or Xq_rowmajor, Mq < 1, a non-finite coordinate or an unknown acq_id; LB_ERR_STATE before
+ * lb_spgp_compute.  May be called from several threads, as lb_spgp_query. */
+int lb_spgp_acq_grad(const lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* Xq_rowmajor, int optimized,
+    const double* mean_at_q, double mean_const, const double* mean_grad_at_q, double* acq_out, double* grad_out);
 /* kernels launched by this model so far */
 long long lb_spgp_launch_count(const lb_spgp* s);
 

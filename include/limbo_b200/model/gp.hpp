@@ -30,6 +30,7 @@
 #include <Eigen/Core>
 
 #include "../../limbo_b200.h"
+#include "mean_traits.hpp" // mean_is_input_free
 
 namespace limbo {
     namespace kernel {
@@ -37,12 +38,6 @@ namespace limbo {
         template <typename Params> struct MaternFiveHalves;
         template <typename Params> struct MaternThreeHalves;
         template <typename Params> struct Exp;
-    }
-    namespace mean {
-        template <typename Params> struct NullFunction;
-        template <typename Params> struct Constant;
-        template <typename Params> struct Data;
-        template <typename Params, typename MeanFunction> struct FunctionARD;
     }
 }
 
@@ -68,15 +63,6 @@ namespace limbo_b200 {
             static constexpr int id = LB_KERNEL_EXP;
             static void check() {}
         };
-
-        // Means whose value does not depend on the input: the candidate gradients (acq_grad, query_grad) add no mean term for them.
-        // FunctionARD is an affine map of its inner mean's value (mean/function_ard.hpp:88-92).  Other means have no input
-        // gradient here, and requesting one does not compile.
-        template <typename M> struct mean_is_input_free : std::false_type {};
-        template <typename P> struct mean_is_input_free<limbo::mean::NullFunction<P>> : std::true_type {};
-        template <typename P> struct mean_is_input_free<limbo::mean::Constant<P>> : std::true_type {};
-        template <typename P> struct mean_is_input_free<limbo::mean::Data<P>> : std::true_type {};
-        template <typename P, typename M> struct mean_is_input_free<limbo::mean::FunctionARD<P, M>> : mean_is_input_free<M> {};
 
         inline void lb_check(int rc, const char* where)
         {

@@ -23,6 +23,7 @@
 #include <limbo/tools/macros.hpp>
 
 #include "../../limbo_b200.h"
+#include "mean_traits.hpp" // mean_is_input_free
 
 #ifndef LIMBO_MODEL_SPGP_HPP // the reference's header defines the same defaults
 namespace limbo {
@@ -115,6 +116,78 @@ namespace limbo_b200 {
                 return {mu, s2};
             }
             Eigen::MatrixXd mu(const Eigen::MatrixXd& v) const { return predict(v).first; }
+
+            // ---- batched extensions with GP's signatures (not in the reference): what the batch-aware acquisitions of
+            // opt/batched_random.hpp call under BatchedRandom and BatchedGradient ----
+            // mu: M x dim_out (mean function included), sigma2: M
+            void query_batch(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu, Eigen::VectorXd& sigma2) const
+            {
+                Eigen::MatrixXd xt((Eigen::Index)vs.size(), (Eigen::Index)vs[0].size());
+                for (size_t i = 0; i < vs.size(); ++i)
+                    for (int d = 0; d < (int)vs[i].size(); ++d) xt((Eigen::Index)i, d) = vs[i](d);
+                auto r = predict(xt);
+                mu = r.first;
+                sigma2 = Eigen::VectorXd((Eigen::Index)vs.size());
+                for (size_t i = 0; i < vs.size(); ++i) sigma2((Eigen::Index)i) = r.second((Eigen::Index)i, 0);
+            }
+            // fused UCB / EI + argmax on the device with the FirstElem aggregator (lb_spgp_acq_argmax)
+            std::pair<double, long> acq_argmax(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs,
+                std::vector<double>* values = nullptr) const
+            {
+                std::vector<double> xq, mean0;
+                _stage(vs, xq, mean0);
+                double params[2] = {p0, p1}, best = 0;
+                int64_t idx = 0;
+                if (values) values->resize(vs.size());
+                _check(lb_spgp_acq_argmax(_h, acq_id, params, (int64_t)vs.size(), xq.data(), _optimized ? 1 : 0, mean0.data(), 0.0,
+                           values ? values->data() : nullptr, &best, &idx),
+                    "lb_spgp_acq_argmax");
+                return std::make_pair(best, (long)idx);
+            }
+            // UCB / EI values (M) and gradients (M x D) with the FirstElem aggregator in one device pass (lb_spgp_acq_grad)
+            void acq_grad(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs, Eigen::VectorXd& values,
+                Eigen::MatrixXd& grads) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "acq_grad: the mean function has no input gradient");
+                const long M = (long)vs.size();
+                const int D = (int)vs[0].size();
+                std::vector<double> xq, mean0, v((size_t)M), g((size_t)M * D);
+                _stage(vs, xq, mean0);
+                double params[2] = {p0, p1};
+                _check(lb_spgp_acq_grad(_h, acq_id, params, M, xq.data(), _optimized ? 1 : 0, mean0.data(), 0.0, nullptr, v.data(), g.data()),
+                    "lb_spgp_acq_grad");
+                values = Eigen::VectorXd((Eigen::Index)M);
+                grads = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                for (long i = 0; i < M; ++i) {
+                    values(i) = v[(size_t)i];
+                    for (int d = 0; d < D; ++d) grads(i, d) = g[(size_t)i * D + d];
+                }
+            }
+            // mu (M x dim_out, mean added), sigma^2 (M) and their candidate gradients dmu, dsigma2 (M x D) in one device pass
+            // (lb_spgp_query_grad)
+            void query_grad(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu, Eigen::VectorXd& sigma2, Eigen::MatrixXd& dmu,
+                Eigen::MatrixXd& dsigma2) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "query_grad: the mean function has no input gradient");
+                const long M = (long)vs.size();
+                const int D = (int)vs[0].size(), P = std::max(_dim_out, 1);
+                std::vector<double> xq, mean0, m((size_t)M), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
+                _stage(vs, xq, mean0);
+                _check(lb_spgp_query_grad(_h, M, xq.data(), _optimized ? 1 : 0, m.data(), s.data(), gm.data(), gs.data()), "lb_spgp_query_grad");
+                mu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)P);
+                sigma2 = Eigen::VectorXd((Eigen::Index)M);
+                dmu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                dsigma2 = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
+                for (long i = 0; i < M; ++i) {
+                    mu.row(i) = _mean_function(vs[(size_t)i], *this).transpose();
+                    mu(i, 0) += m[(size_t)i];
+                    sigma2(i) = s[(size_t)i];
+                    for (int d = 0; d < D; ++d) {
+                        dmu(i, d) = gm[(size_t)i * D + d];
+                        dsigma2(i, d) = gs[(size_t)i * D + d];
+                    }
+                }
+            }
             double sigma(const Eigen::VectorXd& v) const { return std::get<1>(query(v)); }
 
             int dim_in() const { assert(_dim_in != -1); return _dim_in; }
@@ -166,6 +239,17 @@ namespace limbo_b200 {
                 return m;
             }
             void _create() { _check(lb_spgp_create(&_h, 0), "lb_spgp_create"); }
+            // row-major candidates and the first component of the mean functor at each
+            void _stage(const std::vector<Eigen::VectorXd>& vs, std::vector<double>& xq, std::vector<double>& mean0) const
+            {
+                const size_t D = (size_t)vs[0].size();
+                xq.assign(vs.size() * D, 0.0);
+                mean0.assign(vs.size(), 0.0);
+                for (size_t i = 0; i < vs.size(); ++i) {
+                    for (size_t d = 0; d < D; ++d) xq[i * D + d] = vs[i]((Eigen::Index)d);
+                    mean0[i] = _mean_function(vs[i], *this)(0);
+                }
+            }
 
             void _init(const std::vector<Eigen::VectorXd>& samples, const std::vector<Eigen::VectorXd>& observations) // :353-379
             {

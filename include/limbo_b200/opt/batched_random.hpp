@@ -35,6 +35,7 @@
 #include <limbo/tools/macros.hpp>
 
 #include "../../limbo_b200.h"
+#include "../model/mean_traits.hpp"
 
 namespace limbo_b200 {
     namespace defaults {
@@ -48,6 +49,8 @@ namespace limbo_b200 {
     namespace model {
         template <typename Params, typename KernelFunction, typename MeanFunction, typename HyperParamsOptimizer>
         class GP;
+        template <typename Params, typename KernelFunction, typename MeanFunction, class HyperParamsOptimizer>
+        class SPGP;
     }
 
     namespace opt {
@@ -67,7 +70,7 @@ namespace limbo_b200 {
         }
 
         // The start points announced by BatchedGradient (opt/batched_gradient.hpp) for one call of f: a batch-aware UCB / EI over
-        // limbo_b200::model::GP files every point's value and gradient (one lb_acq_grad).
+        // limbo_b200::model::GP or model::SPGP files every point's value and gradient (one lb_acq_grad or lb_spgp_acq_grad).
         struct GradRequest {
             const std::vector<Eigen::VectorXd>* points = nullptr;
             bool answered = false;
@@ -194,6 +197,8 @@ namespace limbo_b200 {
             template <typename M> struct has_candidate_grad : std::false_type {};
             template <typename P, typename K, typename Mf, typename H>
             struct has_candidate_grad<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
+            template <typename P, typename K, typename Mf, typename H>
+            struct has_candidate_grad<model::SPGP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
         }
 
         // acqui::UCB (acqui/ucb.hpp:83-90), batch-aware

@@ -27,7 +27,7 @@ DECLARED_SYMBOLS = [
     "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_lml_grad_batch", "lb_lml_grad_batch_dev", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
     "lb_nb_samples", "lb_strerror", "lb_last_cuda_error", "lb_spgp_create", "lb_spgp_destroy", "lb_spgp_set_data", "lb_spgp_lik",
-    "lb_spgp_compute", "lb_spgp_query", "lb_spgp_acq_argmax", "lb_spgp_launch_count",
+    "lb_spgp_compute", "lb_spgp_query", "lb_spgp_acq_argmax", "lb_spgp_query_grad", "lb_spgp_acq_grad", "lb_spgp_launch_count",
 ]
 
 _lib = None
@@ -124,6 +124,8 @@ def load() -> C.CDLL:
         "lb_spgp_compute": ([p, i64, i64, dp, dbl], i32),
         "lb_spgp_query": ([p, i64, dp, i32, dp, dp], i32),
         "lb_spgp_acq_argmax": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
+        "lb_spgp_query_grad": ([p, i64, dp, i32, dp, dp, dp, dp], i32),
+        "lb_spgp_acq_grad": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
         "lb_spgp_launch_count": ([p], C.c_longlong),
         "lb_strerror": ([i32], C.c_char_p),
         "lb_last_cuda_error": ([], C.c_char_p),

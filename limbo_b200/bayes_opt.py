@@ -107,7 +107,7 @@ class BatchedGradientSearch:
             try:
                 f, g = grad_batch(x)
             except (AttributeError, NotImplementedError):
-                # a model without candidate gradients (model.SPGP, model.MultiGP) or a mean without an input gradient
+                # a model without candidate gradients (model.MultiGP) or a mean without an input gradient
                 if it == 0:
                     return x_best
                 raise

@@ -243,6 +243,28 @@ __device__ __forceinline__ double lb_acq_value(int acq_id, double mu, double s2,
     return lb_ei_factor(mu, s2, p0, p1);
 }
 
+// gradient of lb_acq_value with respect to the candidate from grad mu (the mean's input gradient included) and grad s2, with
+// f_max and the jitter held fixed (query_grad.cu, spgp.cu)
+//   acq_id 0: UCB / GP_UCB  grad mu + p0 grad s2 / (2 sqrt(s2)), 0 for the second term where s2 <= 0
+//   acq_id 1: EI            Phi(Z) grad mu + phi(Z) grad sigma; 0 below sigma = 1e-10 (ei.hpp:92-97)
+__device__ __forceinline__ double lb_acq_grad_value(int acq_id, double mu, double s2, double gmu, double gs2, double p0, double p1)
+{
+    double g;
+    if (acq_id == 0)
+        g = gmu + (s2 > 0.0 ? p0 * gs2 / (2.0 * sqrt(s2)) : 0.0);
+    else {
+        const double sigma = sqrt(s2);
+        g = 0.0;
+        if (!(sigma < 1e-10)) {
+            const double Z = (mu - p0 - p1) / sigma;
+            const double phi = exp(-0.5 * (Z * Z)) / sqrt(2.0 * M_PI);
+            const double Phi = 0.5 * erfc(-Z / sqrt(2.0));
+            g = Phi * gmu + phi * (gs2 / (2.0 * sigma));
+        }
+    }
+    return g;
+}
+
 // What the candidate-gradient pass (query_grad.cu) writes for one candidate chunk; every pointer may be NULL and starts at
 // the chunk's first candidate.
 struct LbGradOut {

@@ -154,19 +154,7 @@ query_grad_kernel(const double* __restrict__ Xs, int64_t Np, int64_t N, const do
     const double s = s2[m];
     const double mu = mu0[m * P] + (out.mean ? out.mean[m] : out.mean_const);
     if (out.mean_grad) gmu += out.mean_grad[o];
-    double g;
-    if (out.acq_id == 0) // UCB / GP_UCB: mu + p0 sqrt(s)
-        g = gmu + (s > 0.0 ? out.p0 * gs2 / (2.0 * sqrt(s)) : 0.0);
-    else { // EI: Phi(Z) grad mu + phi(Z) grad sigma, f_max and the jitter fixed; 0 below sigma = 1e-10 (ei.hpp:92-97)
-        const double sigma = sqrt(s);
-        g = 0.0;
-        if (!(sigma < 1e-10)) {
-            const double Z = (mu - out.p0 - out.p1) / sigma;
-            const double phi = exp(-0.5 * (Z * Z)) / sqrt(2.0 * M_PI);
-            const double Phi = 0.5 * erfc(-Z / sqrt(2.0));
-            g = Phi * gmu + phi * (gs2 / (2.0 * sigma));
-        }
-    }
+    const double g = lb_acq_grad_value(out.acq_id, mu, s, gmu, gs2, out.p0, out.p1);
     if (out.grad) out.grad[o] = g;
     if (r == 0 && out.acq) out.acq[m] = lb_acq_value(out.acq_id, mu, s, out.p0, out.p1);
 }

@@ -4,6 +4,7 @@
 //   _likelihood / _likelihood_wp  spgp.hpp:446-580  -> lb_spgp_lik
 //   _compute(false)               spgp.hpp:389-407  -> lb_spgp_compute
 //   _predict                      spgp.hpp:582-610  -> lb_spgp_query / lb_spgp_acq_argmax
+//   its candidate gradient        (not in the reference) -> lb_spgp_query_grad / lb_spgp_acq_grad
 //
 // Every M x M factor and inverse reuses the GP path: Q = K(xb, xb) + del I and A = sig I + V~ V~^T are factorised by
 // lb_launch_potrf on two internal lb_gp handles (their dL), L^-1 and Lm^-1 come from the recursive trtri of lml.cu and
@@ -17,6 +18,9 @@
 //   dfxb(:,i) = (G x~)(:,i) - x~b(:,i) o rowsum(G) + x~b(:,i) o rowsum(H) - (H x~b)(:,i)
 //   dfb(i)    = sum_n x~_ni (G^T x~b)_ni - x~_ni^2 colsum(G)_n
 // before the sqrt(b) rescalings of :546-552, so the gradient is one pass over three M x N matrices (spgp_pass_kernel).
+// The candidate gradient (DESIGN.md §4.14): with k_m = K*(m, q), lst = L^-1 k, lmst = Lm^-1 lst, k(x, x) = c constant,
+//   grad mu = -sqrt(b) o sum_m b1_m k_m (x~ - x~b_m),  grad sigma^2 = 2 sqrt(b) o sum_m u_m k_m (x~ - x~b_m),
+//   b1 = L^-T Lm^-T bet (once per lb_spgp_compute),  u = L^-T (lst - sig Lm^-T lmst) (two more triangular products per chunk).
 // Layout: M is padded to Mp = roundup(M, 128) and N to Np = roundup(N, 128); padded rows and columns of K are zero, so they
 // contribute nothing, and the padded parts of Q and A factor as the identity resp. sig I.
 #include "../../include/limbo_b200.h"
@@ -31,6 +35,8 @@ namespace {
 using GC = lbg::CfgDual;
 constexpr int PASS_DC = 8;    // input dimensions per sweep of spgp_pass_kernel
 constexpr int QCHUNK = 8192;  // candidates per prediction chunk
+constexpr int GRAD_THREADS = 128; // spgp_query_grad_kernel: one CTA per candidate
+constexpr int GRAD_DC = 8;        // input dimensions per sweep of spgp_query_grad_kernel
 
 // scalar slots of the per-evaluation reductions
 enum { S_LOGDIAG = 0, S_YY, S_BB, S_LOGEP, S_MUR, S_EPCBIG, S_BIGEP, S_TRQ, S_TRA, S_AQ, S_BQB, S_BB1, S_COUNT };
@@ -429,6 +435,79 @@ __global__ void spgp_pred_kernel(const double* __restrict__ sq1, const double* _
     if (i < n) s2[i] = c - sq1[i] + sig * sq2[i] + add;
 }
 
+// r = lst - sig t over n entries, in place over t
+__global__ void spgp_resid_kernel(const double* __restrict__ lst, double* __restrict__ t, int64_t n, double sig)
+{
+    const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+    if (i < n) t[i] = lst[i] - sig * t[i];
+}
+
+// Candidate gradients of one chunk, one CTA per candidate q: k = K*(:, q) (ld rows, zero below M), u = U(:, q), x~ = xqt(:, q).
+// Every thread takes the pseudo-inputs m = tid + 128 j in a fixed order; the sums are reduced over the lanes, then over the warps
+// in a fixed order, so a candidate's result is run-to-run identical and does not depend on the rest of the batch.  The difference
+// x~_d - x~b_md is formed per term (x~_d sum_m w_m - sum_m w_m x~b_md cancels for candidates far from the origin).  mu0 / s2: the
+// forward outputs of the chunk; out: the gradient outputs (D columns), its pointers from the chunk's first candidate.
+__global__ void __launch_bounds__(GRAD_THREADS)
+spgp_query_grad_kernel(const double* __restrict__ ks, const double* __restrict__ U, int64_t ld, int M, const double* __restrict__ b1,
+    const double* __restrict__ xbt, const double* __restrict__ xqt, int64_t ldq, const double* __restrict__ sb, int D,
+    const double* __restrict__ mu0, const double* __restrict__ s2, const LbGradOut out)
+{
+    __shared__ double sx[LB_MAX_D];
+    __shared__ double red[2][GRAD_THREADS / 32][GRAD_DC];
+    __shared__ double gsum[2][LB_MAX_D];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int64_t q = blockIdx.x;
+    for (int d = tid; d < D; d += GRAD_THREADS) sx[d] = xqt[(int64_t)d * ldq + q];
+    __syncthreads();
+    const double* kc = ks + q * ld;
+    const double* uc = U + q * ld;
+    for (int d0 = 0; d0 < D; d0 += GRAD_DC) {
+        double am[GRAD_DC], aw[GRAD_DC];
+#pragma unroll
+        for (int j = 0; j < GRAD_DC; ++j) am[j] = aw[j] = 0.0;
+        for (int m = tid; m < M; m += GRAD_THREADS) {
+            const double k = kc[m];
+            const double cb = k * b1[m], cu = k * uc[m];
+#pragma unroll
+            for (int j = 0; j < GRAD_DC; ++j)
+                if (d0 + j < D) {
+                    const double t = sx[d0 + j] - xbt[(int64_t)(d0 + j) * ld + m];
+                    am[j] = fma(cb, t, am[j]);
+                    aw[j] = fma(cu, t, aw[j]);
+                }
+        }
+#pragma unroll
+        for (int j = 0; j < GRAD_DC; ++j) {
+            const double a = lb_warp_sum(am[j]), b = lb_warp_sum(aw[j]);
+            if (lane == 0) {
+                red[0][warp][j] = a;
+                red[1][warp][j] = b;
+            }
+        }
+        __syncthreads();
+        if (tid < 2 * GRAD_DC) {
+            const int k = tid / GRAD_DC, j = tid % GRAD_DC;
+            double s = 0.0;
+            for (int w = 0; w < GRAD_THREADS / 32; ++w) s += red[k][w][j];
+            if (d0 + j < D) gsum[k][d0 + j] = s;
+        }
+        __syncthreads();
+    }
+    if (tid >= D) return;
+    const int d = tid;
+    const double gmu = -sb[d] * gsum[0][d], gs2 = 2.0 * sb[d] * gsum[1][d];
+    const int64_t o = q * D + d;
+    if (out.dmu) out.dmu[o] = gmu;
+    if (out.ds2) out.ds2[o] = gs2;
+    if (out.acq_id < 0) return;
+    const double s = s2[q];
+    const double mu = mu0[q] + (out.mean ? out.mean[q] : out.mean_const); // acq_kernel's sum, so the values are lb_spgp_acq_argmax's
+    const double gm = out.mean_grad ? gmu + out.mean_grad[o] : gmu;
+    const double g = lb_acq_grad_value(out.acq_id, mu, s, gm, gs2, out.p0, out.p1);
+    if (out.grad) out.grad[o] = g;
+    if (d == 0 && out.acq) out.acq[q] = lb_acq_value(out.acq_id, mu, s, out.p0, out.p1);
+}
+
 LbOncePerDevice g_attr_once;
 int set_attrs()
 {
@@ -471,9 +550,11 @@ struct lb_spgp {
     DevBuf<double> dWork; // split-K slices, row / block partials
     // prediction state (lb_spgp_compute)
     bool computed = false;
+    bool b1_ready = false; // Mv row 6 holds b1 = L^-T Lm^-T bet of the current factors (candidate gradients)
     double c = 0, sig = 0;
     // query workspace
     DevBuf<double> dQx, dQxt, dMu, dS2;
+    DevBuf<double> dGrad; // candidate gradients: the mean's input gradient, grad mu, grad sigma^2, the acquisition's, Mq x D each
     ArgmaxWs am; // acquisition values, means, argmax records
 };
 
@@ -726,20 +807,23 @@ int likelihood(lb_spgp* s, int M, const double* w, double jitter, double* f, dou
     return LB_OK;
 }
 
-// mu - mean and sigma^2 of Mq candidates (device row-major dQx) into s->dMu.get() / s->dS2.get(), in chunks of QCHUNK
-int predict(lb_spgp* s, int64_t Mq, int optimized)
+// mu - mean and sigma^2 of Mq candidates (device row-major dQx) into s->dMu.get() / s->dS2.get(), in chunks of QCHUNK; with grad,
+// also the candidate gradients of each chunk (b1 in Mv row 6, ensure_b1), whose outputs start at candidate 0.  The gradient
+// products take one more Mp x Cp block behind the forward workspace, whose layout they leave as it is.
+int predict(lb_spgp* s, int64_t Mq, int optimized, const LbGradOut* grad = nullptr)
 {
     const int D = s->D;
     const int64_t Mp = s->Mp;
     const int64_t Cp = round_up(std::min<int64_t>(Mq, QCHUNK), LB_TILE);
     int rc;
     if ((rc = set_attrs())) return rc;
-    if ((rc = s->dQxt.reserve(s->device, s->st, sizeof(double) * (3 * Mp * Cp + (size_t)D * Cp + 2 * Cp)))) return rc;
+    if ((rc = s->dQxt.reserve(s->device, s->st, sizeof(double) * ((grad ? 4 : 3) * Mp * Cp + (size_t)D * Cp + 2 * Cp)))) return rc;
     double* ks = s->dQxt.get() + (size_t)D * Cp;
     double* lst = ks + Mp * Cp;
     double* lmst = lst + Mp * Cp;
     double* sq1 = lmst + Mp * Cp;
     double* sq2 = sq1 + Cp;
+    double* tb = sq2 + Cp; // gradients: Lm^-T lmst, then lst - sig Lm^-T lmst
     for (int64_t q0 = 0; q0 < Mq; q0 += QCHUNK) {
         const int64_t nq = std::min<int64_t>(QCHUNK, Mq - q0), nqp = round_up(nq, LB_TILE);
         spgp_stage_kernel<<<dim3(nblocks(nqp, 256), D), 256, 0, s->st>>>(s->dQx.get() + q0 * D, nq, D, s->dSb.get(), s->dQxt.get(), nqp);
@@ -751,6 +835,23 @@ int predict(lb_spgp* s, int64_t Mq, int optimized)
         spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lst, Mp, nq, nullptr, nullptr, sq1);
         spgp_pred_kernel<<<nblocks(nq, 256), 256, 0, s->st>>>(sq1, sq2, nq, s->c, s->sig, optimized ? s->sig : 0.0, s->dS2.get() + q0);
         s->launches += 3;
+        LB_CUDA(cudaGetLastError());
+        if (!grad) continue;
+        // u = L^-T (lst - sig Lm^-T lmst) over lmst, which the forward reductions above have already read
+        if ((rc = gemm<true, true>(s, s->a->dLinv.get(), Mp, lmst, Mp, tb, Mp, Mp, nqp, Mp, 2, 0.0))) return rc;
+        spgp_resid_kernel<<<nblocks(Mp * nqp, 256), 256, 0, s->st>>>(lst, tb, Mp * nqp, s->sig);
+        s->launches++;
+        if ((rc = gemm<true, true>(s, s->q->dLinv.get(), Mp, tb, Mp, lmst, Mp, Mp, nqp, Mp, 2, 0.0))) return rc;
+        LbGradOut o = *grad;
+        o.mean = grad->mean ? grad->mean + q0 : nullptr;
+        o.mean_grad = grad->mean_grad ? grad->mean_grad + q0 * D : nullptr;
+        o.dmu = grad->dmu ? grad->dmu + q0 * D : nullptr;
+        o.ds2 = grad->ds2 ? grad->ds2 + q0 * D : nullptr;
+        o.acq = grad->acq ? grad->acq + q0 : nullptr;
+        o.grad = grad->grad ? grad->grad + q0 * D : nullptr;
+        spgp_query_grad_kernel<<<(unsigned)nq, GRAD_THREADS, 0, s->st>>>(ks, lmst, Mp, s->M, s->dMv.get() + 6 * Mp, s->dXbt.get(),
+            s->dQxt.get(), nqp, s->dSb.get(), D, s->dMu.get() + q0, s->dS2.get() + q0, o);
+        s->launches++;
         LB_CUDA(cudaGetLastError());
     }
     return LB_OK;
@@ -764,6 +865,65 @@ int ensure_query(lb_spgp* s, int64_t Mq, const double* Xq)
         if ((rc = b->reserve(s->device, s->st, mq))) return rc;
     if ((rc = s->dQx.reserve(s->device, s->st, mq * s->D)) || (rc = s->am.reserve(s->device, s->st, Mq))) return rc;
     LB_CUDA(cudaMemcpyAsync(s->dQx.get(), Xq, mq * s->D, cudaMemcpyHostToDevice, s->st));
+    return LB_OK;
+}
+
+// b1 = L^-T (Lm^-T bet) into Mv row 6 (row 5: Lm^-T bet), once per set of factors; the likelihood's own b1 (row 2) is not touched
+int ensure_b1(lb_spgp* s)
+{
+    if (s->b1_ready) return LB_OK;
+    const int64_t Mp = s->Mp;
+    double* t = s->dMv.get() + 5 * Mp;
+    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->a->dLinv.get(), Mp, Mp, s->dMv.get(), t, nullptr);
+    spgp_coldot_kernel<<<nblocks(Mp, 8), 256, 0, s->st>>>(s->q->dLinv.get(), Mp, Mp, t, s->dMv.get() + 6 * Mp, nullptr);
+    s->launches += 2;
+    LB_CUDA(cudaGetLastError());
+    s->b1_ready = true;
+    return LB_OK;
+}
+
+// lb_spgp_query_grad / lb_spgp_acq_grad (acq_id < 0: no acquisition): the arguments are checked by the callers
+int grad_common(lb_spgp* s, int64_t Mq, const double* Xq, int optimized, int acq_id, const double* acq_params, const double* mean_at_q,
+    double mean_const, const double* mean_grad, double* mu_out, double* s2_out, double* dmu_out, double* ds2_out, double* acq_out,
+    double* grad_out)
+{
+    const int D = s->D;
+    for (int64_t i = 0; i < Mq * D; ++i)
+        if (!std::isfinite(Xq[i])) return LB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (!s->computed) return LB_ERR_STATE;
+    LB_DEVICE(s);
+    int rc;
+    if ((rc = ensure_query(s, Mq, Xq))) return rc;
+    const size_t md = (size_t)Mq * D;
+    if ((rc = s->dGrad.reserve(s->device, s->st, sizeof(double) * 4 * md))) return rc;
+    double* g = s->dGrad.get();
+    LbGradOut out{};
+    out.acq_id = acq_id;
+    out.p0 = acq_id >= 0 ? acq_params[0] : 0.0;
+    out.p1 = acq_id == LB_ACQ_EI ? acq_params[1] : 0.0;
+    out.mean_const = mean_const;
+    if (mean_at_q) {
+        LB_CUDA(cudaMemcpyAsync(s->am.mean.get(), mean_at_q, sizeof(double) * Mq, cudaMemcpyHostToDevice, s->st));
+        out.mean = s->am.mean.get();
+    }
+    if (mean_grad) {
+        LB_CUDA(cudaMemcpyAsync(g, mean_grad, sizeof(double) * md, cudaMemcpyHostToDevice, s->st));
+        out.mean_grad = g;
+    }
+    out.dmu = dmu_out ? g + md : nullptr;
+    out.ds2 = ds2_out ? g + 2 * md : nullptr;
+    out.acq = acq_out ? s->am.vals.get() : nullptr;
+    out.grad = grad_out ? g + 3 * md : nullptr;
+    if ((rc = ensure_b1(s)) || (rc = predict(s, Mq, optimized, &out))) return rc;
+    const auto back = [&](double* dst, const double* src, size_t n) -> int {
+        if (dst) LB_CUDA(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToHost, s->st));
+        return LB_OK;
+    };
+    if ((rc = back(mu_out, s->dMu.get(), Mq)) || (rc = back(s2_out, s->dS2.get(), Mq)) || (rc = back(dmu_out, out.dmu, md))
+        || (rc = back(ds2_out, out.ds2, md)) || (rc = back(acq_out, out.acq, Mq)) || (rc = back(grad_out, out.grad, md)))
+        return rc;
+    LB_CUDA(cudaStreamSynchronize(s->st));
     return LB_OK;
 }
 
@@ -825,6 +985,7 @@ int lb_spgp_set_data(lb_spgp* s, int64_t N, int D, const double* X_rowmajor, con
     s->Np = Np;
     s->D = D;
     s->computed = false;
+    s->b1_ready = false;
     LB_CUDA(cudaMemcpyAsync(s->dX.get(), X_rowmajor, sizeof(double) * N * D, cudaMemcpyHostToDevice, s->st));
     LB_CUDA(cudaMemsetAsync(s->dY.get(), 0, sizeof(double) * Np, s->st));
     LB_CUDA(cudaMemcpyAsync(s->dY.get(), y_zm, sizeof(double) * N, cudaMemcpyHostToDevice, s->st));
@@ -841,6 +1002,7 @@ int lb_spgp_lik(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double jitt
     std::lock_guard<std::mutex> lk(s->mu);
     LB_DEVICE(s);
     s->computed = false; // the factors now belong to this w
+    s->b1_ready = false;
     return likelihood(s, (int)M, w, jitter, f, grad);
 }
 
@@ -853,6 +1015,7 @@ int lb_spgp_compute(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double 
     std::lock_guard<std::mutex> lk(s->mu);
     LB_DEVICE(s);
     s->computed = false;
+    s->b1_ready = false;
     double c, sig;
     if ((rc = forward(s, (int)M, w, jitter, &c, &sig))) return rc;
     if ((rc = read_info(s))) return rc;
@@ -901,6 +1064,25 @@ int lb_spgp_acq_argmax(const lb_spgp* sc, int acq_id, const double* acq_params, 
              am.vals.get(), am.blk_val.get(), am.blk_idx.get(), am.best_val.get(), am.best_idx.get(), &s->launches)))
         return rc;
     return am.read_best(s->st, best_val, best_idx, acq_out, Mq);
+}
+
+int lb_spgp_query_grad(const lb_spgp* sc, int64_t Mq, const double* Xq_rowmajor, int optimized, double* mu_minus_mean, double* sigma2,
+    double* dmu, double* dsigma2)
+{
+    lb_spgp* s = const_cast<lb_spgp*>(sc);
+    if (!s || Mq < 1 || !Xq_rowmajor) return LB_ERR_ARG;
+    return grad_common(s, Mq, Xq_rowmajor, optimized, -1, nullptr, nullptr, 0.0, nullptr, mu_minus_mean, sigma2, dmu, dsigma2, nullptr,
+        nullptr);
+}
+
+int lb_spgp_acq_grad(const lb_spgp* sc, int acq_id, const double* acq_params, int64_t Mq, const double* Xq_rowmajor, int optimized,
+    const double* mean_at_q, double mean_const, const double* mean_grad_at_q, double* acq_out, double* grad_out)
+{
+    lb_spgp* s = const_cast<lb_spgp*>(sc);
+    if (!s || !acq_params || Mq < 1 || !Xq_rowmajor) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
+    return grad_common(s, Mq, Xq_rowmajor, optimized, acq_id, acq_params, mean_at_q, mean_const, mean_grad_at_q, nullptr, nullptr,
+        nullptr, nullptr, acq_out, grad_out);
 }
 
 long long lb_spgp_launch_count(const lb_spgp* s) { return s ? s->launches + s->q->launches + s->a->launches : 0; }

@@ -218,6 +218,47 @@ class SPGP:
             return best.value, idx.value, vals
         return best.value, idx.value
 
+    def _first_mean(self, Xq):
+        """First output of the mean functor at every candidate, as (array, 0.0), or (None, constant) for a constant mean."""
+        if self._mean_function.is_constant():
+            return None, float(np.asarray(self._mean_function(Xq[0], self))[0])
+        return np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0]), 0.0
+
+    def query_grad_batch(self, Xq):
+        """mu (M x 1), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D) and grad sigma^2 (M x D), in
+        one device pass (lb_spgp_query_grad); mu and sigma^2 are query_batch's.  The mean's value and input gradient are added;
+        raises NotImplementedError for a mean without an input gradient (mean.BaseMean.grad_x)."""
+        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        M, D = Xq.shape
+        mgrad = self._mean_function.grad_x(Xq, self)
+        mean = np.array(self._mean_function.batch(Xq, self), dtype=np.float64)
+        if self.nb_samples() == 0:  # the prior (spgp.hpp:587-595): constant variance
+            return mean, np.full(M, self._kernel_function.sigma_sq()), np.array(mgrad[:, 0, :], dtype=np.float64), np.zeros((M, D))
+        mu, s2 = np.empty(M), np.empty(M)
+        dmu, ds2 = np.empty((M, D)), np.empty((M, D))
+        _lib.check(self._lib.lb_spgp_query_grad(self._h, M, _ptr(Xq), int(self._optimized), _ptr(mu), _ptr(s2), _ptr(dmu), _ptr(ds2)),
+                   "lb_spgp_query_grad")
+        mean[:, 0] += mu
+        dmu += mgrad[:, 0, :]
+        return mean, s2, dmu, ds2
+
+    def acq_grad_batch(self, acq_id: int, acq_params, Xq):
+        """Acquisition values (M) and gradients (M x D) of UCB / GP_UCB (acq_id 0) or EI (acq_id 1) with the FirstElem aggregator,
+        in one device pass (lb_spgp_acq_grad); parameters and values as acq_argmax_batch.  The mean's input gradient is added;
+        raises NotImplementedError for a mean without one."""
+        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        M, D = Xq.shape
+        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
+        if ap.size < 2:
+            ap = np.append(ap, 0.0)
+        mgrad = np.ascontiguousarray(self._mean_function.grad_x(Xq, self)[:, 0, :])
+        mean0, mconst = self._first_mean(Xq)
+        vals, grads = np.empty(M), np.empty((M, D))
+        _lib.check(self._lib.lb_spgp_acq_grad(self._h, acq_id, _ptr(ap), M, _ptr(Xq), int(self._optimized),
+                                              _ptr(mean0) if mean0 is not None else None, mconst,
+                                              _ptr(mgrad) if np.any(mgrad) else None, _ptr(vals), _ptr(grads)), "lb_spgp_acq_grad")
+        return vals, grads
+
     def launch_count(self) -> int:
         return int(self._lib.lb_spgp_launch_count(self._h))
 
