@@ -12,38 +12,43 @@ import subprocess
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "_ref", "libref_gp.so")
 REF_ROOT = os.environ.get("LIMBO_REFERENCE_SRC", os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference", "src"))
 REF_SRC = os.path.join(REF_ROOT, "limbo")
 
 
-def available() -> bool:
-    return os.path.exists(LIB_PATH) or os.path.isdir(REF_SRC)
+class RefLibrary:
+    """One library under oracle/_ref/, built by its oracle/ref_shim/Makefile target where the reference's sources are present
+    (make leaves it alone when it is up to date), loaded once, with the C signatures that declare(lib) sets."""
+
+    def __init__(self, name: str, declare):
+        self.name, self.path, self._declare, self._lib = name, os.path.join(HERE, "_ref", name), declare, None
+
+    def available(self) -> bool:
+        return os.path.exists(self.path) or os.path.isdir(REF_SRC)
+
+    def load(self):
+        if self._lib is None:
+            if os.path.isdir(REF_SRC):
+                subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "CXX=g++", f"REF={REF_ROOT}", self.name], check=True,
+                               capture_output=True)
+            lib = C.CDLL(self.path)
+            self._declare(lib)
+            self._lib = lib
+        return self._lib
 
 
-def build() -> str:
-    if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "CXX=g++", f"REF={REF_ROOT}"], check=True, capture_output=True)
-    return LIB_PATH
+def _declare(lib):
+    vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
+    lib.ref_gp_run.argtypes = [i, i, lg, i, i, vp, vp, d, vp, i, lg, lg, vp, i] + [vp] * 10
+    lib.ref_gp_run.restype = i
+    lib.ref_gp_loo.argtypes = [i, i, lg, i, i, vp, vp, d, vp, i, vp, vp]
+    lib.ref_gp_loo.restype = i
+    lib.ref_gp_mean_grad.argtypes = [i, lg, i, i, vp, vp, d, vp, i, vp, i, vp, vp, vp]
+    lib.ref_gp_mean_grad.restype = i
 
 
-_lib = None
-
-
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
-        _lib = C.CDLL(LIB_PATH)
-        vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
-        _lib.ref_gp_run.argtypes = [i, i, lg, i, i, vp, vp, d, vp, i, lg, lg, vp, i] + [vp] * 10
-        _lib.ref_gp_run.restype = i
-        _lib.ref_gp_loo.argtypes = [i, i, lg, i, i, vp, vp, d, vp, i, vp, vp]
-        _lib.ref_gp_loo.restype = i
-        _lib.ref_gp_mean_grad.argtypes = [i, lg, i, i, vp, vp, d, vp, i, vp, i, vp, vp, vp]
-        _lib.ref_gp_mean_grad.restype = i
-    return _lib
+_LIB = RefLibrary("libref_gp.so", _declare)
+LIB_PATH, available, load = _LIB.path, _LIB.available, _LIB.load
 
 
 def run(kernel_id: int, X, Y, noise=0.01, hp=None, Xq=None, n0=0, rprop_iters=0, optimize_noise=False, want_grad=True):

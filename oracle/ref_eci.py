@@ -1,38 +1,23 @@
 """ctypes front-end of oracle/_ref/libref_eci.so: the reference's OWN experimental::acqui::ECI (oracle/ref_shim/eci_driver.cpp,
-built by oracle/ref_shim/eci.mk).  TEST INFRASTRUCTURE ONLY; built only where the reference's sources are present (oracle/ref.py:
+built by oracle/ref_shim/Makefile).  TEST INFRASTRUCTURE ONLY; built only where the reference's sources are present (oracle/ref.py:
 REF_SRC) — elsewhere the tests rely on tests/golden/eci/."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_ROOT, REF_SRC
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "_ref", "libref_eci.so")
-_lib = None
+from .ref import RefLibrary
 
 
-def build() -> str:
-    if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "-f", "eci.mk", "CXX=g++", f"REF={REF_ROOT}", "all"], check=True,
-                       capture_output=True)
-    return LIB_PATH
+def _declare(lib):
+    vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
+    lib.ref_gp_eci.argtypes = [i, lg, i, vp, vp, lg, vp, d, d, lg, vp] + [vp] * 6
+    lib.ref_gp_eci.restype = i
 
 
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
-        _lib = C.CDLL(LIB_PATH)
-        vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
-        _lib.ref_gp_eci.argtypes = [i, lg, i, vp, vp, lg, vp, d, d, lg, vp] + [vp] * 6
-        _lib.ref_gp_eci.restype = i
-    return _lib
+_LIB = RefLibrary("libref_eci.so", _declare)
+LIB_PATH, available, load = _LIB.path, _LIB.available, _LIB.load
 
 
 def eci(con_kernel_id: int, X, y, Yc, Xq, noise=0.01, jitter=0.0):

@@ -1,41 +1,26 @@
 """ctypes front-end of oracle/_ref/libref_ehvi.so: the reference's OWN ehvi2d, experimental::acqui::Ehvi over two of its GPs, and
-pareto::pareto_set (oracle/ref_shim/ehvi_driver.cpp, built by oracle/ref_shim/ehvi.mk).  TEST INFRASTRUCTURE ONLY; built only
+pareto::pareto_set (oracle/ref_shim/ehvi_driver.cpp, built by oracle/ref_shim/Makefile).  TEST INFRASTRUCTURE ONLY; built only
 where the reference's sources are present (oracle/ref.py: REF_SRC) — elsewhere the tests rely on tests/golden/ehvi/."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_ROOT, REF_SRC
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "_ref", "libref_ehvi.so")
-_lib = None
+from .ref import RefLibrary
 
 
-def build() -> str:
-    if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "-f", "ehvi.mk", "CXX=g++", f"REF={REF_ROOT}", "all"], check=True,
-                       capture_output=True)
-    return LIB_PATH
+def _declare(lib):
+    vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
+    lib.ref_ehvi2d.argtypes = [lg, vp, vp, lg, vp, vp, vp]
+    lib.ref_pareto_set.argtypes = [lg, i, vp, vp, vp]
+    lib.ref_gp_ehvi.argtypes = [lg, i, vp, vp, d, vp, lg, vp, vp, vp, vp, vp, vp]
+    for f in (lib.ref_ehvi2d, lib.ref_pareto_set, lib.ref_gp_ehvi):
+        f.restype = i
 
 
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
-        _lib = C.CDLL(LIB_PATH)
-        vp, lg, i, d = C.c_void_p, C.c_long, C.c_int, C.c_double
-        _lib.ref_ehvi2d.argtypes = [lg, vp, vp, lg, vp, vp, vp]
-        _lib.ref_pareto_set.argtypes = [lg, i, vp, vp, vp]
-        _lib.ref_gp_ehvi.argtypes = [lg, i, vp, vp, d, vp, lg, vp, vp, vp, vp, vp, vp]
-        for f in (_lib.ref_ehvi2d, _lib.ref_pareto_set, _lib.ref_gp_ehvi):
-            f.restype = i
-    return _lib
+_LIB = RefLibrary("libref_ehvi.so", _declare)
+LIB_PATH, available, load = _LIB.path, _LIB.available, _LIB.load
 
 
 def _c(a, shape=None):

@@ -1,47 +1,28 @@
 """ctypes front-end of oracle/_ref/libref_ehvi3d.so: the reference's OWN ehvi3d_sliceupdate, ehvi3d_5term, ehvi3d_8term and hvol3d
-(oracle/ref_shim/ehvi3d_driver.cpp, built by oracle/ref_shim/ehvi3d.mk).  TEST INFRASTRUCTURE ONLY; built only where the
+(oracle/ref_shim/ehvi3d_driver.cpp, built by oracle/ref_shim/Makefile).  TEST INFRASTRUCTURE ONLY; built only where the
 reference's sources are present (oracle/ref.py: REF_SRC) — elsewhere the tests rely on tests/golden/ehvi3d/."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_ROOT, REF_SRC
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "_ref", "libref_ehvi3d.so")
-_lib = None
+from .ref import RefLibrary
 
 
-def build() -> str:
-    if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "-f", "ehvi3d.mk", "CXX=g++", f"REF={REF_ROOT}", "all"], check=True,
-                       capture_output=True)
-    return LIB_PATH
+def _declare(lib):
+    vp, lg, i = C.c_void_p, C.c_long, C.c_int
+    for f in (lib.ref_ehvi3d_sliceupdate, lib.ref_ehvi3d_5term, lib.ref_ehvi3d_8term):
+        f.argtypes = [lg, vp, vp, lg, vp, vp, vp]
+        f.restype = i
+    lib.ref_hv3d.argtypes = [lg, vp, vp, vp]
+    lib.ref_hv3d.restype = i
+    lib.ref_gp_ehvi3d.argtypes = [lg, i, vp, vp, C.c_double, vp, lg, vp, vp, vp, vp, vp, vp]
+    lib.ref_gp_ehvi3d.restype = i
 
 
-def available() -> bool:
-    return os.path.exists(LIB_PATH) or os.path.isdir(REF_SRC)
-
-
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
-        _lib = C.CDLL(LIB_PATH)
-        vp, lg, i = C.c_void_p, C.c_long, C.c_int
-        for f in (_lib.ref_ehvi3d_sliceupdate, _lib.ref_ehvi3d_5term, _lib.ref_ehvi3d_8term):
-            f.argtypes = [lg, vp, vp, lg, vp, vp, vp]
-            f.restype = i
-        _lib.ref_hv3d.argtypes = [lg, vp, vp, vp]
-        _lib.ref_hv3d.restype = i
-        _lib.ref_gp_ehvi3d.argtypes = [lg, i, vp, vp, C.c_double, vp, lg, vp, vp, vp, vp, vp, vp]
-        _lib.ref_gp_ehvi3d.restype = i
-    return _lib
+_LIB = RefLibrary("libref_ehvi3d.so", _declare)
+LIB_PATH, available, load = _LIB.path, _LIB.available, _LIB.load
 
 
 def _c(a, shape=None):

@@ -5,7 +5,7 @@
 // there is the 2-D one) behind C entries, and ehvi3d_sliceupdate over three of the reference's model::GP with the dense linear
 // algebra supplied by the stand-in in ./Eigen.  Used to pin oracle/ehvi3d.py (tests/test_ehvi3d_host.py) and to generate
 // tests/golden/ehvi3d/*.npz (tests/golden/make_golden_ehvi3d.py).  No reference source is copied: this file only instantiates
-// its templates and calls the functions of the reference's src/ehvi/*.cc, which ehvi3d.mk links.
+// its templates and calls the functions of the reference's src/ehvi/*.cc, which the Makefile links into libref_ehvi3d.so.
 //
 // The front is handed over in the order given.  The reference sorts it with std::sort, which is not stable;
 // tests/test_ehvi3d_host.py checks that the tested fronts' sums do not depend on their input order.

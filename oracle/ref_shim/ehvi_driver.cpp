@@ -4,7 +4,7 @@
 // two of the reference's model::GP) and its Pareto filter (experimental/tools/pareto.hpp), with the dense linear algebra supplied
 // by the stand-in in ./Eigen.  Used to pin oracle/ehvi.py (tests/test_ehvi_host.py) and to generate tests/golden/ehvi/*.npz
 // (tests/golden/make_golden_ehvi.py).  No reference source is copied: this file only instantiates its templates and links the
-// reference's src/ehvi/*.cc (ehvi.mk).
+// reference's src/ehvi/*.cc (Makefile: libref_ehvi.so).
 #include <deque>
 #include <tuple>
 #include <vector>

@@ -1,42 +1,23 @@
 """ctypes front-end of oracle/_ref/libref_sparse.so: the reference's OWN model::SparsifiedGP::_sparsify
-(oracle/ref_shim/sparse_driver.cpp, built by oracle/ref_shim/sparse.mk).  TEST INFRASTRUCTURE ONLY; built only where the
+(oracle/ref_shim/sparse_driver.cpp, built by oracle/ref_shim/Makefile).  TEST INFRASTRUCTURE ONLY; built only where the
 reference's sources are present (oracle/ref.py: REF_SRC) — elsewhere the tests rely on tests/golden/sparsify/."""
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from .ref import REF_ROOT, REF_SRC
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(HERE, "_ref", "libref_sparse.so")
-_lib = None
+from .ref import RefLibrary
 
 
-def available() -> bool:
-    return os.path.exists(LIB_PATH) or os.path.isdir(REF_SRC)
+def _declare(lib):
+    vp, lg, i = C.c_void_p, C.c_long, C.c_int
+    lib.ref_sparsify.argtypes = [lg, i, vp, lg] + [vp] * 5
+    lib.ref_sparsify.restype = i
 
 
-def build() -> str:
-    if os.path.isdir(REF_SRC):
-        subprocess.run(["make", "-C", os.path.join(HERE, "ref_shim"), "-f", "sparse.mk", "CXX=g++", f"REF={REF_ROOT}", "all"], check=True,
-                       capture_output=True)
-    return LIB_PATH
-
-
-def load():
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
-            build()
-        _lib = C.CDLL(LIB_PATH)
-        vp, lg, i = C.c_void_p, C.c_long, C.c_int
-        _lib.ref_sparsify.argtypes = [lg, i, vp, lg] + [vp] * 5
-        _lib.ref_sparsify.restype = i
-    return _lib
+_LIB = RefLibrary("libref_sparse.so", _declare)
+LIB_PATH, available, load = _LIB.path, _LIB.available, _LIB.load
 
 
 def sparsify(X, max_points: int):

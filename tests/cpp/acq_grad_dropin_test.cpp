@@ -12,6 +12,7 @@
 #include <vector>
 
 #include <Eigen/Core>
+#include "dropin_common.hpp"
 
 #include <limbo/acqui/ucb.hpp>
 #include <limbo/kernel/matern_five_halves.hpp>
@@ -24,10 +25,6 @@
 #include <limbo_b200/opt/batched_gradient.hpp>
 
 using namespace limbo;
-
-struct FirstElem { // bayes_opt/bo_base.hpp:99-105, which needs Boost.Parameter
-    double operator()(const Eigen::VectorXd& x) const { return x(0); }
-};
 
 struct Params {
     struct kernel : public defaults::kernel {};
@@ -53,16 +50,6 @@ struct Params {
 };
 
 using GP_t = limbo_b200::model::GP<Params, kernel::MaternFiveHalves<Params>, mean::Data<Params>, model::gp::NoLFOpt<Params>>;
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
 
 static Eigen::VectorXd target(const Eigen::VectorXd& x)
 {

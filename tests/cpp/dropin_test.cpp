@@ -4,6 +4,7 @@
 // reference's limbo::model::GP; results must agree to the fp64 bar.  Needs a GPU to run.
 // (Eigen is the stand-in from oracle/ref_shim so that no Eigen install is needed.)
 #include <cstdio>
+#include "dropin_common.hpp"
 #include <limbo/acqui/ei.hpp>
 #include <limbo/acqui/ucb.hpp>
 #include <limbo/kernel/matern_five_halves.hpp>
@@ -40,20 +41,6 @@ struct Params {
         BO_PARAM(int, candidates, 4000);
     };
 };
-
-struct FirstElem {
-    double operator()(const Eigen::VectorXd& x) const { return x(0); }
-};
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
 
 // SquaredExpARD with two Lambda columns (squared_exp_ard.hpp:109-126,142-146)
 struct ParamsLambda : Params {

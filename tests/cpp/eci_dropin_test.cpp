@@ -6,6 +6,7 @@
 // must agree to 1e-10 with the same argmax.  Needs a GPU to run; prints "ECI DROPIN OK".
 // (Eigen is the stand-in from oracle/ref_shim so that no Eigen install is needed.)
 #include <cstdio>
+#include "dropin_common.hpp"
 #include <limbo/acqui/ucb.hpp>
 #include <limbo/experimental/acqui/eci.hpp>
 #include <limbo/kernel/exp.hpp>
@@ -30,20 +31,6 @@ struct Params {
     struct opt_batchedrandom : public limbo_b200::defaults::opt_batchedrandom {};
 };
 
-struct FirstElem {
-    double operator()(const Eigen::VectorXd& x) const { return x(0); }
-};
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
-
 using RefGP = model::GP<Params, kernel::SquaredExpARD<Params>, mean::Data<Params>>;
 using RefGPc = model::GP<Params, kernel::Exp<Params>, mean::Constant<Params>>;
 using NewGP = limbo_b200::model::GP<Params, kernel::SquaredExpARD<Params>, mean::Data<Params>, model::gp::NoLFOpt<Params>>;
@@ -56,14 +43,6 @@ static std::vector<double> one_by_one(Acq& acq, const std::vector<Eigen::VectorX
     std::vector<double> v;
     for (auto& q : Q) v.push_back(opt::fun(acq(q, afun, false)));
     return v;
-}
-
-static long first_max(const std::vector<double>& v)
-{
-    long i = 0;
-    for (long k = 1; k < (long)v.size(); ++k)
-        if (v[(size_t)k] > v[(size_t)i]) i = k;
-    return i;
 }
 
 // nc: constraint samples (0: a constraint model without samples, Pf = 1)

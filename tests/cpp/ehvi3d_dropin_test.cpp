@@ -18,11 +18,7 @@
 
 #include <Eigen/Core>
 
-namespace limbo { // bayes_opt/bo_base.hpp:99-105, which needs Boost.Parameter
-    struct FirstElem {
-        double operator()(const Eigen::VectorXd& x) const { return x(0); }
-    };
-} // namespace limbo
+#include "dropin_common.hpp"
 
 #include <limbo/experimental/tools/pareto.hpp>
 #include <limbo/kernel/matern_five_halves.hpp>
@@ -50,16 +46,6 @@ struct Scaled { // not FirstElem-like: the host path
     double operator()(const Eigen::VectorXd& x) const { return 0.5 * x(0); }
 };
 
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
-
 static Eigen::VectorXd dtlz2(const Eigen::VectorXd& x) // three objectives, negated so that they are maximised
 {
     double g = 0;
@@ -70,14 +56,6 @@ static Eigen::VectorXd dtlz2(const Eigen::VectorXd& x) // three objectives, nega
     r(1) = -(1 + g) * std::cos(a) * std::sin(b);
     r(2) = -(1 + g) * std::sin(a);
     return r;
-}
-
-static long first_max(const std::vector<double>& v)
-{
-    long i = 0;
-    for (long k = 1; k < (long)v.size(); ++k)
-        if (v[(size_t)k] > v[(size_t)i]) i = k;
-    return i;
 }
 
 template <typename Agg>

@@ -15,11 +15,7 @@
 
 #include <Eigen/Core>
 
-namespace limbo { // bayes_opt/bo_base.hpp:99-105, which needs Boost.Parameter
-    struct FirstElem {
-        double operator()(const Eigen::VectorXd& x) const { return x(0); }
-    };
-} // namespace limbo
+#include "dropin_common.hpp"
 
 #include <limbo/experimental/tools/pareto.hpp>
 #include <limbo/kernel/matern_five_halves.hpp>
@@ -43,16 +39,6 @@ struct Params {
 using RefGP = model::GP<Params, kernel::MaternFiveHalves<Params>, mean::Data<Params>>;
 using NewGP = limbo_b200::model::GP<Params, kernel::MaternFiveHalves<Params>, mean::Data<Params>, model::gp::NoLFOpt<Params>>;
 
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
-
 static Eigen::VectorXd mop2(const Eigen::VectorXd& x) // examples/experimental/multi.cpp
 {
     const double c = 1.0 / std::sqrt((double)x.size());
@@ -66,14 +52,6 @@ static Eigen::VectorXd mop2(const Eigen::VectorXd& x) // examples/experimental/m
     r(0) = std::exp(-v1);
     r(1) = std::exp(-v2);
     return r;
-}
-
-static long first_max(const std::vector<double>& v)
-{
-    long i = 0;
-    for (long k = 1; k < (long)v.size(); ++k)
-        if (v[(size_t)k] > v[(size_t)i]) i = k;
-    return i;
 }
 
 static int run_case(int N, int D, double ref0, double ref1)

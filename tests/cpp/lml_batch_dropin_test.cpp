@@ -12,6 +12,7 @@
 #include <vector>
 
 #include <Eigen/Core>
+#include "dropin_common.hpp"
 
 #include <limbo/kernel/matern_five_halves.hpp>
 #include <limbo/kernel/squared_exp_ard.hpp>
@@ -38,16 +39,6 @@ struct Params {
         BO_PARAM(double, epsilon, 1e-2);
     };
 };
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
 
 static void data(int N, int D, std::vector<Eigen::VectorXd>& X, std::vector<Eigen::VectorXd>& Y)
 {

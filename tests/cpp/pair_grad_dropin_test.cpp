@@ -18,11 +18,7 @@
 
 #include <Eigen/Core>
 
-namespace limbo { // bayes_opt/bo_base.hpp:99-105, which needs Boost.Parameter
-    struct FirstElem {
-        double operator()(const Eigen::VectorXd& x) const { return x(0); }
-    };
-} // namespace limbo
+#include "dropin_common.hpp"
 
 #include <limbo/kernel/exp.hpp>
 #include <limbo/kernel/matern_five_halves.hpp>
@@ -65,16 +61,6 @@ using ObjGP = limbo_b200::model::GP<Params, kernel::SquaredExpARD<Params>, mean:
 using ConGP = limbo_b200::model::GP<Params, kernel::Exp<Params>, mean::Constant<Params>, model::gp::NoLFOpt<Params>>;
 using MoGP = limbo_b200::model::GP<Params, kernel::MaternFiveHalves<Params>, mean::Data<Params>, model::gp::NoLFOpt<Params>>;
 using ECI_t = limbo_b200::acqui::ECI<Params, ObjGP, ConGP>;
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
 
 static Eigen::VectorXd point(unsigned long long& seed, double lo = 0.0, double hi = 1.0)
 {

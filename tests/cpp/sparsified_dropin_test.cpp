@@ -7,6 +7,7 @@
 #include <Eigen/Core> // first: the stand-in with the writable VectorXd::Map (sparse_eigen/Eigen/Core)
 #include <cmath>
 #include <cstdio>
+#include "dropin_common.hpp"
 #include <limbo/kernel/matern_five_halves.hpp>
 #include <limbo/kernel/squared_exp_ard.hpp>
 #include <limbo/mean/constant.hpp>
@@ -29,16 +30,6 @@ struct Params {
     };
 };
 BO_DECLARE_DYN_PARAM(int, Params::model_sparse_gp, max_points);
-
-static double u01(unsigned long long& s)
-{ // splitmix64, as limbo_b200/synth.py
-    s += 0x9E3779B97F4A7C15ULL;
-    unsigned long long z = s;
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-    z ^= z >> 31;
-    return (double)(z >> 11) * (1.0 / 9007199254740992.0);
-}
 
 static int failures = 0;
 static void check(bool ok, const char* what)

@@ -1,5 +1,5 @@
 // tests/cpp/spgp_dropin_test.cpp — the reference's experimental::model::SPGP next to limbo_b200::model::SPGP, built by
-// oracle/ref_shim/spgp.mk against the Eigen stand-in of oracle/ref_shim/spgp_eigen and run by tests/test_gpu_spgp.py.
+// oracle/ref_shim/Makefile's spgp_dropin_test against the Eigen stand-in of oracle/ref_shim/spgp_eigen; run by tests/test_gpu_spgp.py.
 // At a fixed w both models' _likelihood(w, true) and _compute(false) + predict must agree (value <= 1e-10 relative, gradient
 // <= 1e-7 |g|inf, mu and sigma^2 <= 1e-9 c); then limbo_b200's public compute + query runs with the reference's Rprop.
 // Prints "SPGP DROPIN OK" on success.
@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <vector>
+#include "dropin_common.hpp"
 
 namespace nlopt {
 enum algorithm { LD_LBFGS = 11 };

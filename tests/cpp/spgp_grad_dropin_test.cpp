@@ -1,5 +1,5 @@
 // tests/cpp/spgp_grad_dropin_test.cpp — the batch-aware acquisitions over limbo_b200::model::SPGP, next to the reference's
-// experimental::model::SPGP at the same w; built by oracle/ref_shim/spgp_grad.mk against the Eigen stand-in
+// experimental::model::SPGP at the same w; built by oracle/ref_shim/Makefile's spgp_grad_dropin_test against the Eigen stand-in
 // of oracle/ref_shim/spgp_eigen and run by tests/test_gpu_spgp_grad.py:
 //   (1) limbo_b200::acqui::UCB / EI operator()(v, afun, true) (one lb_spgp_acq_grad) agrees with central differences of
 //       operator()(v, afun, false) to 1e-6 relative;
@@ -11,6 +11,7 @@
 #include <cmath>
 #include <cstdio>
 #include <vector>
+#include "dropin_common.hpp"
 
 namespace nlopt {
 enum algorithm { LD_LBFGS = 11 };
@@ -31,10 +32,6 @@ struct NLOptGrad;
 #include <limbo_b200/opt/batched_gradient.hpp>
 
 using namespace limbo;
-
-struct FirstElem { // bayes_opt/bo_base.hpp:99-105, which needs Boost.Parameter
-    double operator()(const Eigen::VectorXd& x) const { return x(0); }
-};
 
 struct Params {
     struct kernel : public defaults::kernel {};

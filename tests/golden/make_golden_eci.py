@@ -1,7 +1,7 @@
 """Generates tests/golden/eci/*.npz: the REFERENCE'S OWN experimental::acqui::ECI (oracle/_ref/libref_eci.so, entry ref_gp_eci,
 see oracle/ref_shim/eci_driver.cpp) on seeded inputs, stored together with those inputs.  Objective: SE-ARD / mean::Data, P = 1;
 constraint: Exp or Matern-5/2 / mean::Constant (constant 0.25), P = 2; default hyper-parameters; 500 candidates.  Needs a built
-oracle/_ref/libref_eci.so (oracle/ref_shim/eci.mk):
+oracle/_ref/libref_eci.so (oracle/ref_shim/Makefile: libref_eci.so):
     python tests/golden/make_golden_eci.py"""
 import os
 import sys

@@ -1,7 +1,7 @@
 """Generates tests/golden/ehvi/*.npz: the REFERENCE'S OWN experimental::acqui::Ehvi over two of its GPs (oracle/_ref/libref_ehvi.so,
 entry ref_gp_ehvi) and its raw ehvi2d (entry ref_ehvi2d) on seeded inputs, stored together with those inputs.  Models:
 Matern-5/2 / mean::Data, P = 1, default hyper-parameters; reference point (-11, -11) as bayes_opt_ehvi's defaults.  Needs a built
-oracle/_ref/libref_ehvi.so (oracle/ref_shim/ehvi.mk):
+oracle/_ref/libref_ehvi.so (oracle/ref_shim/Makefile: libref_ehvi.so):
     python tests/golden/make_golden_ehvi.py"""
 import os
 import sys

@@ -1,6 +1,7 @@
 """Generate tests/golden/sparsify/*.npz from the reference's OWN model::SparsifiedGP::_sparsify (oracle/ref_sparse.py, built by
-oracle/ref_shim/sparse.mk against the Eigen stand-in).  Each file stores X, max_points, the kept indices, the removal order and the
-density of every removed point when it was chosen.  Run from the repository root: python tests/golden/make_golden_sparsify.py"""
+oracle/ref_shim/Makefile as libref_sparse.so against the Eigen stand-in).  Each file stores X, max_points, the kept indices, the
+removal order and the density of every removed point when it was chosen.  Run from the repository root:
+    python tests/golden/make_golden_sparsify.py"""
 from __future__ import annotations
 
 import os

@@ -1,6 +1,7 @@
 """Generate tests/golden/spgp/*.npz from the reference's OWN experimental::model::SPGP (oracle/ref_spgp.py, built by
-oracle/ref_shim/spgp.mk against the Eigen stand-in).  Each file stores X, y, M, w, the jitter, the _likelihood value f and gradient,
-the _compute(false) factors L, Lm and bet at w, and mu (mean(v) included) / sigma^2 of _predict on 500 candidates Xq.
+oracle/ref_shim/Makefile as libref_spgp.so against the Eigen stand-in).  Each file stores X, y, M, w, the jitter, the _likelihood
+value f and gradient, the _compute(false) factors L, Lm and bet at w, and mu (mean(v) included) / sigma^2 of _predict on 500
+candidates Xq.
 w is the reference's starting vector for a seeded permutation, moved off the start so that no pseudo-input sits on a sample.
 Run from the repository root: python tests/golden/make_golden_spgp.py"""
 from __future__ import annotations

@@ -40,10 +40,9 @@ def test_fixtures_present():
 @pytest.mark.parametrize("path", FIXTURES, ids=os.path.basename)
 def test_oracle_eci_equals_reference_live(path):
     """The restatement reproduces the reference's ECI bit for bit on the reference's own mu / sigma^2."""
-    from oracle import ref, ref_eci
-    if not os.path.isdir(ref.REF_SRC):
-        pytest.skip("the reference's sources are not present")
-    ref_eci.build()
+    from oracle import ref_eci
+    if not ref_eci.available():
+        pytest.skip("the reference's ECI is not built and its sources are not present")
     g = np.load(path)
     r = ref_eci.eci(int(g["con_kernel"]), g["X"], g["y"], g["Yc"], g["Xq"], float(g["noise"]), float(g["jitter"]))
     r.update(Yc=g["Yc"], jitter=g["jitter"])

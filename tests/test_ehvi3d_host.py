@@ -21,7 +21,7 @@ FIXTURES = sorted(glob.glob(os.path.join(ROOT, "tests", "golden", "ehvi3d", "*.n
 def ref():
     from oracle import ref_ehvi3d as R
     if not R.available():
-        pytest.skip("the reference's sources are not present")
+        pytest.skip("the reference's EHVI is not built and its sources are not present")
     return R
 
 

@@ -5,8 +5,6 @@ acquisition optimiser bayes_opt.BatchedGradientSearch."""
 import ctypes as C
 import gc
 import math
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,6 +12,7 @@ from scipy.linalg import cho_solve, cholesky
 from scipy.optimize import minimize
 from scipy.spatial.distance import cdist
 
+from dropin import run_dropin
 from oracle import acq_grad as AG
 
 pytestmark = pytest.mark.gpu
@@ -377,11 +376,4 @@ def test_no_samples_acquisition_follows_the_mean():
 def test_cpp_dropin():
     """tests/cpp/acq_grad_dropin_test.cpp: limbo_b200::acqui::UCB / EI gradients against central differences and the batched
     answer, the reference's opt::GradientAscent / opt::Adam over them, and limbo_b200::opt::BatchedGradient"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    binary = os.path.join(root, "oracle", "_ref", "acq_grad_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/acq_grad_dropin_test not built (needs the reference's sources at build time)")
-    env = dict(os.environ, LD_LIBRARY_PATH=os.path.join(root, "limbo_b200", "lib") + ":" + os.environ.get("LD_LIBRARY_PATH", ""))
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600, env=env)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "ACQ GRAD DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("acq_grad_dropin_test", "ACQ GRAD DROPIN OK")

@@ -4,12 +4,12 @@ where it must degenerate to it, and through the Python and C++ callers."""
 import ctypes as C
 import glob
 import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
+from dropin import run_dropin
 from oracle import eci as oracle_eci
 
 pytestmark = pytest.mark.gpu
@@ -284,9 +284,4 @@ def test_cboptimizer_converges_to_constrained_optimum():
 
 
 def test_cpp_eci_dropin():
-    binary = os.path.join(ROOT, "oracle", "_ref", "eci_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/eci_dropin_test not built (needs the reference's sources at build time)")
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "ECI DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("eci_dropin_test", "ECI DROPIN OK")

@@ -4,13 +4,13 @@ determinism and concurrency, lb_pareto_set against the oracle, and a bayes_opt.E
 import ctypes as C
 import glob
 import os
-import subprocess
 import threading
 import time
 
 import numpy as np
 import pytest
 
+from dropin import run_dropin
 from oracle import ehvi as E
 
 pytestmark = pytest.mark.gpu
@@ -308,9 +308,4 @@ def test_bayes_opt_ehvi_on_mop2():
 def test_cpp_ehvi_dropin():
     """The reference's primary acqui::Ehvi over reference GPs against the specialisation over limbo_b200::model::GP, one point
     at a time, answering a BatchRequest, and driven by BatchedRandom (tests/cpp/ehvi_dropin_test.cpp)."""
-    binary = os.path.join(ROOT, "oracle", "_ref", "ehvi_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/ehvi_dropin_test not built (needs the reference's sources at build time)")
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "EHVI DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("ehvi_dropin_test", "EHVI DROPIN OK")

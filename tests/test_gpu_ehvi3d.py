@@ -5,12 +5,12 @@ variant, determinism, concurrency, multi-output models and a bayes_opt.Ehvi run 
 import ctypes as C
 import glob
 import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 
+from dropin import run_dropin
 from oracle import ehvi as E2
 from oracle import ehvi3d as E
 
@@ -107,12 +107,7 @@ def test_cpp_ehvi3d_dropin():
     """ehvi3d_sliceupdate over three reference GPs against the three-model acqui::Ehvi specialisation over limbo_b200::model::GP,
     one point at a time, answering a BatchRequest (and leaving the GradRequest), on the host path of another aggregator, and
     driven by BatchedRandom (tests/cpp/ehvi3d_dropin_test.cpp)."""
-    binary = os.path.join(ROOT, "oracle", "_ref", "ehvi3d_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/ehvi3d_dropin_test not built (needs the reference's sources at build time)")
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "EHVI3D DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("ehvi3d_dropin_test", "EHVI3D DROPIN OK")
 
 
 def test_ehvi3d_dtlz2_models_against_oracle():

@@ -11,6 +11,7 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
+from dropin import run_dropin  # noqa: E402
 from limbo_b200 import _lib, kernel, mean, model, opt, synth  # noqa: E402
 
 KERNELS = {0: kernel.SquaredExpARD, 1: kernel.MaternFiveHalves, 2: kernel.MaternThreeHalves, 3: kernel.Exp}
@@ -389,13 +390,4 @@ def test_rows_match_reference_fixtures(path):
 
 
 def test_cpp_dropin():
-    import os
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    binary = os.path.join(root, "oracle", "_ref", "lml_batch_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/lml_batch_dropin_test not built (needs the reference's sources at build time)")
-    env = dict(os.environ, LD_LIBRARY_PATH=os.path.join(root, "limbo_b200", "lib") + ":" + os.environ.get("LD_LIBRARY_PATH", ""))
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600, env=env)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "LML BATCH DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("lml_batch_dropin_test", "LML BATCH DROPIN OK")

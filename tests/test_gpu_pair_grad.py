@@ -5,8 +5,6 @@ the two handles, determinism, concurrent calls, plumbing (leases, errors), and b
 import ctypes as C
 import gc
 import math
-import os
-import subprocess
 import threading
 
 import numpy as np
@@ -15,6 +13,7 @@ from scipy.linalg import cho_solve, cholesky
 from scipy.optimize import minimize
 from scipy.spatial.distance import cdist
 
+from dropin import run_dropin
 from oracle import acq_grad as AG
 from oracle import ehvi as OH
 from oracle import pair_grad as PG
@@ -536,11 +535,4 @@ def test_cpp_dropin():
     """tests/cpp/pair_grad_dropin_test.cpp: limbo_b200::acqui::ECI gradients against central differences and the batched answer,
     the reference's opt::Adam over them, and limbo_b200::opt::BatchedGradient in the inner loops of CBOptimizer and Ehvi over
     limbo_b200::acqui::ECI and the acqui::Ehvi specialisation"""
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    binary = os.path.join(root, "oracle", "_ref", "pair_grad_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/pair_grad_dropin_test not built (needs the reference's sources at build time)")
-    env = dict(os.environ, LD_LIBRARY_PATH=os.path.join(root, "limbo_b200", "lib") + ":" + os.environ.get("LD_LIBRARY_PATH", ""))
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600, env=env)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "PAIR GRAD DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("pair_grad_dropin_test", "PAIR GRAD DROPIN OK")

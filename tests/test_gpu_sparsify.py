@@ -4,11 +4,11 @@ BOptimizer over it and the compiled C++ drop-in against the reference's Sparsifi
 import ctypes as C
 import glob
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from dropin import run_dropin
 from oracle import sparsify as oracle_sparsify
 
 pytestmark = pytest.mark.gpu
@@ -226,9 +226,4 @@ def test_boptimizer_with_sparsified_gp():
 
 
 def test_cpp_sparsified_dropin():
-    binary = os.path.join(ROOT, "oracle", "_ref", "sparse_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/sparse_dropin_test not built (needs the reference's sources at build time)")
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "SPARSE DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("sparse_dropin_test", "SPARSE DROPIN OK")

@@ -6,11 +6,11 @@ import ctypes as C
 import glob
 import math
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from dropin import run_dropin
 from oracle import spgp as O
 
 pytestmark = pytest.mark.gpu
@@ -265,9 +265,4 @@ def test_boptimizer_with_spgp():
 
 
 def test_cpp_spgp_dropin():
-    binary = os.path.join(ROOT, "oracle", "_ref", "spgp_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/spgp_dropin_test not built (needs the reference's sources at build time)")
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "SPGP DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("spgp_dropin_test", "SPGP DROPIN OK")

@@ -8,13 +8,13 @@ import ctypes as C
 import glob
 import math
 import os
-import subprocess
 import threading
 
 import numpy as np
 import pytest
 from scipy.optimize import minimize
 
+from dropin import run_dropin
 from oracle import acq_grad as AG
 from oracle import spgp as O
 from oracle import spgp_grad as SG
@@ -377,10 +377,4 @@ def test_gradient_search_reaches_the_lbfgsb_maximum(acq_name):
 
 
 def test_cpp_spgp_grad_dropin():
-    binary = os.path.join(ROOT, "oracle", "_ref", "spgp_grad_dropin_test")
-    if not os.path.exists(binary):
-        pytest.skip("oracle/_ref/spgp_grad_dropin_test not built (needs the reference's sources at build time)")
-    env = dict(os.environ, LD_LIBRARY_PATH=os.path.join(ROOT, "limbo_b200", "lib") + ":" + os.environ.get("LD_LIBRARY_PATH", ""))
-    r = subprocess.run([binary], capture_output=True, text=True, timeout=600, env=env)
-    print(r.stdout, r.stderr)
-    assert r.returncode == 0 and "SPGP GRAD DROPIN OK" in r.stdout, r.stdout + r.stderr
+    run_dropin("spgp_grad_dropin_test", "SPGP GRAD DROPIN OK")

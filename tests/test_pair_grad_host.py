@@ -3,7 +3,6 @@ differences of the restatements pinned to the reference (oracle.eci.eci_one, ora
 oracle/acq_grad.query_grad against central differences in the candidate, and, where the reference's own ECI and ehvi2d are built
 (oracle/_ref/libref_eci.so, libref_ehvi.so), the same checks against the reference's values.  CPU only."""
 import math
-import os
 
 import numpy as np
 import pytest
@@ -14,9 +13,8 @@ from oracle import acq_grad as AG
 from oracle import eci as OE
 from oracle import ehvi as OH
 from oracle import pair_grad as PG
+from oracle import ref_eci, ref_ehvi
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-REF_DIR = os.path.join(os.path.dirname(HERE), "oracle", "_ref")
 RTOL = 1e-6
 
 
@@ -150,9 +148,8 @@ def test_chains_match_central_differences_in_the_candidate():
             assert np.all((np.abs(g[:, d] - fd) <= RTOL * 10 * scale)[ok]), (fun.__name__, np.abs(g[:, d] - fd).max())
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(REF_DIR, "libref_ehvi.so")), reason="the reference's ehvi2d is not built")
+@pytest.mark.skipif(not ref_ehvi.available(), reason="the reference's ehvi2d is not built and its sources are not present")
 def test_ehvi_partials_against_the_reference():
-    from oracle import ref_ehvi
     rng = np.random.default_rng(7)
     F = _front(rng, 7)
     r = (-0.2, -0.1)
@@ -168,11 +165,10 @@ def test_ehvi_partials_against_the_reference():
             assert _close(P[0, i], (vp - vm) / 2e-6, 1e-3 * (mag[0, i] + abs(val[0]) + 1.0)), (i, P[0, i], (vp - vm) / 2e-6)
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(REF_DIR, "libref_eci.so")), reason="the reference's ECI is not built")
+@pytest.mark.skipif(not ref_eci.available(), reason="the reference's ECI is not built and its sources are not present")
 def test_eci_partials_against_the_reference():
     """the reference's ECI over its own GPs: d ECI / dx by central differences against the partials at its mu / sigma^2, chained
     with central differences of its own mu / sigma^2"""
-    from oracle import ref_eci
     rng = np.random.default_rng(8)
     X = rng.random((30, 2))
     y = np.sin(3 * X[:, 0]) + X[:, 1]

@@ -46,10 +46,9 @@ def test_lattice_fixture_pins_the_tie_rule():
 
 
 def _ref_or_skip():
-    from oracle import ref, ref_sparse
-    if not os.path.isdir(ref.REF_SRC):
-        pytest.skip("the reference's sources are not present")
-    ref_sparse.build()
+    from oracle import ref_sparse
+    if not ref_sparse.available():
+        pytest.skip("the reference's _sparsify is not built and its sources are not present")
     return ref_sparse
 
 

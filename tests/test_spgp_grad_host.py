@@ -82,7 +82,7 @@ def test_oracle_matches_central_differences_of_its_prediction(M, D, N, optimized
 def test_oracle_matches_central_differences_of_the_reference(M, D, N):
     from oracle import ref_spgp
     if not ref_spgp.available():
-        pytest.skip("the reference's SPGP was not built (oracle/_ref/libref_spgp.so)")
+        pytest.skip("the reference's SPGP is not built and its sources are not present")
     X, y, w, Xq = _case(M, D, N)
     st = O.State(w, X, y, M, JITTER)
     _, _, dmu, ds2, _ = SG.query_grad(st, Xq)
