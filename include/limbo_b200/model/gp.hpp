@@ -30,6 +30,7 @@
 #include <Eigen/Core>
 
 #include "../../limbo_b200.h"
+#include "batch_args.hpp"
 #include "mean_traits.hpp" // mean_is_input_free
 
 namespace limbo {
@@ -150,35 +151,23 @@ namespace limbo_b200 {
             {
                 const long M = (long)vs.size();
                 const int P = _dim_out > 0 ? _dim_out : 1;
-                const int D = (int)vs[0].size();
-                if (_samples.empty()) _push_prior(D);
-                std::vector<double> xq((size_t)M * D), m((size_t)M * P), s((size_t)M);
-                for (long i = 0; i < M; ++i)
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
+                if (_samples.empty()) _push_prior((int)vs[0].size());
+                std::vector<double> xq = detail::pack_rows(vs), m((size_t)M * P), s((size_t)M);
                 lb_check(lb_query(_h, M, xq.data(), m.data(), s.data()), "lb_query");
-                mu.resize(M, P);
-                sigma2.resize(M);
-                for (long i = 0; i < M; ++i) {
-                    Eigen::VectorXd mv = _mean_function(vs[i], *this); // gp.hpp:615 (host functor)
-                    for (int p = 0; p < P; ++p) mu(i, p) = m[(size_t)i * P + p] + mv(p);
-                    sigma2(i) = s[(size_t)i];
-                }
+                detail::unpack(m, M, P, mu);
+                _add_mean(vs, mu); // gp.hpp:615 (host functor)
+                detail::unpack(s, sigma2);
             }
             // fused UCB / EI + argmax on the device with the FirstElem aggregator (bo_base.hpp:99-105)
             std::pair<double, long> acq_argmax(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs,
                 std::vector<double>* values = nullptr) const
             {
-                const long M = (long)vs.size();
-                const int D = (int)vs[0].size();
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs);
                 double params[2] = {p0, p1}, best = 0;
                 int64_t idx = 0;
-                if (values) values->resize((size_t)M);
-                lb_check(lb_acq_argmax(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, values ? values->data() : nullptr, &best, &idx),
+                if (values) values->resize(vs.size());
+                lb_check(lb_acq_argmax(_h, acq_id, params, (int64_t)vs.size(), xq.data(), mean0.data(), 0.0, values ? values->data() : nullptr,
+                             &best, &idx),
                     "lb_acq_argmax");
                 return std::make_pair(best, (long)idx);
             }
@@ -190,19 +179,12 @@ namespace limbo_b200 {
                 static_assert(mean_is_input_free<MeanFunction>::value, "acq_grad: the mean function has no input gradient");
                 const long M = (long)vs.size();
                 const int D = (int)vs[0].size();
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), v((size_t)M), g((size_t)M * D);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs);
+                std::vector<double> v((size_t)M), g((size_t)M * D);
                 double params[2] = {p0, p1};
                 lb_check(lb_acq_grad(_h, acq_id, params, M, xq.data(), mean0.data(), 0.0, nullptr, v.data(), g.data()), "lb_acq_grad");
-                values = Eigen::VectorXd((Eigen::Index)M);
-                grads = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                for (long i = 0; i < M; ++i) {
-                    values(i) = v[(size_t)i];
-                    for (int d = 0; d < D; ++d) grads(i, d) = g[(size_t)i * D + d];
-                }
+                detail::unpack(v, values);
+                detail::unpack(g, M, D, grads);
             }
             // mu (M x P, mean added), sigma^2 (M) and their candidate gradients: dmu (M x D, of the first output), dsigma2 (M x D)
             // in one device pass (lb_query_grad)
@@ -212,23 +194,14 @@ namespace limbo_b200 {
                 static_assert(mean_is_input_free<MeanFunction>::value, "query_grad: the mean function has no input gradient");
                 const long M = (long)vs.size();
                 const int D = (int)vs[0].size(), P = (int)_dim_out;
-                std::vector<double> xq((size_t)M * D), m((size_t)M * P), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
-                for (long i = 0; i < M; ++i)
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
+                const std::vector<double> xq = detail::pack_rows(vs);
+                std::vector<double> m((size_t)M * P), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
                 lb_check(lb_query_grad(_h, M, xq.data(), m.data(), s.data(), gm.data(), gs.data()), "lb_query_grad");
-                mu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)P);
-                sigma2 = Eigen::VectorXd((Eigen::Index)M);
-                dmu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                dsigma2 = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                for (long i = 0; i < M; ++i) {
-                    Eigen::VectorXd mv = _mean_function(vs[i], *this);
-                    for (int p = 0; p < P; ++p) mu(i, p) = m[(size_t)i * P + p] + mv(p);
-                    sigma2(i) = s[(size_t)i];
-                    for (int d = 0; d < D; ++d) {
-                        dmu(i, d) = gm[(size_t)i * D + d];
-                        dsigma2(i, d) = gs[(size_t)i * D + d];
-                    }
-                }
+                detail::unpack(m, M, P, mu);
+                _add_mean(vs, mu);
+                detail::unpack(s, sigma2);
+                detail::unpack(gm, M, D, dmu);
+                detail::unpack(gs, M, D, dsigma2);
             }
             // fused ECI + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem aggregator): this GP is the objective,
             // `con` the constraint model, whose first output gives Pf (Pf = 1 while it has no samples).  Both mean functors run on
@@ -239,19 +212,13 @@ namespace limbo_b200 {
             {
                 if (values) values->assign(vs.size(), 0.0);
                 if (_samples.empty()) return std::make_pair(0.0, 0L);
-                const long M = (long)vs.size();
-                const int D = (int)vs[0].size();
                 const bool use_con = !con._samples.empty();
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), cmean0(use_con ? (size_t)M : 0);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                    if (use_con) cmean0[(size_t)i] = con._mean_function(vs[i], con)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs),
+                                          cmean0 = use_con ? detail::first_means(con, vs) : std::vector<double>();
                 double params[2] = {f_max, jitter}, best = 0;
                 int64_t idx = 0;
-                lb_check(lb_eci_argmax(_h, con._h, params, M, xq.data(), mean0.data(), 0.0, use_con ? cmean0.data() : nullptr, 0.0,
-                             values ? values->data() : nullptr, &best, &idx),
+                lb_check(lb_eci_argmax(_h, con._h, params, (int64_t)vs.size(), xq.data(), mean0.data(), 0.0, use_con ? cmean0.data() : nullptr,
+                             0.0, values ? values->data() : nullptr, &best, &idx),
                     "lb_eci_argmax");
                 return std::make_pair(best, (long)idx);
             }
@@ -264,20 +231,15 @@ namespace limbo_b200 {
                 const std::vector<Eigen::VectorXd>& vs, std::vector<double>* values = nullptr) const
             {
                 if (values) values->resize(vs.size());
-                const long M = (long)vs.size();
                 const int D = (int)vs[0].size();
                 if (_samples.empty()) _push_prior(D);
                 if (other._samples.empty()) other._push_prior(D);
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), mean1((size_t)M);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                    mean1[(size_t)i] = other._mean_function(vs[i], other)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs),
+                                          mean1 = detail::first_means(other, vs);
                 double best = 0;
                 int64_t idx = 0;
                 const int64_t k = (int64_t)(front.size() / 2);
-                lb_check(lb_ehvi_argmax(_h, other._h, ref_point, k, k ? front.data() : nullptr, M, xq.data(), mean0.data(), 0.0,
+                lb_check(lb_ehvi_argmax(_h, other._h, ref_point, k, k ? front.data() : nullptr, (int64_t)vs.size(), xq.data(), mean0.data(), 0.0,
                              mean1.data(), 0.0, values ? values->data() : nullptr, &best, &idx),
                     "lb_ehvi_argmax");
                 return std::make_pair(best, (long)idx);
@@ -292,22 +254,16 @@ namespace limbo_b200 {
                 const std::vector<Eigen::VectorXd>& vs, std::vector<double>* values = nullptr) const
             {
                 if (values) values->resize(vs.size());
-                const long M = (long)vs.size();
                 const int D = (int)vs[0].size();
                 if (_samples.empty()) _push_prior(D);
                 if (m1._samples.empty()) m1._push_prior(D);
                 if (m2._samples.empty()) m2._push_prior(D);
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), mean1((size_t)M), mean2((size_t)M);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                    mean1[(size_t)i] = m1._mean_function(vs[i], m1)(0);
-                    mean2[(size_t)i] = m2._mean_function(vs[i], m2)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs),
+                                          mean1 = detail::first_means(m1, vs), mean2 = detail::first_means(m2, vs);
                 double best = 0;
                 int64_t idx = 0;
                 const int64_t k = (int64_t)(front.size() / 3);
-                lb_check(lb_ehvi3d_argmax(_h, m1._h, m2._h, r, k, k ? front.data() : nullptr, M, xq.data(), mean0.data(), 0.0,
+                lb_check(lb_ehvi3d_argmax(_h, m1._h, m2._h, r, k, k ? front.data() : nullptr, (int64_t)vs.size(), xq.data(), mean0.data(), 0.0,
                              mean1.data(), 0.0, mean2.data(), 0.0, values ? values->data() : nullptr, &best, &idx),
                     "lb_ehvi3d_argmax");
                 return std::make_pair(best, (long)idx);
@@ -328,17 +284,15 @@ namespace limbo_b200 {
                 grads = Eigen::MatrixXd::Zero((Eigen::Index)M, (Eigen::Index)D);
                 if (_samples.empty()) return;
                 const bool use_con = !con._samples.empty();
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), cmean0(use_con ? (size_t)M : 0), v((size_t)M), g((size_t)M * D);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                    if (use_con) cmean0[(size_t)i] = con._mean_function(vs[i], con)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs),
+                                          cmean0 = use_con ? detail::first_means(con, vs) : std::vector<double>();
+                std::vector<double> v((size_t)M), g((size_t)M * D);
                 double params[2] = {f_max, jitter};
                 lb_check(lb_eci_grad(_h, con._h, params, M, xq.data(), mean0.data(), 0.0, nullptr, use_con ? cmean0.data() : nullptr, 0.0,
                              nullptr, v.data(), g.data()),
                     "lb_eci_grad");
-                _unpack_grad(M, D, v, g, values, grads);
+                detail::unpack(v, values);
+                detail::unpack(g, M, D, grads);
             }
 
             // EHVI values (M) and gradients (M x D) with respect to the candidates in one device pass over both models (lb_ehvi_grad,
@@ -353,17 +307,15 @@ namespace limbo_b200 {
                 const int D = (int)vs[0].size();
                 if (_samples.empty()) _push_prior(D);
                 if (other._samples.empty()) other._push_prior(D);
-                std::vector<double> xq((size_t)M * D), mean0((size_t)M), mean1((size_t)M), v((size_t)M), g((size_t)M * D);
-                for (long i = 0; i < M; ++i) {
-                    for (int d = 0; d < D; ++d) xq[(size_t)i * D + d] = vs[i](d);
-                    mean0[(size_t)i] = _mean_function(vs[i], *this)(0);
-                    mean1[(size_t)i] = other._mean_function(vs[i], other)(0);
-                }
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs),
+                                          mean1 = detail::first_means(other, vs);
+                std::vector<double> v((size_t)M), g((size_t)M * D);
                 const int64_t k = (int64_t)(front.size() / 2);
                 lb_check(lb_ehvi_grad(_h, other._h, ref_point, k, k ? front.data() : nullptr, M, xq.data(), mean0.data(), 0.0, nullptr,
                              mean1.data(), 0.0, nullptr, v.data(), g.data()),
                     "lb_ehvi_grad");
-                _unpack_grad(M, D, v, g, values, grads);
+                detail::unpack(v, values);
+                detail::unpack(g, M, D, grads);
             }
 
             int dim_in() const { assert(_dim_in != -1); return _dim_in; }
@@ -594,15 +546,12 @@ namespace limbo_b200 {
                 for (int i = 0; i < own; ++i) p[(size_t)i] = hp(i);
                 lb_check(lb_set_kernel(_h, kernel_traits<KernelFunction>::id, p.data(), own, _kernel_function.noise()), "lb_set_kernel");
             }
-            // row-major device results (M values, M x D gradients) into Eigen
-            static void _unpack_grad(long M, int D, const std::vector<double>& v, const std::vector<double>& g, Eigen::VectorXd& values,
-                Eigen::MatrixXd& grads)
+            // adds the host mean functor's value at every candidate to mu (M x dim_out)
+            void _add_mean(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu) const
             {
-                values = Eigen::VectorXd((Eigen::Index)M);
-                grads = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                for (long i = 0; i < M; ++i) {
-                    values(i) = v[(size_t)i];
-                    for (int d = 0; d < D; ++d) grads(i, d) = g[(size_t)i * D + d];
+                for (size_t i = 0; i < vs.size(); ++i) {
+                    const Eigen::VectorXd mv = _mean_function(vs[i], *this);
+                    for (int p = 0; p < (int)mu.cols(); ++p) mu((Eigen::Index)i, p) += mv(p);
                 }
             }
             void _push_prior(int D) const

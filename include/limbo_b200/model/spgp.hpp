@@ -23,6 +23,7 @@
 #include <limbo/tools/macros.hpp>
 
 #include "../../limbo_b200.h"
+#include "batch_args.hpp"
 #include "mean_traits.hpp" // mean_is_input_free
 
 #ifndef LIMBO_MODEL_SPGP_HPP // the reference's header defines the same defaults
@@ -92,28 +93,22 @@ namespace limbo_b200 {
 
             std::tuple<Eigen::VectorXd, double> query(const Eigen::VectorXd& v) const // :193-197
             {
-                auto r = predict(_row(v));
-                return std::make_tuple(Eigen::VectorXd(r.first.row(0)), r.second(0, 0));
+                Eigen::MatrixXd mu;
+                Eigen::VectorXd s2;
+                query_batch(std::vector<Eigen::VectorXd>(1, v), mu, s2);
+                return std::make_tuple(Eigen::VectorXd(mu.row(0)), s2(0));
             }
             // :204-207 and _predict :582-610; xt holds one point per row
             std::pair<Eigen::MatrixXd, Eigen::MatrixXd> predict(const Eigen::MatrixXd& xt) const
             {
-                const int64_t nq = xt.rows();
-                Eigen::MatrixXd mu(nq, std::max(_dim_out, 1)), s2(nq, 1);
-                for (int64_t i = 0; i < nq; ++i) mu.row(i) = _mean_function(Eigen::VectorXd(xt.row(i)), *this).transpose();
-                if (_samples.empty()) {
-                    for (int64_t i = 0; i < nq; ++i) s2(i, 0) = _kernel_function(Eigen::VectorXd(xt.row(i)), Eigen::VectorXd(xt.row(i)));
-                    return {mu, s2};
-                }
-                std::vector<double> q((size_t)(nq * _dim_in)), m((size_t)nq), s((size_t)nq);
-                for (int64_t i = 0; i < nq; ++i)
-                    for (int d = 0; d < _dim_in; ++d) q[(size_t)(i * _dim_in + d)] = xt(i, d);
-                _check(lb_spgp_query(_h, nq, q.data(), _optimized ? 1 : 0, m.data(), s.data()), "lb_spgp_query");
-                for (int64_t i = 0; i < nq; ++i) {
-                    mu(i, 0) += m[(size_t)i];
-                    s2(i, 0) = s[(size_t)i];
-                }
-                return {mu, s2};
+                std::vector<Eigen::VectorXd> vs;
+                for (Eigen::Index i = 0; i < xt.rows(); ++i) vs.push_back(Eigen::VectorXd(xt.row(i)));
+                Eigen::MatrixXd mu;
+                Eigen::VectorXd s2;
+                query_batch(vs, mu, s2);
+                Eigen::MatrixXd s2m(s2.size(), 1);
+                for (Eigen::Index i = 0; i < s2.size(); ++i) s2m(i, 0) = s2(i);
+                return {mu, s2m};
             }
             Eigen::MatrixXd mu(const Eigen::MatrixXd& v) const { return predict(v).first; }
 
@@ -122,20 +117,24 @@ namespace limbo_b200 {
             // mu: M x dim_out (mean function included), sigma2: M
             void query_batch(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu, Eigen::VectorXd& sigma2) const
             {
-                Eigen::MatrixXd xt((Eigen::Index)vs.size(), (Eigen::Index)vs[0].size());
-                for (size_t i = 0; i < vs.size(); ++i)
-                    for (int d = 0; d < (int)vs[i].size(); ++d) xt((Eigen::Index)i, d) = vs[i](d);
-                auto r = predict(xt);
-                mu = r.first;
-                sigma2 = Eigen::VectorXd((Eigen::Index)vs.size());
-                for (size_t i = 0; i < vs.size(); ++i) sigma2((Eigen::Index)i) = r.second((Eigen::Index)i, 0);
+                const int64_t nq = (int64_t)vs.size();
+                mu = Eigen::MatrixXd(nq, std::max(_dim_out, 1));
+                for (int64_t i = 0; i < nq; ++i) mu.row(i) = _mean_function(vs[(size_t)i], *this).transpose();
+                if (_samples.empty()) {
+                    sigma2 = Eigen::VectorXd(nq);
+                    for (int64_t i = 0; i < nq; ++i) sigma2(i) = _kernel_function(vs[(size_t)i], vs[(size_t)i]);
+                    return;
+                }
+                std::vector<double> q = detail::pack_rows(vs), m((size_t)nq), s((size_t)nq);
+                _check(lb_spgp_query(_h, nq, q.data(), _optimized ? 1 : 0, m.data(), s.data()), "lb_spgp_query");
+                for (int64_t i = 0; i < nq; ++i) mu(i, 0) += m[(size_t)i];
+                detail::unpack(s, sigma2);
             }
             // fused UCB / EI + argmax on the device with the FirstElem aggregator (lb_spgp_acq_argmax)
             std::pair<double, long> acq_argmax(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs,
                 std::vector<double>* values = nullptr) const
             {
-                std::vector<double> xq, mean0;
-                _stage(vs, xq, mean0);
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs);
                 double params[2] = {p0, p1}, best = 0;
                 int64_t idx = 0;
                 if (values) values->resize(vs.size());
@@ -151,17 +150,13 @@ namespace limbo_b200 {
                 static_assert(mean_is_input_free<MeanFunction>::value, "acq_grad: the mean function has no input gradient");
                 const long M = (long)vs.size();
                 const int D = (int)vs[0].size();
-                std::vector<double> xq, mean0, v((size_t)M), g((size_t)M * D);
-                _stage(vs, xq, mean0);
+                const std::vector<double> xq = detail::pack_rows(vs), mean0 = detail::first_means(*this, vs);
+                std::vector<double> v((size_t)M), g((size_t)M * D);
                 double params[2] = {p0, p1};
                 _check(lb_spgp_acq_grad(_h, acq_id, params, M, xq.data(), _optimized ? 1 : 0, mean0.data(), 0.0, nullptr, v.data(), g.data()),
                     "lb_spgp_acq_grad");
-                values = Eigen::VectorXd((Eigen::Index)M);
-                grads = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                for (long i = 0; i < M; ++i) {
-                    values(i) = v[(size_t)i];
-                    for (int d = 0; d < D; ++d) grads(i, d) = g[(size_t)i * D + d];
-                }
+                detail::unpack(v, values);
+                detail::unpack(g, M, D, grads);
             }
             // mu (M x dim_out, mean added), sigma^2 (M) and their candidate gradients dmu, dsigma2 (M x D) in one device pass
             // (lb_spgp_query_grad)
@@ -171,22 +166,17 @@ namespace limbo_b200 {
                 static_assert(mean_is_input_free<MeanFunction>::value, "query_grad: the mean function has no input gradient");
                 const long M = (long)vs.size();
                 const int D = (int)vs[0].size(), P = std::max(_dim_out, 1);
-                std::vector<double> xq, mean0, m((size_t)M), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
-                _stage(vs, xq, mean0);
+                const std::vector<double> xq = detail::pack_rows(vs);
+                std::vector<double> m((size_t)M), s((size_t)M), gm((size_t)M * D), gs((size_t)M * D);
                 _check(lb_spgp_query_grad(_h, M, xq.data(), _optimized ? 1 : 0, m.data(), s.data(), gm.data(), gs.data()), "lb_spgp_query_grad");
                 mu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)P);
-                sigma2 = Eigen::VectorXd((Eigen::Index)M);
-                dmu = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
-                dsigma2 = Eigen::MatrixXd((Eigen::Index)M, (Eigen::Index)D);
                 for (long i = 0; i < M; ++i) {
                     mu.row(i) = _mean_function(vs[(size_t)i], *this).transpose();
                     mu(i, 0) += m[(size_t)i];
-                    sigma2(i) = s[(size_t)i];
-                    for (int d = 0; d < D; ++d) {
-                        dmu(i, d) = gm[(size_t)i * D + d];
-                        dsigma2(i, d) = gs[(size_t)i * D + d];
-                    }
                 }
+                detail::unpack(s, sigma2);
+                detail::unpack(gm, M, D, dmu);
+                detail::unpack(gs, M, D, dsigma2);
             }
             double sigma(const Eigen::VectorXd& v) const { return std::get<1>(query(v)); }
 
@@ -232,24 +222,7 @@ namespace limbo_b200 {
             {
                 if (rc != LB_OK) throw std::runtime_error(std::string(where) + ": " + lb_strerror(rc));
             }
-            static Eigen::MatrixXd _row(const Eigen::VectorXd& v)
-            {
-                Eigen::MatrixXd m(1, v.size());
-                for (int d = 0; d < (int)v.size(); ++d) m(0, d) = v(d);
-                return m;
-            }
             void _create() { _check(lb_spgp_create(&_h, 0), "lb_spgp_create"); }
-            // row-major candidates and the first component of the mean functor at each
-            void _stage(const std::vector<Eigen::VectorXd>& vs, std::vector<double>& xq, std::vector<double>& mean0) const
-            {
-                const size_t D = (size_t)vs[0].size();
-                xq.assign(vs.size() * D, 0.0);
-                mean0.assign(vs.size(), 0.0);
-                for (size_t i = 0; i < vs.size(); ++i) {
-                    for (size_t d = 0; d < D; ++d) xq[i * D + d] = vs[i]((Eigen::Index)d);
-                    mean0[i] = _mean_function(vs[i], *this)(0);
-                }
-            }
 
             void _init(const std::vector<Eigen::VectorXd>& samples, const std::vector<Eigen::VectorXd>& observations) // :353-379
             {

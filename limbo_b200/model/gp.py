@@ -15,10 +15,7 @@ import numpy as np
 from .. import _lib
 from .. import kernel as _kernel
 from .. import mean as _mean
-
-
-def _ptr(a: np.ndarray) -> int:
-    return a.ctypes.data
+from ._calls import acq_param_pair, argmax, candidates, first_mean, first_mean_and_grad, ptr, values_and_grads
 
 
 class GP:
@@ -93,7 +90,7 @@ class GP:
     def _push_kernel(self) -> None:
         k = self._kernel_function
         own = np.ascontiguousarray(k.params(), dtype=np.float64)
-        _lib.check(self._lib.lb_set_kernel(self._h, k.kernel_id, _ptr(own), own.size, k.noise()), "lb_set_kernel")
+        _lib.check(self._lib.lb_set_kernel(self._h, k.kernel_id, ptr(own), own.size, k.noise()), "lb_set_kernel")
 
     def _sample_matrix(self) -> np.ndarray:
         X = getattr(self, "_X", None)
@@ -105,7 +102,7 @@ class GP:
     def _push_data(self) -> None:
         X = self._sample_matrix()
         Y = np.asfortranarray(self._obs_mean, dtype=np.float64)
-        _lib.check(self._lib.lb_set_data(self._h, X.shape[0], X.shape[1], Y.shape[1], _ptr(X), _ptr(Y)), "lb_set_data")
+        _lib.check(self._lib.lb_set_data(self._h, X.shape[0], X.shape[1], Y.shape[1], ptr(X), ptr(Y)), "lb_set_data")
 
     # ---- gp.hpp:88-116 ----
     def compute(self, samples, observations, compute_kernel: bool = True) -> None:
@@ -174,99 +171,70 @@ class GP:
 
     def query_batch(self, Xq):
         """mu (M x P) and sigma^2 (M) for M candidates in one device pass."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
         P = max(self._dim_out, 1)
         if M == 0 or Xq.size == 0:
             return np.zeros((0, P)), np.zeros(0)
-        if len(self._samples) == 0:
-            # gp.hpp:161-163: mean(v) and k(v,v) + noise; the kernel state is still needed on the device
-            self._ensure_dims_for_prior(Xq.shape[1])
+        self._push_prior_if_empty(Xq.shape[1])
         mu = np.empty((M, P))
         s2 = np.empty(M)
-        _lib.check(self._lib.lb_query(self._h, M, _ptr(Xq), _ptr(mu), _ptr(s2)), "lb_query")
+        _lib.check(self._lib.lb_query(self._h, M, ptr(Xq), ptr(mu), ptr(s2)), "lb_query")
         mu += self._mean_function.batch(Xq, self)  # gp.hpp:615
         return mu, s2
 
-    def _ensure_dims_for_prior(self, d: int) -> None:
+    def _push_prior_if_empty(self, d: int) -> None:
+        # gp.hpp:161-163: without samples, mean(v) and k(v,v) + noise; the kernel state is still needed on the device
+        if len(self._samples) != 0:
+            return
         if self._dim_in != d:
             self._dim_in = d
             self._kernel_function = self._kernel_cls(self._params, d)
         if self._dim_out < 1:
             self._dim_out = 1
-        X = np.zeros((0, d))
-        Y = np.zeros((0, self._dim_out))
         _lib.check(self._lib.lb_set_data(self._h, 0, d, self._dim_out, None, None), "lb_set_data")
         self._push_kernel()
 
     def acq_argmax_batch(self, acq_id: int, acq_params, Xq, return_values: bool = False):
         """Fused batched acquisition + argmax on the device (FirstElem aggregator,
         bo_base.hpp:99-105).  Returns (best_value, best_index[, values])."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
-        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
-        if ap.size < 2:
-            ap = np.append(ap, 0.0)
-        mean0, mconst = self._first_mean(Xq)
-        mptr = _ptr(mean0) if mean0 is not None else None
-        vals = np.empty(M) if return_values else None
-        best = C.c_double()
-        idx = C.c_int64()
-        _lib.check(self._lib.lb_acq_argmax(self._h, acq_id, _ptr(ap), M, _ptr(Xq), mptr, mconst,
-                                           _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
-                   "lb_acq_argmax")
-        if return_values:
-            return best.value, idx.value, vals
-        return best.value, idx.value
+        ap = acq_param_pair(acq_params)
+        mean0, mconst = first_mean(self, Xq)
+        return argmax(self._lib, "lb_acq_argmax", M, return_values, self._h, acq_id, ptr(ap), M, ptr(Xq), ptr(mean0), mconst)
 
     def eci_argmax_batch(self, constraint_model, f_max: float, jitter: float, Xq, return_values: bool = False):
         """Fused batched expected constrained improvement + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem
         aggregator): this GP is the objective, `constraint_model` (a GP on the same device, or None for no constraints) gives
         Pf from its first output.  Returns (best_value, best_index[, values])."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
         ep = np.array([f_max, jitter], dtype=np.float64)
-        mean0, mconst = self._first_mean(Xq)
+        mean0, mconst = first_mean(self, Xq)
         con_h, cmean0, cconst = None, None, 0.0
         if constraint_model is not None:
             con_h = constraint_model._h
             if constraint_model.nb_samples() > 0:
-                cmean0, cconst = constraint_model._first_mean(Xq)
-        vals = np.empty(M) if return_values else None
-        best = C.c_double()
-        idx = C.c_int64()
-        _lib.check(self._lib.lb_eci_argmax(self._h, con_h, _ptr(ep), M, _ptr(Xq), _ptr(mean0) if mean0 is not None else None, mconst,
-                                           _ptr(cmean0) if cmean0 is not None else None, cconst,
-                                           _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
-                   "lb_eci_argmax")
-        if return_values:
-            return best.value, idx.value, vals
-        return best.value, idx.value
+                cmean0, cconst = first_mean(constraint_model, Xq)
+        return argmax(self._lib, "lb_eci_argmax", M, return_values, self._h, con_h, ptr(ep), M, ptr(Xq), ptr(mean0), mconst, ptr(cmean0),
+                      cconst)
 
     def ehvi_argmax_batch(self, other, ref_point, front, Xq, return_values: bool = False):
         """Fused batched two-objective expected hypervolume improvement + argmax on the device (experimental/acqui/ehvi.hpp:70-79,
         FirstElem aggregator): this GP models the first objective and `other` (a distinct GP on the same device) the second;
         front is the k x 2 array of current Pareto objective values, ref_point the reference point.  A model without samples
         scores with its prior.  Returns (best_value, best_index[, values])."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
         F = np.ascontiguousarray(np.asarray(front, dtype=np.float64).reshape(-1, 2))
         r = np.ascontiguousarray(np.asarray(ref_point, dtype=np.float64).reshape(-1)[:2])
         for g in (self, other):
-            if g.nb_samples() == 0:
-                g._ensure_dims_for_prior(Xq.shape[1])
-        mean0, c0 = self._first_mean(Xq)
-        mean1, c1 = other._first_mean(Xq)
-        vals = np.empty(M) if return_values else None
-        best = C.c_double()
-        idx = C.c_int64()
-        _lib.check(self._lib.lb_ehvi_argmax(self._h, other._h, _ptr(r), F.shape[0], _ptr(F) if F.size else None, M, _ptr(Xq),
-                                            _ptr(mean0) if mean0 is not None else None, c0, _ptr(mean1) if mean1 is not None else None,
-                                            c1, _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
-                   "lb_ehvi_argmax")
-        if return_values:
-            return best.value, idx.value, vals
-        return best.value, idx.value
+            g._push_prior_if_empty(Xq.shape[1])
+        mean0, c0 = first_mean(self, Xq)
+        mean1, c1 = first_mean(other, Xq)
+        return argmax(self._lib, "lb_ehvi_argmax", M, return_values, self._h, other._h, ptr(r), F.shape[0], ptr(F) if F.size else None, M,
+                      ptr(Xq), ptr(mean0), c0, ptr(mean1), c1)
 
     def ehvi3d_argmax_batch(self, m1, m2, ref_point, front, Xq, return_values: bool = False):
         """Fused batched three-objective expected hypervolume improvement + argmax on the device (ehvi3d_sliceupdate,
@@ -275,40 +243,28 @@ class GP:
         front is the k x 3 array of current Pareto objective values (k <= LB_EHVI3D_MAX_K = 256), ref_point the reference point
         (its first three entries are used).  A model without samples scores with its prior.  Returns (best_value,
         best_index[, values])."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
         F = np.ascontiguousarray(np.asarray(front, dtype=np.float64).reshape(-1, 3))
         r = np.ascontiguousarray(np.asarray(ref_point, dtype=np.float64).reshape(-1)[:3])
         for g in (self, m1, m2):
-            if g.nb_samples() == 0:
-                g._ensure_dims_for_prior(Xq.shape[1])
-        means = [g._first_mean(Xq) for g in (self, m1, m2)]
-        vals = np.empty(M) if return_values else None
-        best = C.c_double()
-        idx = C.c_int64()
-        args = []
-        for m, c in means:
-            args += [_ptr(m) if m is not None else None, c]
-        _lib.check(self._lib.lb_ehvi3d_argmax(self._h, m1._h, m2._h, _ptr(r), F.shape[0], _ptr(F) if F.size else None, M, _ptr(Xq),
-                                              *args, _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
-                   "lb_ehvi3d_argmax")
-        if return_values:
-            return best.value, idx.value, vals
-        return best.value, idx.value
+            g._push_prior_if_empty(Xq.shape[1])
+        means = [first_mean(g, Xq) for g in (self, m1, m2)]
+        return argmax(self._lib, "lb_ehvi3d_argmax", M, return_values, self._h, m1._h, m2._h, ptr(r), F.shape[0], ptr(F) if F.size else None,
+                      M, ptr(Xq), *[a for m, c in means for a in (ptr(m), c)])
 
     def query_grad_batch(self, Xq):
         """mu (M x P), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D, of the first output) and
         grad sigma^2 (M x D), in one device pass (lb_query_grad); the mean's value and input gradient are added.  Raises
         NotImplementedError for a mean without an input gradient (mean.BaseMean.grad_x)."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
         P = max(self._dim_out, 1)
         mgrad = self._mean_function.grad_x(Xq, self)
-        if len(self._samples) == 0:
-            self._ensure_dims_for_prior(D)
+        self._push_prior_if_empty(D)
         mu, s2 = np.empty((M, P)), np.empty(M)
         dmu, ds2 = np.empty((M, D)), np.empty((M, D))
-        _lib.check(self._lib.lb_query_grad(self._h, M, _ptr(Xq), _ptr(mu), _ptr(s2), _ptr(dmu), _ptr(ds2)), "lb_query_grad")
+        _lib.check(self._lib.lb_query_grad(self._h, M, ptr(Xq), ptr(mu), ptr(s2), ptr(dmu), ptr(ds2)), "lb_query_grad")
         mu += self._mean_function.batch(Xq, self)
         dmu += mgrad[:, 0, :]
         return mu, s2, dmu, ds2
@@ -316,69 +272,39 @@ class GP:
     def acq_grad_batch(self, acq_id: int, acq_params, Xq):
         """Acquisition values (M) and gradients (M x D) of UCB / GP_UCB (acq_id 0) or EI (acq_id 1) with the FirstElem aggregator,
         in one device pass (lb_acq_grad); parameters and values as acq_argmax_batch."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
-        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
-        if ap.size < 2:
-            ap = np.append(ap, 0.0)
-        mgrad = np.ascontiguousarray(self._mean_function.grad_x(Xq, self)[:, 0, :])
-        if len(self._samples) == 0:
-            self._ensure_dims_for_prior(D)
-        mean0, mconst = self._first_mean(Xq)
-        vals, grads = np.empty(M), np.empty((M, D))
-        _lib.check(self._lib.lb_acq_grad(self._h, acq_id, _ptr(ap), M, _ptr(Xq), _ptr(mean0) if mean0 is not None else None, mconst,
-                                         _ptr(mgrad) if np.any(mgrad) else None, _ptr(vals), _ptr(grads)), "lb_acq_grad")
-        return vals, grads
-
-    def _first_mean_and_grad(self, Xq):
-        """(mean array or None, mean constant, M x D input gradient of the mean's first output or None when it is 0); raises
-        NotImplementedError for a mean without an input gradient."""
-        mgrad = np.ascontiguousarray(self._mean_function.grad_x(Xq, self)[:, 0, :])
-        if len(self._samples) == 0:
-            self._ensure_dims_for_prior(Xq.shape[1])
-        mean0, mconst = self._first_mean(Xq)
-        return mean0, mconst, (mgrad if np.any(mgrad) else None)
+        ap = acq_param_pair(acq_params)
+        mean0, mconst, mgrad = first_mean_and_grad(self, Xq, self._push_prior_if_empty)
+        return values_and_grads(self._lib, "lb_acq_grad", M, D, self._h, acq_id, ptr(ap), M, ptr(Xq), ptr(mean0), mconst, ptr(mgrad))
 
     def eci_grad_batch(self, constraint_model, f_max: float, jitter: float, Xq):
         """ECI values (M) and gradients (M x D) with respect to the candidates, in one device pass over both models (lb_eci_grad);
         arguments and values as eci_argmax_batch.  The means' input gradients are added; NotImplementedError for a mean without one."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
         ep = np.array([f_max, jitter], dtype=np.float64)
-        mean0, mconst, mgrad = self._first_mean_and_grad(Xq)
+        mean0, mconst, mgrad = first_mean_and_grad(self, Xq, self._push_prior_if_empty)
         con_h, cmean0, cconst, cgrad = None, None, 0.0, None
         if constraint_model is not None:
             con_h = constraint_model._h
             if constraint_model.nb_samples() > 0:
-                cmean0, cconst, cgrad = constraint_model._first_mean_and_grad(Xq)
-        vals, grads = np.empty(M), np.empty((M, D))
-        _lib.check(self._lib.lb_eci_grad(self._h, con_h, _ptr(ep), M, _ptr(Xq), _ptr(mean0) if mean0 is not None else None, mconst,
-                                         _ptr(mgrad) if mgrad is not None else None, _ptr(cmean0) if cmean0 is not None else None,
-                                         cconst, _ptr(cgrad) if cgrad is not None else None, _ptr(vals), _ptr(grads)), "lb_eci_grad")
-        return vals, grads
+                cmean0, cconst, cgrad = first_mean_and_grad(constraint_model, Xq)
+        return values_and_grads(self._lib, "lb_eci_grad", M, D, self._h, con_h, ptr(ep), M, ptr(Xq), ptr(mean0), mconst, ptr(mgrad),
+                                ptr(cmean0), cconst, ptr(cgrad))
 
     def ehvi_grad_batch(self, other, ref_point, front, Xq):
         """Two-objective EHVI values (M) and gradients (M x D) with respect to the candidates, in one device pass over both models
         (lb_ehvi_grad); arguments and values as ehvi_argmax_batch.  The means' input gradients are added; NotImplementedError for a
         mean without one."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
         F = np.ascontiguousarray(np.asarray(front, dtype=np.float64).reshape(-1, 2))
         r = np.ascontiguousarray(np.asarray(ref_point, dtype=np.float64).reshape(-1)[:2])
-        mean0, c0, g0 = self._first_mean_and_grad(Xq)
-        mean1, c1, g1 = other._first_mean_and_grad(Xq)
-        vals, grads = np.empty(M), np.empty((M, D))
-        _lib.check(self._lib.lb_ehvi_grad(self._h, other._h, _ptr(r), F.shape[0], _ptr(F) if F.size else None, M, _ptr(Xq),
-                                          _ptr(mean0) if mean0 is not None else None, c0, _ptr(g0) if g0 is not None else None,
-                                          _ptr(mean1) if mean1 is not None else None, c1, _ptr(g1) if g1 is not None else None,
-                                          _ptr(vals), _ptr(grads)), "lb_ehvi_grad")
-        return vals, grads
-
-    def _first_mean(self, Xq):
-        """First output of the mean functor at every candidate, as (array, 0.0), or (None, constant) for a constant mean."""
-        if self._mean_function.is_constant():
-            return None, float(np.asarray(self._mean_function(Xq[0], self))[0])
-        return np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0]), 0.0
+        mean0, c0, g0 = first_mean_and_grad(self, Xq, self._push_prior_if_empty)
+        mean1, c1, g1 = first_mean_and_grad(other, Xq, other._push_prior_if_empty)
+        return values_and_grads(self._lib, "lb_ehvi_grad", M, D, self._h, other._h, ptr(r), F.shape[0], ptr(F) if F.size else None, M,
+                                ptr(Xq), ptr(mean0), c0, ptr(g0), ptr(mean1), c1, ptr(g1))
 
     # ---- accessors gp.hpp:194-238 ----
     def dim_in(self) -> int:
@@ -439,7 +365,7 @@ class GP:
     def compute_kernel_grad_log_lik(self) -> np.ndarray:
         k = self._kernel_function
         g = np.empty(k.h_params_size())
-        _lib.check(self._lib.lb_kernel_grad_log_lik(self._h, int(k.optimize_noise()), _ptr(g)), "lb_kernel_grad_log_lik")
+        _lib.check(self._lib.lb_kernel_grad_log_lik(self._h, int(k.optimize_noise()), ptr(g)), "lb_kernel_grad_log_lik")
         self._inv_kernel_updated = True
         return g
 
@@ -462,15 +388,15 @@ class GP:
         lik = np.empty(R)
         grad = np.empty((R, nh)) if compute_grad else None
         info = np.empty(R, dtype=np.int32)
-        _lib.check(self._lib.lb_lml_grad_batch(self._h, k.kernel_id, R, nk, _ptr(own), _ptr(noise), int(k.optimize_noise()), _ptr(lik),
-                                               _ptr(grad) if grad is not None else None, _ptr(info)), "lb_lml_grad_batch")
+        _lib.check(self._lib.lb_lml_grad_batch(self._h, k.kernel_id, R, nk, ptr(own), ptr(noise), int(k.optimize_noise()), ptr(lik),
+                                               ptr(grad), ptr(info)), "lb_lml_grad_batch")
         return lik, grad, info
 
     # ---- gp.hpp:313-330: obs_mean^T K^-1 on the device (lb_kinv_obs_mean); the mean functor's gradient is host code ----
     def compute_mean_grad_log_lik(self) -> np.ndarray:
         n = self.nb_samples()
         w = np.empty((n, self._dim_out), order="F")
-        _lib.check(self._lib.lb_kinv_obs_mean(self._h, _ptr(w)), "lb_kinv_obs_mean")
+        _lib.check(self._lib.lb_kinv_obs_mean(self._h, ptr(w)), "lb_kinv_obs_mean")
         self._inv_kernel_updated = True
         grad = np.zeros(self._mean_function.h_params_size())
         for n_obs in range(n):
@@ -491,7 +417,7 @@ class GP:
     def compute_kernel_grad_log_loo_cv(self) -> np.ndarray:
         k = self._kernel_function
         g = np.empty(k.h_params_size())
-        _lib.check(self._lib.lb_kernel_grad_log_loo_cv(self._h, int(k.optimize_noise()), _ptr(g)), "lb_kernel_grad_log_loo_cv")
+        _lib.check(self._lib.lb_kernel_grad_log_loo_cv(self._h, int(k.optimize_noise()), ptr(g)), "lb_kernel_grad_log_loo_cv")
         self._inv_kernel_updated = True
         return g
 
@@ -510,7 +436,7 @@ class GP:
     # ---- gp.hpp:404-436 ----
     def _get(self, what: int, shape) -> np.ndarray:
         out = np.empty(shape, order="F")
-        _lib.check(self._lib.lb_get(self._h, what, _ptr(out)), "lb_get")
+        _lib.check(self._lib.lb_get(self._h, what, ptr(out)), "lb_get")
         return out
 
     def matrixL(self) -> np.ndarray:
@@ -583,7 +509,7 @@ class GP:
             self._push_kernel()
             L = np.asfortranarray(archive.load_matrix("matrixL"))
             A = np.asfortranarray(archive.load_matrix("alpha").reshape(len(self._samples), self._dim_out))
-            _lib.check(self._lib.lb_load_factor(self._h, _ptr(L), _ptr(A)), "lb_load_factor")
+            _lib.check(self._lib.lb_load_factor(self._h, ptr(L), ptr(A)), "lb_load_factor")
             self._inv_kernel_updated = False
 
     # ---- protected helpers (same names as the reference) ----
@@ -616,7 +542,7 @@ class GP:
         self._push_kernel()  # unchanged functor state keeps the factor (lb_set_kernel compares)
         x = np.ascontiguousarray(self._samples[-1])
         Y = np.asfortranarray(self._obs_mean)
-        rc = self._lib.lb_append(self._h, _ptr(x), _ptr(Y))
+        rc = self._lib.lb_append(self._h, ptr(x), ptr(Y))
         if rc == -3:  # factor not resident (compute(..., compute_kernel=False) before, or the h-params changed since the fit)
             self._compute_full_kernel()
             return
@@ -627,7 +553,7 @@ class GP:
 
     def _compute_alpha(self) -> None:  # gp.hpp:605-611
         Y = np.asfortranarray(self._obs_mean)
-        rc = self._lib.lb_refit_alpha(self._h, _ptr(Y))
+        rc = self._lib.lb_refit_alpha(self._h, ptr(Y))
         if rc < 0:
             _lib.check(rc, "lb_refit_alpha")
 

@@ -20,10 +20,7 @@ from .. import kernel as _kernel
 from .. import mean as _mean
 from .. import opt as _opt
 from .. import params as _params
-
-
-def _ptr(a: np.ndarray) -> int:
-    return a.ctypes.data
+from ._calls import acq_param_pair, argmax, candidates, first_mean, first_mean_and_grad, ptr, values_and_grads
 
 
 class SPGP:
@@ -90,7 +87,7 @@ class SPGP:
         y_zm = np.ascontiguousarray(Y[:, 0] - self._mean_function.batch(X, self)[:, 0], dtype=np.float64)
         self._y_zm = y_zm
         self._update_m()
-        _lib.check(self._lib.lb_spgp_set_data(self._h, X.shape[0], X.shape[1], _ptr(X), _ptr(y_zm)), "lb_spgp_set_data")
+        _lib.check(self._lib.lb_spgp_set_data(self._h, X.shape[0], X.shape[1], ptr(X), ptr(y_zm)), "lb_spgp_set_data")
 
     def compute(self, samples, observations) -> None:  # spgp.hpp:132-152
         assert len(samples) != 0 and len(observations) != 0 and len(samples) == len(observations)
@@ -151,7 +148,7 @@ class SPGP:
     def compute_at(self, w) -> None:
         """_compute(false) at HyperParams(w): the factors the queries use."""
         w = np.ascontiguousarray(w, dtype=np.float64)
-        _lib.check(self._lib.lb_spgp_compute(self._h, self._m, w.size, _ptr(w), self.jitter()), "lb_spgp_compute")
+        _lib.check(self._lib.lb_spgp_compute(self._h, self._m, w.size, ptr(w), self.jitter()), "lb_spgp_compute")
         self._w = w.copy()
 
     def _likelihood(self, w, eval_grad: bool = False):
@@ -159,7 +156,7 @@ class SPGP:
         w = np.ascontiguousarray(w, dtype=np.float64)
         f = C.c_double()
         g = np.empty(w.size) if eval_grad else None
-        rc = self._lib.lb_spgp_lik(self._h, self._m, w.size, _ptr(w), self.jitter(), C.addressof(f), _ptr(g) if g is not None else None)
+        rc = self._lib.lb_spgp_lik(self._h, self._m, w.size, ptr(w), self.jitter(), C.addressof(f), ptr(g))
         if rc > 0:
             return -math.inf, (np.zeros(w.size) if eval_grad else None)
         _lib.check(rc, "lb_spgp_lik")
@@ -168,7 +165,7 @@ class SPGP:
     # ---- spgp.hpp:193-236, 582-610 ----
     def query_batch(self, Xq):
         """mu (Mq x 1) and sigma^2 (Mq) for Mq candidates in one device pass."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
         P = max(self._dim_out, 1)
         if M == 0:
@@ -178,7 +175,7 @@ class SPGP:
             return np.array(mean, dtype=np.float64), np.full(M, self._kernel_function.sigma_sq())
         mu = np.empty(M)
         s2 = np.empty(M)
-        _lib.check(self._lib.lb_spgp_query(self._h, M, _ptr(Xq), int(self._optimized), _ptr(mu), _ptr(s2)), "lb_spgp_query")
+        _lib.check(self._lib.lb_spgp_query(self._h, M, ptr(Xq), int(self._optimized), ptr(mu), ptr(s2)), "lb_spgp_query")
         out = np.array(mean, dtype=np.float64)
         out[:, 0] += mu
         return out, s2
@@ -198,37 +195,18 @@ class SPGP:
 
     def acq_argmax_batch(self, acq_id: int, acq_params, Xq, return_values: bool = False):
         """Batched acquisition + argmax on the device (FirstElem aggregator).  Returns (best_value, best_index[, values])."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M = Xq.shape[0]
-        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
-        if ap.size < 2:
-            ap = np.append(ap, 0.0)
-        if self._mean_function.is_constant():
-            mean0, mconst = None, float(np.asarray(self._mean_function(Xq[0], self))[0])
-        else:
-            mean0, mconst = np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0]), 0.0
-        vals = np.empty(M) if return_values else None
-        best = C.c_double()
-        idx = C.c_int64()
-        _lib.check(self._lib.lb_spgp_acq_argmax(self._h, acq_id, _ptr(ap), M, _ptr(Xq), int(self._optimized),
-                                                _ptr(mean0) if mean0 is not None else None, mconst,
-                                                _ptr(vals) if vals is not None else None, C.addressof(best), C.addressof(idx)),
-                   "lb_spgp_acq_argmax")
-        if return_values:
-            return best.value, idx.value, vals
-        return best.value, idx.value
-
-    def _first_mean(self, Xq):
-        """First output of the mean functor at every candidate, as (array, 0.0), or (None, constant) for a constant mean."""
-        if self._mean_function.is_constant():
-            return None, float(np.asarray(self._mean_function(Xq[0], self))[0])
-        return np.ascontiguousarray(self._mean_function.batch(Xq, self)[:, 0]), 0.0
+        ap = acq_param_pair(acq_params)
+        mean0, mconst = first_mean(self, Xq)
+        return argmax(self._lib, "lb_spgp_acq_argmax", M, return_values, self._h, acq_id, ptr(ap), M, ptr(Xq), int(self._optimized),
+                      ptr(mean0), mconst)
 
     def query_grad_batch(self, Xq):
         """mu (M x 1), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D) and grad sigma^2 (M x D), in
         one device pass (lb_spgp_query_grad); mu and sigma^2 are query_batch's.  The mean's value and input gradient are added;
         raises NotImplementedError for a mean without an input gradient (mean.BaseMean.grad_x)."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
         mgrad = self._mean_function.grad_x(Xq, self)
         mean = np.array(self._mean_function.batch(Xq, self), dtype=np.float64)
@@ -236,7 +214,7 @@ class SPGP:
             return mean, np.full(M, self._kernel_function.sigma_sq()), np.array(mgrad[:, 0, :], dtype=np.float64), np.zeros((M, D))
         mu, s2 = np.empty(M), np.empty(M)
         dmu, ds2 = np.empty((M, D)), np.empty((M, D))
-        _lib.check(self._lib.lb_spgp_query_grad(self._h, M, _ptr(Xq), int(self._optimized), _ptr(mu), _ptr(s2), _ptr(dmu), _ptr(ds2)),
+        _lib.check(self._lib.lb_spgp_query_grad(self._h, M, ptr(Xq), int(self._optimized), ptr(mu), ptr(s2), ptr(dmu), ptr(ds2)),
                    "lb_spgp_query_grad")
         mean[:, 0] += mu
         dmu += mgrad[:, 0, :]
@@ -246,18 +224,12 @@ class SPGP:
         """Acquisition values (M) and gradients (M x D) of UCB / GP_UCB (acq_id 0) or EI (acq_id 1) with the FirstElem aggregator,
         in one device pass (lb_spgp_acq_grad); parameters and values as acq_argmax_batch.  The mean's input gradient is added;
         raises NotImplementedError for a mean without one."""
-        Xq = np.ascontiguousarray(np.atleast_2d(Xq), dtype=np.float64)
+        Xq = candidates(Xq)
         M, D = Xq.shape
-        ap = np.ascontiguousarray(np.atleast_1d(acq_params), dtype=np.float64)
-        if ap.size < 2:
-            ap = np.append(ap, 0.0)
-        mgrad = np.ascontiguousarray(self._mean_function.grad_x(Xq, self)[:, 0, :])
-        mean0, mconst = self._first_mean(Xq)
-        vals, grads = np.empty(M), np.empty((M, D))
-        _lib.check(self._lib.lb_spgp_acq_grad(self._h, acq_id, _ptr(ap), M, _ptr(Xq), int(self._optimized),
-                                              _ptr(mean0) if mean0 is not None else None, mconst,
-                                              _ptr(mgrad) if np.any(mgrad) else None, _ptr(vals), _ptr(grads)), "lb_spgp_acq_grad")
-        return vals, grads
+        ap = acq_param_pair(acq_params)
+        mean0, mconst, mgrad = first_mean_and_grad(self, Xq)
+        return values_and_grads(self._lib, "lb_spgp_acq_grad", M, D, self._h, acq_id, ptr(ap), M, ptr(Xq), int(self._optimized), ptr(mean0),
+                                mconst, ptr(mgrad))
 
     def launch_count(self) -> int:
         return int(self._lib.lb_spgp_launch_count(self._h))
