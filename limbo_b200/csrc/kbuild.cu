@@ -11,11 +11,9 @@
 // value is evaluated once and written twice (tile and mirrored tile) with
 // 16-byte stores; noise + 1e-8 is fused on the diagonal; the padding region is
 // the identity.
-#include "common.cuh"
+#include "pair_tile.cuh"
 
 namespace {
-
-constexpr int DCH = 16; // input dimensions staged per pass
 
 __global__ void scale_x_kernel(const double* __restrict__ X, double* __restrict__ Xs, int64_t Np, KernParams kp)
 {
@@ -27,15 +25,6 @@ __global__ void scale_x_kernel(const double* __restrict__ X, double* __restrict_
     Xs[d * Np + i] = lb_staged_coord(kp, d, [&](int r) { return X[r * Np + i]; });
 }
 
-__device__ __forceinline__ void tile_from_index(int t, int& bi, int& bj)
-{
-    int r = (int)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
-    while ((int64_t)(r + 1) * (r + 2) / 2 <= t) ++r;
-    while ((int64_t)r * (r + 1) / 2 > t) --r;
-    bi = r;
-    bj = t - r * (r + 1) / 2;
-}
-
 // KID: kernel id (compile time, so only one functor is inlined); EDGE: the tile touches the diagonal or the identity
 // padding (noise / padding predicates); interior tiles (the vast majority) skip every per-element test.
 // NC: 8-column chunks per pass (8: two passes of 64 columns, 128 registers, two CTAs per SM; 4: four passes of 32 columns, fewer
@@ -43,61 +32,25 @@ __device__ __forceinline__ void tile_from_index(int t, int& bi, int& bj)
 // are bound by latency / issue, not by HBM, and want the extra warps)
 template <int KID, bool EDGE, int NC>
 __device__ __forceinline__ void kbuild_tile(const double* __restrict__ Xs, double* __restrict__ K, int64_t N, int64_t Np,
-    const KernParams& kp, int bi, int bj, double (*sxi)[LB_TILE], double (*sxj)[LB_TILE], uint64_t* barp)
+    const KernParams& kp, int bi, int bj, double (*sxi)[LB_TILE], double (*sxj)[LB_TILE], uint64_t* bar)
 {
-    uint64_t& bar = *barp;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int li = lane & 7, lj = lane >> 3;
-    const int D = kp.D;
     const int64_t i0 = (int64_t)bi * LB_TILE, j0 = (int64_t)bj * LB_TILE;
     const int r0 = warp * 16 + 2 * li; // local rows r0, r0+1
     const bool diag_tile = (bi == bj);
 
     if (tid == 0) {
-        lb_mbar_init(&bar, 1);
+        lb_mbar_init(bar, 1);
         lb_fence_barrier_init();
     }
     __syncthreads();
     uint32_t phase = 0;
-    const int npass = (D + DCH - 1) / DCH;
 
     constexpr int NH = 16 / NC, HW = 8 * NC; // passes over the 128 columns, columns per pass
     for (int h = 0; h < NH; ++h) {
         double z[NC][4];
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) z[c][e] = 0.0;
-
-        for (int pass = 0; pass < npass; ++pass) {
-            const int d0 = pass * DCH;
-            const int dc = min(DCH, D - d0);
-            if (!(npass == 1 && h >= 1)) { // single-pass inputs stay resident for the later column passes
-                __syncthreads();           // previous readers done before TMA overwrites
-                if (tid == 0) {
-                    lb_fence_proxy_async();
-                    lb_mbar_expect_tx(&bar, (uint32_t)(2 * dc * LB_TILE * sizeof(double)));
-                    for (int d = 0; d < dc; ++d) {
-                        lb_bulk_g2s(&sxi[d][0], Xs + (int64_t)(d0 + d) * Np + i0, LB_TILE * sizeof(double), &bar);
-                        lb_bulk_g2s(&sxj[d][0], Xs + (int64_t)(d0 + d) * Np + j0, LB_TILE * sizeof(double), &bar);
-                    }
-                }
-                lb_mbar_wait(&bar, phase);
-                phase ^= 1;
-            }
-            for (int d = 0; d < dc; ++d) {
-                const double2 xi = *reinterpret_cast<const double2*>(&sxi[d][r0]);
-#pragma unroll
-                for (int c = 0; c < NC; ++c) {
-                    const double2 xj = *reinterpret_cast<const double2*>(&sxj[d][h * HW + c * 8 + 2 * lj]);
-                    double q;
-                    q = xi.x - xj.x; z[c][0] = fma(q, q, z[c][0]);
-                    q = xi.y - xj.x; z[c][1] = fma(q, q, z[c][1]);
-                    q = xi.x - xj.y; z[c][2] = fma(q, q, z[c][2]);
-                    q = xi.y - xj.y; z[c][3] = fma(q, q, z[c][3]);
-                }
-            }
-        }
+        pair_distances<NC>(Xs, Np, i0, Xs, Np, j0, kp.D, sxi, sxj, bar, phase, h, z);
 
         const int64_t gi = i0 + r0; // global rows gi, gi+1
 #pragma unroll

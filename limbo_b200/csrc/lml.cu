@@ -9,10 +9,9 @@
 //                                   lower tiles of K^-1, k_ij and d k_ij / d theta recomputed from X
 //                                   (W = alpha alpha^T - K^-1 is never materialised)
 #include "gemm.cuh"
+#include "pair_tile.cuh"
 
 namespace {
-
-constexpr int DCH = 16;
 
 __global__ void __launch_bounds__(1024)
 loglik_kernel(const double* __restrict__ L, int64_t ld, int64_t N, const double* __restrict__ Y,
@@ -109,11 +108,8 @@ lauum_kernel(const double* __restrict__ X, int64_t ld, double* __restrict__ Kinv
 {
     extern __shared__ __align__(16) double smem[];
     // longest K ranges (small i) first: enumerate tiles so that i ascends
-    int t = blockIdx.x;
-    int r = (int)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
-    while ((int64_t)(r + 1) * (r + 2) / 2 <= t) ++r;
-    while ((int64_t)r * (r + 1) / 2 > t) --r;
-    const int i = r, j = t - r * (r + 1) / 2;
+    int i, j;
+    tile_from_index(blockIdx.x, i, j);
     lbg::Acc<lbg::CfgWide> acc;
     acc.zero();
     const int64_t k0 = (int64_t)i * LB_TILE;
@@ -139,15 +135,6 @@ __global__ void symmetrize_kernel(double* __restrict__ A, int64_t n)
     }
 }
 
-__device__ __forceinline__ void tile_from_index(int t, int& bi, int& bj)
-{
-    int r = (int)((sqrt(8.0 * (double)t + 1.0) - 1.0) * 0.5);
-    while ((int64_t)(r + 1) * (r + 2) / 2 <= t) ++r;
-    while ((int64_t)r * (r + 1) / 2 > t) --r;
-    bi = r;
-    bj = t - r * (r + 1) / 2;
-}
-
 // grad partials: part[tile][q], q < nh.
 //   sum_{i>=j} w_ij * dK_ij/dtheta_q * (1/2 if i==j)        gp.hpp:299-308
 //   w = alpha alpha^T - K^-1                                  gp.hpp:293-296
@@ -164,9 +151,8 @@ template <int KID, bool EDGE>
 __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const double* __restrict__ Kinv, const double* __restrict__ alpha, int P,
     int64_t N, int64_t Np, const KernParams& kp, int optimize_noise, int nh, double* __restrict__ part, int bi, int bj,
     double (*sxi)[LB_TILE], double (*sxj)[LB_TILE], double (*sai)[LB_TILE], double (*saj)[LB_TILE], double (*sred)[DCH + 4], double* stot,
-    uint64_t* barp)
+    uint64_t* bar)
 {
-    uint64_t& bar = *barp;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int li = lane & 7, lj = lane >> 3;
     const int D = kp.D;
@@ -174,7 +160,7 @@ __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const d
     const int r0 = warp * 16 + 2 * li;
     constexpr bool ard = (KID == LB_K_SE_ARD);
     if (tid == 0) {
-        lb_mbar_init(&bar, 1);
+        lb_mbar_init(bar, 1);
         lb_fence_barrier_init();
     }
     for (int q = tid; q < LB_MAX_D + 2; q += 256) stot[q] = 0.0;
@@ -188,30 +174,8 @@ __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const d
     uint32_t phase = 0;
     const int npass = (D + DCH - 1) / DCH;
 
-    auto stage = [&](int pass) {
-        const int d0 = pass * DCH;
-        const int dc = min(DCH, D - d0);
-        __syncthreads();
-        if (tid == 0) {
-            lb_fence_proxy_async();
-            lb_mbar_expect_tx(&bar, (uint32_t)(2 * dc * LB_TILE * sizeof(double)));
-            for (int d = 0; d < dc; ++d) {
-                lb_bulk_g2s(&sxi[d][0], Xs + (int64_t)(d0 + d) * Np + i0, LB_TILE * sizeof(double), &bar);
-                lb_bulk_g2s(&sxj[d][0], Xs + (int64_t)(d0 + d) * Np + j0, LB_TILE * sizeof(double), &bar);
-            }
-        }
-        lb_mbar_wait(&bar, phase);
-        phase ^= 1;
-        return dc;
-    };
-
     double g_sf = 0.0, g_l = 0.0, g_noise = 0.0;
     for (int h = 0; h < GNH; ++h) { // GNH passes of GHW columns
-        double z[GNC][4];
-#pragma unroll
-        for (int c = 0; c < GNC; ++c)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) z[c][e] = 0.0;
         // the K^-1 values of this half: issued before the distance sweep so that their latency hides under it
         const int64_t gi = i0 + r0;
         double2 kv[GNC][2];
@@ -221,23 +185,8 @@ __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const d
             kv[c][0] = __ldcs(reinterpret_cast<const double2*>(&Kinv[gi + gj * Np]));
             kv[c][1] = __ldcs(reinterpret_cast<const double2*>(&Kinv[gi + (gj + 1) * Np]));
         }
-        for (int pass = 0; pass < npass; ++pass) {
-            int dc = D;
-            if (!(npass == 1 && h >= 1)) dc = stage(pass);
-            else dc = min(DCH, D);
-            for (int d = 0; d < dc; ++d) {
-                const double2 xi = *reinterpret_cast<const double2*>(&sxi[d][r0]);
-#pragma unroll
-                for (int c = 0; c < GNC; ++c) {
-                    const double2 xj = *reinterpret_cast<const double2*>(&sxj[d][h * GHW + c * 8 + 2 * lj]);
-                    double q;
-                    q = xi.x - xj.x; z[c][0] = fma(q, q, z[c][0]);
-                    q = xi.y - xj.x; z[c][1] = fma(q, q, z[c][1]);
-                    q = xi.x - xj.y; z[c][2] = fma(q, q, z[c][2]);
-                    q = xi.y - xj.y; z[c][3] = fma(q, q, z[c][3]);
-                }
-            }
-        }
+        double z[GNC][4];
+        pair_distances<GNC>(Xs, Np, i0, Xs, Np, j0, D, sxi, sxj, bar, phase, h, z);
         // weights w_ij * f_ij and the parameter-independent factors
         double wk[GNC][4]; // SE-ARD: w * f * k
 #pragma unroll
@@ -275,7 +224,7 @@ __device__ __forceinline__ void grad_tile(const double* __restrict__ Xs, const d
             // second sweep over the input dimensions: g_d += w k q_d^2
             for (int pass = 0; pass < npass; ++pass) {
                 int dc;
-                if (npass > 1) dc = stage(pass);
+                if (npass > 1) dc = pair_stage(Xs, Np, i0, Xs, Np, j0, D, pass, sxi, sxj, bar, phase);
                 else dc = D;
                 const int d0 = pass * DCH;
                 double gd[DCH];

@@ -8,11 +8,10 @@
 //   acqui::UCB / GP_UCB / EI (acqui/ucb.hpp:83-90, gp_ucb.hpp:96-103, ei.hpp:85-116)
 //                                           -> acq_kernel + argmax reduction
 #include "gemm.cuh"
+#include "pair_tile.cuh"
 #include <cfloat>
 
 namespace {
-
-constexpr int DCH = 16;
 
 // K*[n, m] = k(x_n, q_m), no noise (kernel.hpp:81-84 with i=-1, j=-2).
 // grid: (Np/128, Mp/128); V is Np x Mp column-major (ld = Np).
@@ -25,7 +24,6 @@ kstar_kernel(const double* __restrict__ Xs, int64_t Np, int64_t N, const double*
     __shared__ __align__(8) uint64_t bar;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int li = lane & 7, lj = lane >> 3;
-    const int D = kp.D;
     const int64_t i0 = (int64_t)blockIdx.x * LB_TILE, j0 = (int64_t)blockIdx.y * LB_TILE;
     const int r0 = warp * 16 + 2 * li;
     if (tid == 0) {
@@ -34,42 +32,9 @@ kstar_kernel(const double* __restrict__ Xs, int64_t Np, int64_t N, const double*
     }
     __syncthreads();
     uint32_t phase = 0;
-    const int npass = (D + DCH - 1) / DCH;
     for (int h = 0; h < 2; ++h) {
         double z[8][4];
-#pragma unroll
-        for (int c = 0; c < 8; ++c)
-#pragma unroll
-            for (int e = 0; e < 4; ++e) z[c][e] = 0.0;
-        for (int pass = 0; pass < npass; ++pass) {
-            const int d0 = pass * DCH;
-            const int dc = min(DCH, D - d0);
-            if (!(npass == 1 && h == 1)) {
-                __syncthreads();
-                if (tid == 0) {
-                    lb_fence_proxy_async();
-                    lb_mbar_expect_tx(&bar, (uint32_t)(2 * dc * LB_TILE * sizeof(double)));
-                    for (int d = 0; d < dc; ++d) {
-                        lb_bulk_g2s(&sxi[d][0], Xs + (int64_t)(d0 + d) * Np + i0, LB_TILE * sizeof(double), &bar);
-                        lb_bulk_g2s(&sxj[d][0], Qs + (int64_t)(d0 + d) * Mp + j0, LB_TILE * sizeof(double), &bar);
-                    }
-                }
-                lb_mbar_wait(&bar, phase);
-                phase ^= 1;
-            }
-            for (int d = 0; d < dc; ++d) {
-                const double2 xi = *reinterpret_cast<const double2*>(&sxi[d][r0]);
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const double2 xj = *reinterpret_cast<const double2*>(&sxj[d][h * 64 + c * 8 + 2 * lj]);
-                    double q;
-                    q = xi.x - xj.x; z[c][0] = fma(q, q, z[c][0]);
-                    q = xi.y - xj.x; z[c][1] = fma(q, q, z[c][1]);
-                    q = xi.x - xj.y; z[c][2] = fma(q, q, z[c][2]);
-                    q = xi.y - xj.y; z[c][3] = fma(q, q, z[c][3]);
-                }
-            }
-        }
+        pair_distances<8>(Xs, Np, i0, Qs, Mp, j0, kp.D, sxi, sxj, &bar, phase, h, z);
         const int64_t gi = i0 + r0;
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
