@@ -242,6 +242,37 @@ int lb_ehvi3d_argmax_dev(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, cons
     const double* dMean1_at_q, double mean1_const, const double* dMean2_at_q, double mean2_const, double* dAcq_out, double* dBest_val,
     int64_t* dBest_idx);
 
+/* Batched CMA-ES acquisition optimiser (DESIGN.md §4.15): R independent (mu/mu_w, lambda)-CMA-ES instances with the active
+ * covariance update, in the default setting of Hansen's tutorial (arXiv:1604.00772, Table 1), sampling through the Cholesky
+ * factor of C.  It is not a port of libcmaes (the reference's opt::Cmaes).  One generation of every instance is one batched
+ * scoring of R * lambda candidates on the device; ask, score and tell are stream-ordered and the host reads one word every 8
+ * generations.  Instance r starts from starts[r] (row-major R x D); bounded searches run in [0, 1]^D through Hansen's
+ * linear-quadratic box transform.  An instance stops after `generations` generations, when sigma sqrt(max diag C) < tolx, or when
+ * the factorisation of C fails.  Returns the best point scored over every instance and generation (best_x, D values), its value
+ * (ties to the lower instance, within an instance to the earlier generation) and the number of candidates scored (n_evals).  The draws come from
+ * u(i) = (splitmix64(seed + i) >> 11) 2^-53, so a seed gives the same bits on every run. */
+typedef struct lb_cmaes_opts {
+    int lambda;       /* offspring per instance, <= 256; <= 0: 4 + floor(3 ln D) */
+    double sigma0;    /* initial step size, > 0 (the reference's opt::Cmaes: 0.5) */
+    int generations;  /* generations per instance, > 0 */
+    double tolx;      /* > 0 */
+    uint64_t seed;
+    int bounded;      /* nonzero: [0, 1]^D; zero: unbounded */
+} lb_cmaes_opts;
+
+/* lb_acq_argmax's UCB / GP_UCB / EI (acq_id, acq_params) with an input-free mean (mean_const added to every mu).  Any precision
+ * mode; LB_ERR_TIMEOUT when a reduced-precision scoring pass of any generation timed out.  h is locked for the whole search.
+ * LB_ERR_ARG for a NULL argument, R <= 0, a non-finite start, sigma0 or tolx <= 0, generations <= 0 or an unknown acq_id;
+ * LB_ERR_UNSUPPORTED for D > 64 or lambda > 256; LB_ERR_STATE for a handle without a kernel.  Synchronises h's stream. */
+int lb_acq_cmaes(const lb_gp* h, int acq_id, const double* acq_params, double mean_const, const lb_cmaes_opts* opts, int64_t R,
+    const double* starts_rowmajor, double* best_x, double* best_val, int64_t* n_evals);
+/* two-objective (m2 NULL, lb_ehvi_argmax, k x 2 front) or three-objective (lb_ehvi3d_argmax, k x 3 front) EHVI with input-free
+ * means; the argument and lock rules of those calls (every handle is locked for the whole search), and lb_acq_cmaes's.  The
+ * three-objective front pass runs once per search. */
+int lb_ehvi_cmaes(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, const double* ref_point, int64_t k, const double* front_rowmajor,
+    double mean0_const, double mean1_const, double mean2_const, const lb_cmaes_opts* opts, int64_t R, const double* starts_rowmajor,
+    double* best_x, double* best_val, int64_t* n_evals);
+
 /* pareto::impl::pareto_set_std (experimental/tools/pareto.hpp:138-162) over n points of K objectives (row-major n x K): the
  * indices of the points no other point dominates (dominate_flag == 1), duplicates kept, in compare_objs_lex order
  * (lexicographically descending, exact ties by ascending index).  Runs on h's device and stream under h's query lock; h's model

@@ -19,7 +19,8 @@
 // value is ehvi3d_sliceupdate (src/ehvi/ehvi_sliceupdate.cc) at (mu_i(v)[0]) and (sigma_i(v)), read from pop's f[0..2] and
 // ref_point(0..2).  A BatchRequest is answered with one lb_ehvi3d_argmax, and a point outside a batch is a batch of one.  The
 // GradRequest is left unanswered (there is no three-objective gradient on the device), so limbo_b200::opt::BatchedGradient stops
-// after scoring its start points (batched_gradient.hpp:103).  Aggregators that do not act like FirstElem run the reference's
+// after scoring its start points (batched_gradient.hpp:103); limbo_b200::opt::BatchedCmaes climbs it instead: with two or three
+// models and input-free means, its CmaesRequest is answered by one lb_ehvi_cmaes.  Aggregators that do not act like FirstElem run the reference's
 // ehvi3d_sliceupdate on the host, one point at a time: an aggregator type other than limbo::FirstElem instantiates that path, and
 // then src/ehvi/ehvi_sliceupdate.cc must be linked too (with FirstElem it is never referenced).
 //
@@ -71,6 +72,7 @@ namespace limbo {
                             greq->answered = true;
                         }
                     }
+                    _answer_cmaes(r, front, nullptr);
                     limbo_b200::opt::BatchRequest* req = limbo_b200::opt::current_batch();
                     limbo_b200::acqui::detail::answer_batch([&](const std::vector<Eigen::VectorXd>& c) {
                         return _models[0].ehvi_argmax(_models[1], r, front, c, req ? req->values : nullptr);
@@ -103,6 +105,7 @@ namespace limbo {
                     }
                 }
                 const std::vector<double> front = _front(3);
+                _answer_cmaes(r, front, &_models[2]);
                 limbo_b200::opt::BatchRequest* req = limbo_b200::opt::current_batch();
                 limbo_b200::acqui::detail::answer_batch([&](const std::vector<Eigen::VectorXd>& c) {
                     return _models[0].ehvi3d_argmax(_models[1], _models[2], r, front, c, req ? req->values : nullptr);
@@ -112,6 +115,16 @@ namespace limbo {
 
             // means that do not depend on the input: gradients from lb_ehvi_grad
             static constexpr bool has_grad = limbo_b200::acqui::detail::has_candidate_grad<Model>::value;
+
+            // BatchedCmaes's start points: one lb_ehvi_cmaes over two (m2 NULL) or three models (means that do not depend on the input)
+            void _answer_cmaes(const double* r, const std::vector<double>& front, const Model* m2) const
+            {
+                if constexpr (limbo_b200::acqui::detail::has_device_cmaes<Model>::value)
+                    limbo_b200::acqui::detail::answer_cmaes(
+                        [&](const std::vector<Eigen::VectorXd>& st, const lb_cmaes_opts& o, Eigen::VectorXd& x, int64_t& n) {
+                            return _models[0].ehvi_cmaes(_models[1], m2, r, front, st, o, x, n);
+                        });
+            }
 
             const std::vector<Model>& _models;
             const std::deque<individual*>& _pop;

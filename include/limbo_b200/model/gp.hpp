@@ -269,6 +269,44 @@ namespace limbo_b200 {
                 return std::make_pair(best, (long)idx);
             }
 
+            // Batched CMA-ES on the device (lb_acq_cmaes) over UCB / EI (acq_id, p0, p1 as acq_argmax), one instance from each start;
+            // the mean must not depend on the input (its first output is passed as a constant).  Returns the best value; best_x and
+            // n_evals (candidates scored) are filled in.
+            double acq_cmaes(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& starts, const lb_cmaes_opts& opts,
+                Eigen::VectorXd& best_x, int64_t& n_evals) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "acq_cmaes: the mean function depends on the input");
+                const int D = (int)starts[0].size();
+                if (_samples.empty()) _push_prior(D);
+                const std::vector<double> st = detail::pack_rows(starts);
+                double params[2] = {p0, p1}, best = 0;
+                best_x.resize(D);
+                lb_check(lb_acq_cmaes(_h, acq_id, params, _mean_const(D), &opts, (int64_t)starts.size(), st.data(), best_x.data(), &best,
+                             &n_evals),
+                    "lb_acq_cmaes");
+                return best;
+            }
+            // Batched CMA-ES on the device (lb_ehvi_cmaes) over the EHVI of ehvi_argmax (m2 == nullptr, front k x 2) or of
+            // ehvi3d_argmax (front k x 3); arguments and results as acq_cmaes.
+            template <typename GP1, typename GP2>
+            double ehvi_cmaes(const GP1& m1, const GP2* m2, const double* r, const std::vector<double>& front,
+                const std::vector<Eigen::VectorXd>& starts, const lb_cmaes_opts& opts, Eigen::VectorXd& best_x, int64_t& n_evals) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "ehvi_cmaes: the mean function depends on the input");
+                const int D = (int)starts[0].size();
+                if (_samples.empty()) _push_prior(D);
+                if (m1._samples.empty()) m1._push_prior(D);
+                if (m2 && m2->_samples.empty()) m2->_push_prior(D);
+                const std::vector<double> st = detail::pack_rows(starts);
+                const int64_t k = (int64_t)(front.size() / (m2 ? 3 : 2));
+                double best = 0;
+                best_x.resize(D);
+                lb_check(lb_ehvi_cmaes(_h, m1._h, m2 ? m2->_h : nullptr, r, k, k ? front.data() : nullptr, _mean_const(D), m1._mean_const(D),
+                             m2 ? m2->_mean_const(D) : 0.0, &opts, (int64_t)starts.size(), st.data(), best_x.data(), &best, &n_evals),
+                    "lb_ehvi_cmaes");
+                return best;
+            }
+
             // ECI values (M) and gradients (M x D) with respect to the candidates in one device pass over both models (lb_eci_grad,
             // FirstElem aggregator): arguments and values as eci_argmax.  Without objective samples both are 0 (eci.hpp:86).
             template <typename ConstraintGP>
@@ -554,6 +592,8 @@ namespace limbo_b200 {
                     for (int p = 0; p < (int)mu.cols(); ++p) mu((Eigen::Index)i, p) += mv(p);
                 }
             }
+            // first output of an input-free mean (lb_acq_cmaes / lb_ehvi_cmaes take it as a constant)
+            double _mean_const(int D) const { return _mean_function(Eigen::VectorXd::Zero(D), *this)(0); }
             void _push_prior(int D) const
             {
                 lb_check(lb_set_data(_h, 0, D, _dim_out > 0 ? _dim_out : 1, nullptr, nullptr), "lb_set_data");

@@ -83,6 +83,23 @@ namespace limbo_b200 {
             return req;
         }
 
+        // The start points announced by BatchedCmaes (opt/batched_cmaes.hpp) for one call of f: a batch-aware UCB / EI over
+        // limbo_b200::model::GP, or the acqui::Ehvi specialisation (acqui/ehvi.hpp), runs one device CMA-ES from them
+        // (lb_acq_cmaes / lb_ehvi_cmaes) and files its best point, value and evaluations.  Means must not depend on the input.
+        struct CmaesRequest {
+            const std::vector<Eigen::VectorXd>* starts = nullptr;
+            lb_cmaes_opts opts{};
+            bool answered = false;
+            Eigen::VectorXd best_x;
+            double best_value = 0.0;
+            int64_t n_evals = 0;
+        };
+        inline CmaesRequest*& current_cmaes()
+        {
+            static thread_local CmaesRequest* req = nullptr;
+            return req;
+        }
+
         template <typename Params>
         struct BatchedRandom {
             // opt/optimizer.hpp:84-96: maximise f from `init`; bounded = search inside [0, 1]^D
@@ -181,6 +198,22 @@ namespace limbo_b200 {
                 model.acq_grad(acq_id, p0, p1, *req->points, req->values, req->grads);
                 req->answered = true;
             }
+            // runs the pending CmaesRequest, if any, through run(starts, opts, best_x, n_evals) -> best value
+            template <typename Run>
+            inline void answer_cmaes(const Run& run)
+            {
+                opt::CmaesRequest* req = opt::current_cmaes();
+                if (!req || req->answered || !req->starts || req->starts->empty()) return;
+                req->best_value = run(*req->starts, req->opts, req->best_x, req->n_evals);
+                req->answered = true;
+            }
+            template <typename Model>
+            inline void answer_cmaes(const Model& model, int acq_id, double p0, double p1)
+            {
+                answer_cmaes([&](const std::vector<Eigen::VectorXd>& st, const lb_cmaes_opts& o, Eigen::VectorXd& x, int64_t& n) {
+                    return model.acq_cmaes(acq_id, p0, p1, st, o, x, n);
+                });
+            }
             // value and gradient at one point from one lb_acq_grad call
             template <typename Model>
             inline limbo::opt::eval_t one_point_grad(const Model& model, int acq_id, double p0, double p1, const Eigen::VectorXd& v)
@@ -199,6 +232,10 @@ namespace limbo_b200 {
             struct has_candidate_grad<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
             template <typename P, typename K, typename Mf, typename H>
             struct has_candidate_grad<model::SPGP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
+            // a device GP with an input-free mean: the device CMA-ES (lb_acq_cmaes, lb_ehvi_cmaes) takes it
+            template <typename M> struct has_device_cmaes : std::false_type {};
+            template <typename P, typename K, typename Mf, typename H>
+            struct has_device_cmaes<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
         }
 
         // acqui::UCB (acqui/ucb.hpp:83-90), batch-aware
@@ -222,6 +259,9 @@ namespace limbo_b200 {
                 }
                 else
                     assert(!gradient);
+                if constexpr (detail::has_device_cmaes<Model>::value)
+                    if (opt::current_cmaes() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                        detail::answer_cmaes(_model, LB_ACQ_UCB, Params::acqui_ucb::alpha(), 0.0);
                 if (opt::current_batch() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
                     detail::answer_batch(_model, LB_ACQ_UCB, Params::acqui_ucb::alpha(), 0.0);
                     if (!detail::has_candidate_grad<Model>::value) opt::current_batch()->gradients = false;
@@ -272,6 +312,9 @@ namespace limbo_b200 {
                     if (opt::current_grad_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
                         detail::answer_grad_batch(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter());
                 }
+                if constexpr (detail::has_device_cmaes<Model>::value)
+                    if (opt::current_cmaes() && detail::acts_like_first_elem(afun, (int)_model.dim_out()))
+                        detail::answer_cmaes(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter());
                 if (opt::current_batch() && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
                     detail::answer_batch(_model, LB_ACQ_EI, _f_max, Params::acqui_ei::jitter());
                     if (!detail::has_candidate_grad<Model>::value) opt::current_batch()->gradients = false;

@@ -17,13 +17,20 @@ ACQ_UCB, ACQ_EI = 0, 1
 GET_K, GET_L, GET_ALPHA, GET_KINV = 0, 1, 2, 3
 EHVI_MAX_K, PARETO_MAX_K = 4096, 8  # LB_EHVI_MAX_K, LB_PARETO_MAX_K
 LML_BATCH_MAX_N = 200  # LB_LML_BATCH_MAX_N
+CMAES_MAX_D, CMAES_MAX_LAMBDA = 64, 256
+
+
+class CmaesOpts(C.Structure):
+    """lb_cmaes_opts"""
+    _fields_ = [("lambda_", C.c_int), ("sigma0", C.c_double), ("generations", C.c_int), ("tolx", C.c_double), ("seed", C.c_uint64),
+                ("bounded", C.c_int)]
 
 # every symbol include/limbo_b200.h declares
 DECLARED_SYMBOLS = [
     "lb_create", "lb_destroy", "lb_clone", "lb_set_stream", "lb_sync", "lb_launch_count", "lb_set_data",
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
     "lb_acq_argmax", "lb_acq_argmax_dev", "lb_query_grad", "lb_query_grad_dev", "lb_acq_grad", "lb_acq_grad_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_eci_grad", "lb_eci_grad_dev", "lb_ehvi_argmax", "lb_ehvi_argmax_dev",
-    "lb_ehvi3d_argmax", "lb_ehvi3d_argmax_dev",
+    "lb_ehvi3d_argmax", "lb_ehvi3d_argmax_dev", "lb_acq_cmaes", "lb_ehvi_cmaes",
     "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_lml_grad_batch", "lb_lml_grad_batch_dev", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
     "lb_nb_samples", "lb_strerror", "lb_last_cuda_error", "lb_spgp_create", "lb_spgp_destroy", "lb_spgp_set_data", "lb_spgp_lik",
@@ -97,6 +104,10 @@ def load() -> C.CDLL:
         "lb_ehvi_argmax_dev": ([p, p, dp, i64, dp, i64, dp, dp, dbl, dp, dbl, dp, dp, dp], i32),
         "lb_ehvi3d_argmax": ([p, p, p, dp, i64, dp, i64, dp, dp, dbl, dp, dbl, dp, dbl, dp, dp, dp], i32),
         "lb_ehvi3d_argmax_dev": ([p, p, p, dp, i64, dp, i64, dp, dp, dbl, dp, dbl, dp, dbl, dp, dp, dp], i32),
+        "lb_acq_cmaes": ([p, i32, dp, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
+        "lb_ehvi_cmaes": ([p, p, p, dp, i64, dp, dbl, dbl, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
+        "lb_debug_cmaes_capture": ([i32], i32),
+        "lb_debug_cmaes_trace": ([dp, C.c_longlong], C.c_longlong),
         "lb_eci_grad": ([p, p, dp, i64, dp, dp, dbl, dp, dp, dbl, dp, dp, dp], i32),
         "lb_eci_grad_dev": ([p, p, dp, i64, dp, dp, dbl, dp, dp, dbl, dp, dp, dp], i32),
         "lb_ehvi_grad": ([p, p, dp, i64, dp, i64, dp, dp, dbl, dp, dp, dbl, dp, dp, dp], i32),

@@ -41,6 +41,10 @@ class UCB:
         """values (M) and gradients (M x D) at M candidates in one device pass"""
         return self._model.acq_grad_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], Xq)
 
+    def cmaes_batch(self, starts, **opts):
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (model.GP.acq_cmaes_batch)"""
+        return self._model.acq_cmaes_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], starts, **opts)
+
 
 def _one_point_grad(acqui, v, afun):
     assert afun is first_elem
@@ -113,6 +117,15 @@ class EI(_Improvement):
             return np.zeros(len(Xq)), np.zeros(Xq.shape)
         self._update_f_max(first_elem)
         return self._model.acq_grad_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], Xq)
+
+    def cmaes_batch(self, starts, **opts):
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (model.GP.acq_cmaes_batch); before
+        the model has samples every value is 0 and the first start is returned"""
+        starts = np.atleast_2d(starts)
+        if len(self._model.samples()) < 1:
+            return np.array(starts[0], dtype=np.float64), 0.0, 0
+        self._update_f_max(first_elem)
+        return self._model.acq_cmaes_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], starts, **opts)
 
 
 class ECI(_Improvement):
@@ -204,3 +217,8 @@ class EHVI:
         if len(self._models) == 3:
             raise NotImplementedError("the three-objective EHVI has no gradient on the device")
         return self._models[0].ehvi_grad_batch(self._models[1], self._ref_point, self._pop, Xq)
+
+    def cmaes_batch(self, starts, **opts):
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts, over two or three objectives
+        (model.GP.ehvi_cmaes_batch)"""
+        return self._models[0].ehvi_cmaes_batch(self._models[1:], self._ref_point, self._pop, starts, **opts)

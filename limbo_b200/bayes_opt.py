@@ -28,6 +28,16 @@ class defaults_bo:
         iterations = 30
         alpha = 0.01
 
+    class opt_batchedcmaes:  # DESIGN.md §4.15 gives the measurement behind these
+        candidates = 10000
+        starts = 32
+        # "lambda" is a Python keyword: read with getattr
+        sigma = 0.1
+        generations = 50
+        tolx = 1e-6
+
+setattr(defaults_bo.opt_batchedcmaes, "lambda", 0)
+
 
 def _get(params, section, name):
     sec = getattr(params, section, None) if params is not None else None
@@ -66,6 +76,20 @@ class BatchedRandomSearch:
         return x
 
 
+def _best_distinct(cand, vals, n: int) -> np.ndarray:
+    """the (at most) n best distinct rows of cand by vals, descending, NaN last"""
+    order = np.argsort(-np.nan_to_num(np.asarray(vals), nan=-np.inf), kind="stable")
+    chosen, seen = [], set()
+    for i in order:
+        key = cand[i].tobytes()
+        if key not in seen:
+            seen.add(key)
+            chosen.append(i)
+        if len(chosen) == n:
+            break
+    return cand[chosen].copy()
+
+
 class BatchedGradientSearch:
     """acquiopt<> policy: one random pass of `candidates` uniform points in [0,1]^D scored in one device pass, then the best
     `starts` distinct points climb the acquisition in lockstep for `iterations` steps of Adam with the reference's update
@@ -90,16 +114,7 @@ class BatchedGradientSearch:
         grad_batch = getattr(acqui, "grad_batch", None)
         if grad_batch is None:
             return x_best
-        order = np.argsort(-np.nan_to_num(np.asarray(vals), nan=-np.inf), kind="stable")
-        chosen, seen = [], set()
-        for i in order:
-            key = cand[i].tobytes()
-            if key not in seen:
-                seen.add(key)
-                chosen.append(i)
-            if len(chosen) == int(self._p("starts")):
-                break
-        x = cand[chosen].copy()
+        x = _best_distinct(cand, vals, int(self._p("starts")))
         alpha = float(self._p("alpha"))
         m, v = np.zeros_like(x), np.zeros_like(x)
         b1_t, b2_t = self.B1, self.B2
@@ -123,6 +138,38 @@ class BatchedGradientSearch:
             b1_t *= self.B1
             b2_t *= self.B2
         return x_best
+
+
+class BatchedCmaesSearch:
+    """acquiopt<> policy: one random pass of `candidates` uniform points in [0,1]^D scored in one device pass, then one batched
+    CMA-ES on the device (the acquisition's cmaes_batch, DESIGN.md §4.15) with one instance from each of the best `starts`
+    distinct points: `lambda` offspring per instance (0: 4 + floor(3 ln D)), initial step `sigma`, at most `generations`
+    generations, an instance stopping when sigma sqrt(max diag C) < `tolx`.  Returns the better of the search's best point and the
+    random pass's (the random pass on ties); with an acquisition that has no cmaes_batch, or a model or mean the device search
+    does not take (model.MultiGP, a mean that depends on the input), the best point of the random pass."""
+
+    def __init__(self, params=None, rng: np.random.Generator | None = None):
+        self._params = params
+        self._rng = rng if rng is not None else np.random.default_rng()
+
+    def _p(self, name):
+        return _get(self._params, "opt_batchedcmaes", name)
+
+    def __call__(self, acqui, dim: int, bounded: bool = True) -> np.ndarray:
+        cand = self._rng.random((int(self._p("candidates")), dim))
+        best, idx, vals = acqui.argmax_batch(cand, return_values=True)
+        x_best = cand[idx].copy()
+        cmaes_batch = getattr(acqui, "cmaes_batch", None)
+        if cmaes_batch is None:
+            return x_best
+        starts = _best_distinct(cand, vals, int(self._p("starts")))
+        try:
+            x, v, _ = cmaes_batch(starts, lam=int(self._p("lambda")), sigma0=float(self._p("sigma")),
+                                  generations=int(self._p("generations")), tolx=float(self._p("tolx")),
+                                  seed=int(self._rng.integers(0, 2**63 - 1)), bounded=bounded)
+        except (AttributeError, NotImplementedError):
+            return x_best
+        return np.asarray(x, dtype=np.float64) if v > best else x_best
 
 
 class BOptimizer:

@@ -995,7 +995,7 @@ static int query_timed_out(lb_gp_full* h)
 
 static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_dev, double* mu_out, double* s2_out,
     bool out_dev, int acq_id, const double* acq_params, const double* mean_at_q, double mean_const, double* acq_out,
-    double* best_val, int64_t* best_idx, bool with_acq)
+    double* best_val, int64_t* best_idx, bool with_acq, bool lock_held = false)
 {
     if (!hc || M < 0) return LB_ERR_ARG;
     if (M == 0) return LB_OK;
@@ -1003,7 +1003,8 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
     lb_gp_full* h = full(hc);
     if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
     LB_DEVICE(h);
-    std::lock_guard<std::mutex> lock(h->ex.qmutex);
+    std::unique_lock<std::mutex> lock(h->ex.qmutex, std::defer_lock); // lock_held: the caller holds it (lb_acq_cmaes)
+    if (!lock_held) lock.lock();
     QueryWs& w = h->ex.ws;
     cudaStream_t st = h->stream;
     const int De = h->kp.D, P = n_outputs(h);
@@ -1429,6 +1430,18 @@ static int upload_front(lb_gp_full* a, const std::vector<double>& sorted)
     return LB_OK;
 }
 
+// The scoring of lb_ehvi_argmax after the models' passes, on a's stream: ehvi_kernel over a's uploaded front and the argmax
+static int ehvi_score(lb_gp_full* a, lb_gp_full* b, const double* ref_point, int64_t k, int64_t M, std::array<const double*, 3> dMeans,
+    double mean0_const, double mean1_const, double* dAcq, double* dBV, long long* dBI)
+{
+    QueryWs& w = a->ex.ws;
+    int rc;
+    if ((rc = lb_launch_ehvi(a->stream, ref_point[0], ref_point[1], k, w.dFront.get(), M, w.dMu.get(), n_outputs(a), dMeans[0], mean0_const,
+             w.dS2.get(), b->ex.ws.dMu.get(), n_outputs(b), dMeans[1], mean1_const, b->ex.ws.dS2.get(), dAcq, &a->launches)))
+        return rc;
+    return lb_launch_values_argmax(a->stream, M, dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &a->launches);
+}
+
 // experimental/acqui/ehvi.hpp:70-79 over the models m0 and m1 (ehvi.cu: ehvi_kernel), the front and the reference point on the
 // host.  The front is sorted by f[0] once (ehvi_front).
 static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point, int64_t k, const double* front, int64_t M,
@@ -1445,19 +1458,10 @@ static int ehvi_common(const lb_gp* m0, const lb_gp* m1, const double* ref_point
     std::scoped_lock lock(a->ex.qmutex, b->ex.qmutex); // deadlock-free whatever order other callers pass the pair in
     if (a->D <= 0 || !a->kernel_set || b->D <= 0 || !b->kernel_set) return LB_ERR_STATE;
     if (a->D != b->D) return LB_ERR_ARG;
-    cudaStream_t st = a->stream;
     return pair_argmax_locked(a, {b, nullptr}, M, Xq, dev, {mean0_at_q, mean1_at_q, nullptr}, acq_out, best_val, best_idx, true,
         [&](std::array<const double*, 3> dMeans, double* dAcq, double* dBV, long long* dBI) {
-            const double* dMean0 = dMeans[0];
-            const double* dMean1 = dMeans[1];
-            QueryWs& w = a->ex.ws;
-            int rc;
-            if ((rc = upload_front(a, sorted))) return rc;
-            const int Pa = n_outputs(a), Pb = n_outputs(b);
-            if ((rc = lb_launch_ehvi(st, ref_point[0], ref_point[1], k, w.dFront.get(), M, w.dMu.get(), Pa, dMean0, mean0_const, w.dS2.get(), b->ex.ws.dMu.get(), Pb,
-                     dMean1, mean1_const, b->ex.ws.dS2.get(), dAcq, &a->launches)))
-                return rc;
-            return lb_launch_values_argmax(st, M, dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &a->launches);
+            int rc = upload_front(a, sorted);
+            return rc ? rc : ehvi_score(a, b, ref_point, k, M, dMeans, mean0_const, mean1_const, dAcq, dBV, dBI);
         });
 }
 
@@ -1474,6 +1478,29 @@ int lb_ehvi_argmax_dev(const lb_gp* m0, const lb_gp* m1, const double* ref_point
 {
     return ehvi_common(m0, m1, ref_point, k, front_rowmajor, M, dXq_rowmajor, true, dMean0_at_q, mean0_const, dMean1_at_q, mean1_const,
         dAcq_out, dBest_val, dBest_idx);
+}
+
+// The front pass of lb_ehvi3d_argmax on a's stream: the sorted front into a's dFront and its per-cell planes into a's dEhvi3, sized
+// for M candidates.  The cell passes of any number of M-candidate batches may follow.
+static int ehvi3d_front_pass(lb_gp_full* a, const std::vector<double>& sorted, const double* ref_point, int64_t k, int64_t M)
+{
+    QueryWs& w = a->ex.ws;
+    int rc;
+    if ((rc = upload_front(a, sorted)) || (rc = ensure(a, w.dEhvi3, sizeof(double) * lb_ehvi3d_ws_doubles(k, M)))) return rc;
+    return lb_launch_ehvi3d_front(a->stream, ref_point, k, w.dFront.get(), w.dEhvi3.get(), &a->launches);
+}
+
+// The scoring of lb_ehvi3d_argmax after the models' passes and the front pass, on a's stream: the cell pass and the argmax
+static int ehvi3d_score(lb_gp_full* a, lb_gp_full* b, lb_gp_full* c, const double* ref_point, int64_t k, int64_t M,
+    std::array<const double*, 3> dMeans, std::array<double, 3> mean_const, double* dAcq, double* dBV, long long* dBI)
+{
+    QueryWs& w = a->ex.ws;
+    const LbEhvi3Model g0 = {w.dMu.get(), n_outputs(a), dMeans[0], mean_const[0], w.dS2.get()};
+    const LbEhvi3Model g1 = {b->ex.ws.dMu.get(), n_outputs(b), dMeans[1], mean_const[1], b->ex.ws.dS2.get()};
+    const LbEhvi3Model g2 = {c->ex.ws.dMu.get(), n_outputs(c), dMeans[2], mean_const[2], c->ex.ws.dS2.get()};
+    int rc = lb_launch_ehvi3d_cells(a->stream, ref_point, k, w.dFront.get(), M, g0, g1, g2, w.dEhvi3.get(), dAcq, &a->launches);
+    if (rc) return rc;
+    return lb_launch_values_argmax(a->stream, M, dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &a->launches);
 }
 
 // ehvi3d_sliceupdate (src/ehvi/ehvi_sliceupdate.cc) over the models m0, m1 and m2 (ehvi.cu: the front pass and
@@ -1495,18 +1522,10 @@ static int ehvi3d_common(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, cons
     for (lb_gp_full* h : {a, b, c})
         if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
     if (a->D != b->D || a->D != c->D) return LB_ERR_ARG;
-    cudaStream_t st = a->stream;
     return pair_argmax_locked(a, {b, c}, M, Xq, dev, {mean0_at_q, mean1_at_q, mean2_at_q}, acq_out, best_val, best_idx, true,
         [&](std::array<const double*, 3> dMeans, double* dAcq, double* dBV, long long* dBI) {
-            QueryWs& w = a->ex.ws;
-            int rc;
-            if ((rc = upload_front(a, sorted))) return rc;
-            if ((rc = ensure(a, w.dEhvi3, sizeof(double) * lb_ehvi3d_ws_doubles(k, M)))) return rc;
-            const LbEhvi3Model g0 = {w.dMu.get(), n_outputs(a), dMeans[0], mean0_const, w.dS2.get()};
-            const LbEhvi3Model g1 = {b->ex.ws.dMu.get(), n_outputs(b), dMeans[1], mean1_const, b->ex.ws.dS2.get()};
-            const LbEhvi3Model g2 = {c->ex.ws.dMu.get(), n_outputs(c), dMeans[2], mean2_const, c->ex.ws.dS2.get()};
-            if ((rc = lb_launch_ehvi3d(st, ref_point, k, w.dFront.get(), M, g0, g1, g2, w.dEhvi3.get(), dAcq, &a->launches))) return rc;
-            return lb_launch_values_argmax(st, M, dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &a->launches);
+            int rc = ehvi3d_front_pass(a, sorted, ref_point, k, M);
+            return rc ? rc : ehvi3d_score(a, b, c, ref_point, k, M, dMeans, {mean0_const, mean1_const, mean2_const}, dAcq, dBV, dBI);
         });
 }
 
@@ -1524,6 +1543,177 @@ int lb_ehvi3d_argmax_dev(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, cons
 {
     return ehvi3d_common(m0, m1, m2, ref_point, k, front_rowmajor, M, dXq_rowmajor, true, dMean0_at_q, mean0_const, dMean1_at_q,
         mean1_const, dMean2_at_q, mean2_const, dAcq_out, dBest_val, dBest_idx);
+}
+
+// ---- batched CMA-ES (lb_acq_cmaes, lb_ehvi_cmaes; cmaes.cu) -----------------------------------------------------------------------
+
+// Testing hook: with capture on, each search on the calling thread keeps the instances' states after every generation (R x
+// lb_cmaes_state_doubles(D) doubles each), then the last generation's R lambda x D candidates and R lambda values.
+static thread_local bool g_cmaes_capture = false;
+static thread_local std::vector<double> g_cmaes_trace;
+extern "C" int lb_debug_cmaes_capture(int on)
+{
+    g_cmaes_capture = on != 0;
+    g_cmaes_trace.clear();
+    return LB_OK;
+}
+// copies min(n, size) doubles of the last capture to dst (may be NULL) and returns its size
+extern "C" long long lb_debug_cmaes_trace(double* dst, long long n)
+{
+    const long long size = (long long)g_cmaes_trace.size();
+    if (dst) std::memcpy(dst, g_cmaes_trace.data(), sizeof(double) * (size_t)std::max(0LL, std::min(n, size)));
+    return size;
+}
+
+extern "C++" {
+// The search loop on h's stream (h: the handle whose stream, pool and launch count the search uses; every handle the scoring reads
+// is locked by the caller).  prepare(M) runs once before the first generation; per generation the ask kernel writes the R lambda
+// candidates to the device, score(dCand, M, dVals, dBestVal, dBestIdx) enqueues the scorer of the _dev entry points on them, and
+// the tell kernel updates every live instance.  Each reduced-precision handle in `scored` clears and sets its timeout flag in
+// every fill, so after each generation the flags are ORed into one word of the search: a timeout in any generation makes the
+// search return LB_ERR_TIMEOUT.  After every 8th generation the host reads that word and the number of live instances, and stops
+// when none is left.  The best point over the instances (ties to the lower instance) and the candidates scored come back on the
+// host.
+template <typename Prepare, typename Score>
+static int cmaes_search(lb_gp_full* h, std::array<lb_gp_full*, 3> scored, const lb_cmaes_opts* opts, int64_t R, const double* starts,
+    Prepare&& prepare, Score&& score, double* best_x, double* best_val, int64_t* n_evals)
+{
+    const int D = h->D;
+    LbCmaes s{};
+    std::vector<double> w;
+    int rc = lb_cmaes_setup(*opts, D, (int)R, &s, &w);
+    if (rc) return rc;
+    const int64_t S = lb_cmaes_state_doubles(D), M = R * s.lam;
+    std::vector<double> hs((size_t)(R * S));
+    for (int64_t r = 0; r < R; ++r) lb_cmaes_init_state(s, opts->sigma0, starts + r * D, hs.data() + r * S);
+    cudaStream_t st = h->stream;
+    StreamTemps tmp(h->device, st);
+    double *dW = nullptr, *dVals = nullptr, *dBV = nullptr;
+    long long* dBI = nullptr;
+    int* dLive = nullptr; // [0] live instances, [1] a reduced-precision timeout in some generation
+    const size_t nd = sizeof(double) * (size_t)(M * D);
+    if ((rc = tmp.alloc(sizeof(double) * w.size(), &dW)) || (rc = tmp.alloc(sizeof(double) * hs.size(), &s.state)) || (rc = tmp.alloc(nd, &s.z))
+        || (rc = tmp.alloc(nd, &s.y)) || (rc = tmp.alloc(nd, &s.cand)) || (rc = tmp.alloc(sizeof(double) * M, &dVals))
+        || (rc = tmp.alloc(sizeof(double), &dBV)) || (rc = tmp.alloc(sizeof(long long), &dBI)) || (rc = tmp.alloc(2 * sizeof(int), &dLive)))
+        return rc;
+    LB_CUDA(cudaMemsetAsync(dLive, 0, 2 * sizeof(int), st));
+    s.w = dW;
+    LB_CUDA(cudaMemcpyAsync(dW, w.data(), sizeof(double) * w.size(), cudaMemcpyHostToDevice, st));
+    LB_CUDA(cudaMemcpyAsync(s.state, hs.data(), sizeof(double) * hs.size(), cudaMemcpyHostToDevice, st));
+    const bool capture = g_cmaes_capture;
+    if (capture) g_cmaes_trace.clear();
+    if ((rc = prepare(M))) return rc;
+    int g = 0;
+    while (g < opts->generations) {
+        if ((rc = lb_launch_cmaes_ask(st, s, g, &h->launches)) || (rc = score(s.cand, M, dVals, dBV, dBI))) return rc;
+        for (lb_gp_full* q : scored) // the scoring of every handle is ordered before this point of h's stream
+            if (q && q->precision != LB_PREC_FP64 && q->N > 0 && q->ex.ws.dErr
+                && (rc = lb_launch_cmaes_flag(st, q->ex.ws.dErr.get(), dLive + 1, &h->launches)))
+                return rc;
+        const bool count = (g + 1) % 8 == 0 && g + 1 < opts->generations;
+        if (count) LB_CUDA(cudaMemsetAsync(dLive, 0, sizeof(int), st));
+        if ((rc = lb_launch_cmaes_tell(st, s, g, dVals, count ? dLive : nullptr, &h->launches))) return rc;
+        ++g;
+        if (capture) {
+            LB_CUDA(cudaMemcpyAsync(hs.data(), s.state, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
+            LB_CUDA(cudaStreamSynchronize(st));
+            g_cmaes_trace.insert(g_cmaes_trace.end(), hs.begin(), hs.end());
+        }
+        if (count) {
+            int word[2] = {0, 0};
+            LB_CUDA(cudaMemcpyAsync(word, dLive, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+            LB_CUDA(cudaStreamSynchronize(st));
+            if (word[1]) return LB_ERR_TIMEOUT;
+            if (word[0] == 0) break;
+        }
+    }
+    LB_CUDA(cudaMemcpyAsync(hs.data(), s.state, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
+    if (capture) {
+        const size_t n0 = g_cmaes_trace.size();
+        g_cmaes_trace.resize(n0 + (size_t)(M * D + M));
+        LB_CUDA(cudaMemcpyAsync(g_cmaes_trace.data() + n0, s.cand, nd, cudaMemcpyDeviceToHost, st));
+        LB_CUDA(cudaMemcpyAsync(g_cmaes_trace.data() + n0 + M * D, dVals, sizeof(double) * M, cudaMemcpyDeviceToHost, st));
+    }
+    int timeout = 0;
+    LB_CUDA(cudaMemcpyAsync(&timeout, dLive + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+    LB_CUDA(cudaStreamSynchronize(st));
+    if (timeout) return LB_ERR_TIMEOUT;
+    // per instance: best_x at 3 D, best_val at 4 D + 2 D^2 + 1 (cmaes.cu's layout)
+    int64_t best = 0;
+    for (int64_t r = 1; r < R; ++r)
+        if (hs[(size_t)(r * S + S - 2)] > hs[(size_t)(best * S + S - 2)]) best = r;
+    std::memcpy(best_x, hs.data() + best * S + 3 * D, sizeof(double) * D);
+    *best_val = hs[(size_t)(best * S + S - 2)];
+    *n_evals = (int64_t)g * M;
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+} // extern "C++"
+
+// the checks lb_acq_cmaes and lb_ehvi_cmaes share before any lock: pointers, R and finite starts (D columns)
+static int cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts, int D, const double* best_x, const double* best_val,
+    const int64_t* n_evals)
+{
+    if (!opts || !starts || !best_x || !best_val || !n_evals || R <= 0 || R > (int64_t)INT32_MAX) return LB_ERR_ARG;
+    if (D > 0)
+        for (int64_t i = 0; i < R * D; ++i)
+            if (!std::isfinite(starts[i])) return LB_ERR_ARG;
+    return LB_OK;
+}
+
+int lb_acq_cmaes(const lb_gp* hc, int acq_id, const double* acq_params, double mean_const, const lb_cmaes_opts* opts, int64_t R,
+    const double* starts, double* best_x, double* best_val, int64_t* n_evals)
+{
+    if (!hc || !acq_params) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
+    lb_gp_full* h = full(hc);
+    int rc = cmaes_args(opts, R, starts, h->D, best_x, best_val, n_evals);
+    if (rc) return rc;
+    if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex); // the model stays the same for the whole search
+    return cmaes_search(
+        h, {h, nullptr, nullptr}, opts, R, starts, [](int64_t) { return LB_OK; },
+        [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
+            return query_common(h, M, dCand, true, nullptr, nullptr, true, acq_id, acq_params, nullptr, mean_const, dVals, dBV,
+                (int64_t*)dBI, true, true);
+        },
+        best_x, best_val, n_evals);
+}
+
+int lb_ehvi_cmaes(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, const double* ref_point, int64_t k, const double* front,
+    double mean0_const, double mean1_const, double mean2_const, const lb_cmaes_opts* opts, int64_t R, const double* starts,
+    double* best_x, double* best_val, int64_t* n_evals)
+{
+    if (!m0) return LB_ERR_ARG;
+    int rc = cmaes_args(opts, R, starts, m0->D, best_x, best_val, n_evals);
+    if (rc) return rc;
+    std::vector<double> sorted;
+    if ((rc = ehvi_front(m0, m1, m2, ref_point, k, front, 1, starts, &sorted))) return rc;
+    lb_gp_full* a = full(m0);
+    lb_gp_full* b = full(m1);
+    lb_gp_full* c = m2 ? full(m2) : nullptr;
+    LB_DEVICE(a);
+    auto locked = [&] {
+        for (lb_gp_full* h : {a, b, c})
+            if (h && (h->D <= 0 || !h->kernel_set)) return LB_ERR_STATE;
+        if (a->D != b->D || (c && a->D != c->D)) return LB_ERR_ARG;
+        auto prepare = [&](int64_t M) { return c ? ehvi3d_front_pass(a, sorted, ref_point, k, M) : upload_front(a, sorted); };
+        auto score = [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
+            return pair_argmax_locked(a, {b, c}, M, dCand, true, {nullptr, nullptr, nullptr}, dVals, dBV, (int64_t*)dBI, true,
+                [&](std::array<const double*, 3> dMeans, double* dAcq, double* dB, long long* dI) {
+                    return c ? ehvi3d_score(a, b, c, ref_point, k, M, dMeans, {mean0_const, mean1_const, mean2_const}, dAcq, dB, dI)
+                             : ehvi_score(a, b, ref_point, k, M, dMeans, mean0_const, mean1_const, dAcq, dB, dI);
+                });
+        };
+        return cmaes_search(a, {a, b, c}, opts, R, starts, prepare, score, best_x, best_val, n_evals);
+    };
+    if (c) {
+        std::scoped_lock lock(a->ex.qmutex, b->ex.qmutex, c->ex.qmutex); // deadlock-free whatever order other callers pass them in
+        return locked();
+    }
+    std::scoped_lock lock(a->ex.qmutex, b->ex.qmutex);
+    return locked();
 }
 
 // ---- gradients of the two-model acquisitions (lb_eci_grad, lb_ehvi_grad) -------------------------------------------------------

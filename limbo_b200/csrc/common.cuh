@@ -735,12 +735,42 @@ struct LbEhvi3Model {
     double mean_const;
     const double* s2;
 };
-// doubles of lb_launch_ehvi3d's workspace for a front of k points and M candidates
+// doubles of the ehvi3d passes' workspace for a front of k points and M candidates
 size_t lb_ehvi3d_ws_doubles(int64_t k, int64_t M);
-// ehvi3d_sliceupdate of every candidate into dAcq (M): dFront is the 9 k doubles lb_ehvi3d_argmax uploads, dWs has
-// lb_ehvi3d_ws_doubles(k, M) doubles
-int lb_launch_ehvi3d(cudaStream_t st, const double* r, int64_t k, const double* dFront, int64_t M, const LbEhvi3Model& m0,
+// ehvi3d_sliceupdate in two passes over dWs (lb_ehvi3d_ws_doubles(k, M) doubles); dFront is the 9 k doubles lb_ehvi3d_argmax
+// uploads.  The front pass builds the per-cell planes, which depend on the front and ref_point only; the cell pass scores every
+// candidate into dAcq (M) from them, and may run any number of times after one front pass for the same front, k and M.
+int lb_launch_ehvi3d_front(cudaStream_t st, const double* r, int64_t k, const double* dFront, double* dWs, long long* launches);
+int lb_launch_ehvi3d_cells(cudaStream_t st, const double* r, int64_t k, const double* dFront, int64_t M, const LbEhvi3Model& m0,
     const LbEhvi3Model& m1, const LbEhvi3Model& m2, double* dWs, double* dAcq, long long* launches);
+// cmaes.cu: the batched CMA-ES of lb_acq_cmaes / lb_ehvi_cmaes (DESIGN.md §4.15).  Per instance, the device state is
+// lb_cmaes_state_doubles(D) doubles: m, p_sigma, p_c, best_x (D each), C and A (D x D row-major each; A lower), then sigma,
+// best_val and the stop flag.
+#define LB_CMAES_MAX_D 64
+#define LB_CMAES_MAX_LAMBDA 256
+struct lb_cmaes_opts; // include/limbo_b200.h
+struct LbCmaes {
+    int R, D, lam, mu, bounded;
+    uint64_t seed;
+    double cs, ds, cc, c1, cmu, mueff, chi, sumw, tolx;
+    const double* w;   // lam recombination weights (device)
+    double* state;     // R x lb_cmaes_state_doubles(D)
+    double* z;         // R x lam x D: the draws of the current generation
+    double* y;         // R x lam x D: A z
+    double* cand;      // R x lam x D: the phenotypes, the scorer's candidates
+};
+__host__ __device__ inline int64_t lb_cmaes_state_doubles(int D) { return 4 * (int64_t)D + 2 * (int64_t)D * D + 3; }
+// The strategy constants and the weights (host, lam doubles) of lb_cmaes_opts o in dimension D, into s (pointers untouched);
+// LB_ERR_UNSUPPORTED past LB_CMAES_MAX_D / LB_CMAES_MAX_LAMBDA, LB_ERR_ARG for a bad option.
+int lb_cmaes_setup(const lb_cmaes_opts& o, int D, int R, LbCmaes* s, std::vector<double>* w);
+// the initial state of instance r from its start (phenotype), into st (lb_cmaes_state_doubles(D) doubles)
+void lb_cmaes_init_state(const LbCmaes& s, double sigma0, const double* start, double* st);
+// generation g: draws, A z and the phenotypes into s.cand
+int lb_launch_cmaes_ask(cudaStream_t st, const LbCmaes& s, int g, long long* launches);
+// *dFlag |= *dErr (a scoring pass's reduced-precision timeout flag) on st
+int lb_launch_cmaes_flag(cudaStream_t st, const int* dErr, int* dFlag, long long* launches);
+// generation g's update from the R x lam values dVals; dLive (NULL: not counted) gains the instances still live after it
+int lb_launch_cmaes_tell(cudaStream_t st, const LbCmaes& s, int g, const double* dVals, int* dLive, long long* launches);
 // sparsify.cu
 int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const double* dX, int64_t max_points, long long* dKept,
     int64_t* n_kept, long long* dRemoved, double* dRemovedScore, long long* launches);

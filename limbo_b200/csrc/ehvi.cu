@@ -609,31 +609,47 @@ size_t lb_ehvi3d_ws_doubles(int64_t k, int64_t M)
     return 3 * nn + 2 * nn * (size_t)(k + 1) + (size_t)ehvi3d_xblocks(k) * (size_t)M;
 }
 
-int lb_launch_ehvi3d(cudaStream_t st, const double* r, int64_t k, const double* dFront, int64_t M, const LbEhvi3Model& m0,
+// the workspace's planes, in lb_ehvi3d_ws_doubles's order
+struct E3Planes { double *hd, *xlim, *ylim, *slice, *chunk, *part; };
+static E3Planes ehvi3d_planes(int64_t k, double* dWs)
+{
+    const size_t nn = (size_t)(k * k);
+    E3Planes p;
+    p.hd = dWs;
+    p.xlim = p.hd + nn;
+    p.ylim = p.xlim + nn;
+    p.slice = p.ylim + nn;
+    p.chunk = p.slice + nn * (size_t)(k + 1);
+    p.part = p.chunk + nn * (size_t)(k + 1);
+    return p;
+}
+
+int lb_launch_ehvi3d_front(cudaStream_t st, const double* r, int64_t k, const double* dFront, double* dWs, long long* launches)
+{
+    if (k < 0 || k > LB_EHVI3D_MAX_K) return LB_ERR_UNSUPPORTED;
+    if (k == 0) return LB_OK;
+    const int n = (int)k;
+    const E3Planes p = ehvi3d_planes(k, dWs);
+    const unsigned g = (unsigned)(((size_t)n * n + 255) / 256);
+    ehvi3d_dom_kernel<<<g, 256, 0, st>>>(n, dFront, r[0], r[1], p.hd, p.xlim, p.ylim);
+    ehvi3d_slice_kernel<<<n + 1, 256, 0, st>>>(n, dFront, r[0], r[1], p.hd, p.slice);
+    ehvi3d_chunk_kernel<<<g, 256, 0, st>>>(n, dFront, r[2], p.slice, p.chunk);
+    if (launches) *launches += 3;
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+
+int lb_launch_ehvi3d_cells(cudaStream_t st, const double* r, int64_t k, const double* dFront, int64_t M, const LbEhvi3Model& m0,
     const LbEhvi3Model& m1, const LbEhvi3Model& m2, double* dWs, double* dAcq, long long* launches)
 {
     if (k < 0 || k > LB_EHVI3D_MAX_K) return LB_ERR_UNSUPPORTED;
-    const int n = (int)k;
-    const size_t nn = (size_t)n * n;
-    double* hd = dWs;
-    double* xlim = hd + nn;
-    double* ylim = xlim + nn;
-    double* slice = ylim + nn;
-    double* chunk = slice + nn * (n + 1);
-    double* part = chunk + nn * (n + 1);
-    if (n > 0) {
-        const unsigned g = (unsigned)((nn + 255) / 256);
-        ehvi3d_dom_kernel<<<g, 256, 0, st>>>(n, dFront, r[0], r[1], hd, xlim, ylim);
-        ehvi3d_slice_kernel<<<n + 1, 256, 0, st>>>(n, dFront, r[0], r[1], hd, slice);
-        ehvi3d_chunk_kernel<<<g, 256, 0, st>>>(n, dFront, r[2], slice, chunk);
-        if (launches) *launches += 3;
-    }
+    const E3Planes p = ehvi3d_planes(k, dWs);
     static LbOncePerDevice once;
     if (once.need()) LB_CUDA(cudaFuncSetAttribute(ehvi3d_cells_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)E3_SMEM));
     const int nxb = ehvi3d_xblocks(k);
-    ehvi3d_cells_kernel<<<dim3((unsigned)((M + E3_Q - 1) / E3_Q), (unsigned)nxb), E3_Q, E3_SMEM, st>>>(n, dFront, r[0], r[1], r[2], hd, xlim,
-        ylim, chunk, slice, M, m0, m1, m2, part);
-    ehvi3d_sum_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(M, nxb, part, dAcq);
+    ehvi3d_cells_kernel<<<dim3((unsigned)((M + E3_Q - 1) / E3_Q), (unsigned)nxb), E3_Q, E3_SMEM, st>>>((int)k, dFront, r[0], r[1], r[2],
+        p.hd, p.xlim, p.ylim, p.chunk, p.slice, M, m0, m1, m2, p.part);
+    ehvi3d_sum_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(M, nxb, p.part, dAcq);
     if (launches) *launches += 2;
     LB_CUDA(cudaGetLastError());
     return LB_OK;

@@ -57,3 +57,23 @@ def values_and_grads(lib, name: str, M: int, D: int, *args):
     vals, grads = np.empty(M), np.empty((M, D))
     _lib.check(getattr(lib, name)(*args, ptr(vals), ptr(grads)), name)
     return vals, grads
+
+
+def constant_mean(model, D: int) -> float:
+    """The first output of the model's mean functor when it does not depend on the input; NotImplementedError otherwise (a search
+    that runs on the device cannot call a host mean at every generation)."""
+    mf = model.mean_function()
+    if not mf.is_constant():
+        raise NotImplementedError("the device CMA-ES takes input-free means only")
+    return float(np.asarray(mf(np.zeros(D), model))[0])
+
+
+def cmaes(lib, name: str, D: int, *args, lam: int = 0, sigma0: float = 0.5, generations: int = 100, tolx: float = 1e-12, seed: int = 0,
+          bounded: bool = True):
+    """Calls lib.<name>(*args, &opts, R, starts, best_x, &best_val, &n_evals), args ending with the R x D starts; returns
+    (best_x, best_val, n_evals)."""
+    starts = candidates(args[-1])
+    opts = _lib.CmaesOpts(int(lam), float(sigma0), int(generations), float(tolx), int(seed) & 0xFFFFFFFFFFFFFFFF, int(bool(bounded)))
+    bx, bv, n = np.empty(D), C.c_double(), C.c_int64()
+    _lib.check(getattr(lib, name)(*args[:-1], C.byref(opts), starts.shape[0], ptr(starts), ptr(bx), C.addressof(bv), C.addressof(n)), name)
+    return bx, bv.value, n.value

@@ -15,7 +15,7 @@ import numpy as np
 from .. import _lib
 from .. import kernel as _kernel
 from .. import mean as _mean
-from ._calls import acq_param_pair, argmax, candidates, first_mean, first_mean_and_grad, ptr, values_and_grads
+from ._calls import acq_param_pair, argmax, candidates, cmaes, constant_mean, first_mean, first_mean_and_grad, ptr, values_and_grads
 
 
 class GP:
@@ -252,6 +252,32 @@ class GP:
         means = [first_mean(g, Xq) for g in (self, m1, m2)]
         return argmax(self._lib, "lb_ehvi3d_argmax", M, return_values, self._h, m1._h, m2._h, ptr(r), F.shape[0], ptr(F) if F.size else None,
                       M, ptr(Xq), *[a for m, c in means for a in (ptr(m), c)])
+
+    def acq_cmaes_batch(self, acq_id: int, acq_params, starts, **opts):
+        """Batched CMA-ES on the device (lb_acq_cmaes) over UCB / GP_UCB (acq_id 0) or EI (acq_id 1), parameters as
+        acq_argmax_batch: one instance from each row of `starts` (R x D).  opts: lam (0: 4 + floor(3 ln D)), sigma0, generations,
+        tolx, seed, bounded.  Returns (best_x, best_val, n_evals); NotImplementedError for a mean that depends on the input."""
+        S = candidates(starts)
+        mconst = constant_mean(self, S.shape[1])
+        self._push_prior_if_empty(S.shape[1])
+        return cmaes(self._lib, "lb_acq_cmaes", S.shape[1], self._h, acq_id, ptr(acq_param_pair(acq_params)), mconst, S, **opts)
+
+    def ehvi_cmaes_batch(self, others, ref_point, front, starts, **opts):
+        """Batched CMA-ES on the device (lb_ehvi_cmaes) over the two-objective (others = [m1]) or three-objective (others = [m1,
+        m2]) EHVI of ehvi_argmax_batch / ehvi3d_argmax_batch; starts and opts as acq_cmaes_batch.  Returns (best_x, best_val,
+        n_evals); NotImplementedError for a mean that depends on the input."""
+        S = candidates(starts)
+        D = S.shape[1]
+        models = [self, *others]
+        K = len(models)
+        assert K in (2, 3)
+        F = np.ascontiguousarray(np.asarray(front, dtype=np.float64).reshape(-1, K))
+        r = np.ascontiguousarray(np.asarray(ref_point, dtype=np.float64).reshape(-1)[:K])
+        consts = [constant_mean(g, D) for g in models] + [0.0] * (3 - K)
+        for g in models:
+            g._push_prior_if_empty(D)
+        return cmaes(self._lib, "lb_ehvi_cmaes", D, self._h, models[1]._h, models[2]._h if K == 3 else None, ptr(r), F.shape[0],
+                     ptr(F) if F.size else None, *consts, S, **opts)
 
     def query_grad_batch(self, Xq):
         """mu (M x P), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D, of the first output) and
