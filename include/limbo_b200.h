@@ -272,6 +272,14 @@ int lb_acq_cmaes(const lb_gp* h, int acq_id, const double* acq_params, double me
 int lb_ehvi_cmaes(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, const double* ref_point, int64_t k, const double* front_rowmajor,
     double mean0_const, double mean1_const, double mean2_const, const lb_cmaes_opts* opts, int64_t R, const double* starts_rowmajor,
     double* best_x, double* best_val, int64_t* n_evals);
+/* lb_eci_argmax's ECI (eci_params = {f_max, jitter}) with input-free means (obj_mean_const, con_mean_const); every value the
+ * search scores is lb_eci_argmax_dev's on the same candidates.  con may be NULL, and a con without samples gives Pf = 1.  An obj
+ * without samples scores 0 everywhere: best_x is the first start, best_val 0 and n_evals 0, and nothing is launched (its input
+ * dimension must be set, LB_ERR_STATE otherwise).  Both handles are locked for the whole search; LB_ERR_TIMEOUT when a
+ * reduced-precision pass of either timed out in any generation.  LB_ERR_ARG for obj == con, handles on different devices or a con
+ * with samples and another input dimension, and lb_acq_cmaes's cases; LB_ERR_STATE as lb_eci_argmax. */
+int lb_eci_cmaes(const lb_gp* obj, const lb_gp* con, const double* eci_params, double obj_mean_const, double con_mean_const,
+    const lb_cmaes_opts* opts, int64_t R, const double* starts_rowmajor, double* best_x, double* best_val, int64_t* n_evals);
 
 /* pareto::impl::pareto_set_std (experimental/tools/pareto.hpp:138-162) over n points of K objectives (row-major n x K): the
  * indices of the points no other point dominates (dominate_flag == 1), duplicates kept, in compare_objs_lex order
@@ -295,8 +303,8 @@ int lb_sparsify_dev(const lb_gp* h, int64_t N, int D, const double* dX_rowmajor,
     int64_t* n_kept, int64_t* dRemoved, double* dRemovedScore);
 
 /* experimental::model::SPGP (experimental/model/spgp.hpp): Snelson and Ghahramani's sparse GP with M pseudo-inputs, single
- * output, SE-ARD.  Same conventions as lb_gp; lb_spgp_query, lb_spgp_acq_argmax, lb_spgp_query_grad and lb_spgp_acq_grad may be
- * called from several threads, the other calls need exclusive access.  w is the reference's parameter vector (HyperParams, spgp.hpp:94-101) of n_w = (M+1) D + 2
+ * output, SE-ARD.  Same conventions as lb_gp; lb_spgp_query, lb_spgp_acq_argmax, their _dev variants, lb_spgp_acq_cmaes,
+ * lb_spgp_query_grad and lb_spgp_acq_grad may be called from several threads, the other calls need exclusive access.  w is the reference's parameter vector (HyperParams, spgp.hpp:94-101) of n_w = (M+1) D + 2
  * entries: [xb (M x D, column-major), log b (D; b = inverse squared length scales), log c (signal variance), log sig (noise
  * variance)].  lb_spgp_lik and lb_spgp_compute return LB_ERR_ARG for M < 1, M > N, n_w != (M+1) D + 2 or a non-finite w, and
  * the 1-based index (> 0) of the first non-positive pivot of Q = K(xb, xb) + jitter I, or else of A = sig I + V V^T. */
@@ -314,9 +322,21 @@ int lb_spgp_compute(lb_spgp* s, int64_t M, int64_t n_w, const double* w, double 
 /* SPGP::_predict (spgp.hpp:582-610) for Mq candidates (row-major Mq x D): mu_minus_mean (Mq, without mean(v)) and sigma2 (Mq,
  * + sig when optimized != 0).  LB_ERR_STATE before lb_spgp_compute. */
 int lb_spgp_query(const lb_spgp* s, int64_t Mq, const double* Xq_rowmajor, int optimized, double* mu_minus_mean, double* sigma2);
+/* same, device pointers; bit-identical to lb_spgp_query on the same candidates.  No synchronisation: the results are ordered on
+ * the model's stream, behind which any synchronising lb_spgp_* call or a device synchronisation waits. */
+int lb_spgp_query_dev(const lb_spgp* s, int64_t Mq, const double* dXq_rowmajor, int optimized, double* dMu_minus_mean, double* dSigma2);
 /* lb_acq_argmax over lb_spgp_query's mu and sigma^2 (ties to the lowest index). */
 int lb_spgp_acq_argmax(const lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* Xq_rowmajor, int optimized,
     const double* mean_at_q, double mean_const, double* acq_out, double* best_val, int64_t* best_idx);
+/* same, device pointers except acq_params, as lb_acq_argmax_dev; bit-identical to lb_spgp_acq_argmax on the same candidates.  No
+ * synchronisation, results on the model's stream as in lb_spgp_query_dev. */
+int lb_spgp_acq_argmax_dev(const lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* dXq_rowmajor, int optimized,
+    const double* dMean_at_q, double mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
+/* lb_acq_cmaes over the model: lb_spgp_acq_argmax's UCB / GP_UCB / EI with an input-free mean (mean_const); every value the search
+ * scores is lb_spgp_acq_argmax_dev's on the same candidates.  The model is locked for the whole search.  LB_ERR_STATE before
+ * lb_spgp_compute; LB_ERR_ARG for an unknown acq_id, and lb_acq_cmaes's cases.  Synchronises the model's stream. */
+int lb_spgp_acq_cmaes(const lb_spgp* s, int acq_id, const double* acq_params, int optimized, double mean_const, const lb_cmaes_opts* opts,
+    int64_t R, const double* starts_rowmajor, double* best_x, double* best_val, int64_t* n_evals);
 /* Candidate gradients for Mq candidates (row-major Mq x D), extending lb_spgp_query as lb_query_grad extends lb_query:
  * mu_minus_mean and sigma2 are bit-identical to lb_spgp_query's on the same batch; dmu (Mq x D row-major) is the gradient of
  * mu_minus_mean, dsigma2 (Mq x D) that of sigma2.  With b the inverse squared length scales, x~ = x o sqrt(b), k_m the kernel

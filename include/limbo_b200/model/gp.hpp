@@ -306,6 +306,26 @@ namespace limbo_b200 {
                     "lb_ehvi_cmaes");
                 return best;
             }
+            // Batched CMA-ES on the device (lb_eci_cmaes) over the ECI of eci_argmax: this GP is the objective, `con` the constraint
+            // model (Pf = 1 while it has no samples); arguments and results as acq_cmaes.  Without objective samples every value is
+            // 0: best_x is starts[0] and n_evals 0.
+            template <typename ConstraintGP>
+            double eci_cmaes(const ConstraintGP& con, double f_max, double jitter, const std::vector<Eigen::VectorXd>& starts,
+                const lb_cmaes_opts& opts, Eigen::VectorXd& best_x, int64_t& n_evals) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "eci_cmaes: the objective's mean function depends on the input");
+                static_assert(mean_is_input_free<std::decay_t<decltype(con.mean_function())>>::value,
+                    "eci_cmaes: the constraint's mean function depends on the input");
+                const int D = (int)starts[0].size();
+                if (_samples.empty()) _push_prior(D); // the search needs D even when it scores nothing
+                const std::vector<double> st = detail::pack_rows(starts);
+                double params[2] = {f_max, jitter}, best = 0;
+                best_x.resize(D);
+                lb_check(lb_eci_cmaes(_h, con._h, params, _mean_const(D), con._samples.empty() ? 0.0 : con._mean_const(D), &opts,
+                             (int64_t)starts.size(), st.data(), best_x.data(), &best, &n_evals),
+                    "lb_eci_cmaes");
+                return best;
+            }
 
             // ECI values (M) and gradients (M x D) with respect to the candidates in one device pass over both models (lb_eci_grad,
             // FirstElem aggregator): arguments and values as eci_argmax.  Without objective samples both are 0 (eci.hpp:86).

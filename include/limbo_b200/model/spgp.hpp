@@ -113,7 +113,7 @@ namespace limbo_b200 {
             Eigen::MatrixXd mu(const Eigen::MatrixXd& v) const { return predict(v).first; }
 
             // ---- batched extensions with GP's signatures (not in the reference): what the batch-aware acquisitions of
-            // opt/batched_random.hpp call under BatchedRandom and BatchedGradient ----
+            // opt/batched_random.hpp call under BatchedRandom, BatchedGradient and BatchedCmaes ----
             // mu: M x dim_out (mean function included), sigma2: M
             void query_batch(const std::vector<Eigen::VectorXd>& vs, Eigen::MatrixXd& mu, Eigen::VectorXd& sigma2) const
             {
@@ -177,6 +177,22 @@ namespace limbo_b200 {
                 detail::unpack(s, sigma2);
                 detail::unpack(gm, M, D, dmu);
                 detail::unpack(gs, M, D, dsigma2);
+            }
+            // Batched CMA-ES on the device (lb_spgp_acq_cmaes) over UCB / EI (acq_id, p0, p1 as acq_argmax), one instance from each
+            // start; the mean must not depend on the input (its first output is passed as a constant).  Returns the best value; best_x
+            // and n_evals (candidates scored) are filled in.
+            double acq_cmaes(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& starts, const lb_cmaes_opts& opts,
+                Eigen::VectorXd& best_x, int64_t& n_evals) const
+            {
+                static_assert(mean_is_input_free<MeanFunction>::value, "acq_cmaes: the mean function depends on the input");
+                const int D = (int)starts[0].size();
+                const std::vector<double> st = detail::pack_rows(starts);
+                double params[2] = {p0, p1}, best = 0;
+                best_x.resize(D);
+                _check(lb_spgp_acq_cmaes(_h, acq_id, params, _optimized ? 1 : 0, _mean_function(Eigen::VectorXd::Zero(D), *this)(0), &opts,
+                           (int64_t)starts.size(), st.data(), best_x.data(), &best, &n_evals),
+                    "lb_spgp_acq_cmaes");
+                return best;
             }
             double sigma(const Eigen::VectorXd& v) const { return std::get<1>(query(v)); }
 

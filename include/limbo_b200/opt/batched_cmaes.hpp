@@ -7,8 +7,9 @@
 // 1. one random pass of `candidates` points in [0, 1]^D, announced through BatchedRandom's BatchRequest (one lb_acq_argmax /
 //    lb_ehvi*_argmax with every value when a batch-aware functor answers it);
 // 2. the best `starts` distinct points start one batched CMA-ES on the device (DESIGN.md §4.15), announced through a thread-local
-//    CmaesRequest and one call of f: a batch-aware UCB / EI over limbo_b200::model::GP, or the acqui::Ehvi specialisation with
-//    two or three models, answers it with one lb_acq_cmaes / lb_ehvi_cmaes when the means do not depend on the input;
+//    CmaesRequest and one call of f: a batch-aware UCB / EI over limbo_b200::model::GP or model::SPGP, the batch-aware ECI over
+//    two limbo_b200::model::GP (experimental::bayes_opt::CBOptimizer), or the acqui::Ehvi specialisation with two or three models,
+//    answers it with one lb_acq_cmaes / lb_spgp_acq_cmaes / lb_eci_cmaes / lb_ehvi_cmaes when the means do not depend on the input;
 // 3. the better of the search's best point and the random pass's is returned (the random pass's on ties).
 // With a functor that is not batch-aware (the reference's acqui::UCB) the random pass runs one point at a time, as BatchedRandom
 // does, and its best point is returned; so is it when the CmaesRequest stays unanswered.

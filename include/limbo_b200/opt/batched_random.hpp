@@ -84,8 +84,9 @@ namespace limbo_b200 {
         }
 
         // The start points announced by BatchedCmaes (opt/batched_cmaes.hpp) for one call of f: a batch-aware UCB / EI over
-        // limbo_b200::model::GP, or the acqui::Ehvi specialisation (acqui/ehvi.hpp), runs one device CMA-ES from them
-        // (lb_acq_cmaes / lb_ehvi_cmaes) and files its best point, value and evaluations.  Means must not depend on the input.
+        // limbo_b200::model::GP or model::SPGP, ECI over two limbo_b200::model::GP, or the acqui::Ehvi specialisation
+        // (acqui/ehvi.hpp), runs one device CMA-ES from them (lb_acq_cmaes / lb_spgp_acq_cmaes / lb_eci_cmaes / lb_ehvi_cmaes) and
+        // files its best point, value and evaluations.  Means must not depend on the input.
         struct CmaesRequest {
             const std::vector<Eigen::VectorXd>* starts = nullptr;
             lb_cmaes_opts opts{};
@@ -232,10 +233,13 @@ namespace limbo_b200 {
             struct has_candidate_grad<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
             template <typename P, typename K, typename Mf, typename H>
             struct has_candidate_grad<model::SPGP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
-            // a device GP with an input-free mean: the device CMA-ES (lb_acq_cmaes, lb_ehvi_cmaes) takes it
+            // a device model with an input-free mean: the device CMA-ES (lb_acq_cmaes, lb_eci_cmaes and lb_ehvi_cmaes for a GP,
+            // lb_spgp_acq_cmaes for an SPGP) takes it
             template <typename M> struct has_device_cmaes : std::false_type {};
             template <typename P, typename K, typename Mf, typename H>
             struct has_device_cmaes<model::GP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
+            template <typename P, typename K, typename Mf, typename H>
+            struct has_device_cmaes<model::SPGP<P, K, Mf, H>> : model::mean_is_input_free<Mf> {};
         }
 
         // acqui::UCB (acqui/ucb.hpp:83-90), batch-aware
@@ -341,8 +345,9 @@ namespace limbo_b200 {
         // experimental::bayes_opt::CBOptimizer builds it.  When both models are limbo_b200::model::GP and afun acts like FirstElem,
         // it answers BatchedRandom's request with one fused device pass over both models (GP::eci_argmax -> lb_eci_argmax);
         // otherwise it evaluates one point at a time, exactly as eci.hpp does.  When, in addition, both means do not depend on the
-        // input, it answers operator()(v, afun, true) and BatchedGradient's GradRequest with one lb_eci_grad (GP::eci_grad), and
-        // files every candidate's value in BatchedGradient's random pass so that the optimiser climbs.
+        // input, it answers operator()(v, afun, true) and BatchedGradient's GradRequest with one lb_eci_grad (GP::eci_grad), files
+        // every candidate's value in BatchedGradient's random pass so that the optimiser climbs, and answers BatchedCmaes's
+        // CmaesRequest with one lb_eci_cmaes (GP::eci_cmaes) once the objective has samples.
         template <typename Params, typename Model, typename ConstraintModel>
         class ECI {
         public:
@@ -371,6 +376,14 @@ namespace limbo_b200 {
                 }
                 else
                     assert(!gradient);
+                if constexpr (has_cmaes) {
+                    if (opt::current_cmaes() && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
+                        _update_f_max(afun);
+                        detail::answer_cmaes([&](const std::vector<Eigen::VectorXd>& st, const lb_cmaes_opts& o, Eigen::VectorXd& x, int64_t& n) {
+                            return _model.eci_cmaes(_constraint_model, _f_max, Params::acqui_eci::jitter(), st, o, x, n);
+                        });
+                    }
+                }
                 if constexpr (detail::is_device_gp<Model>::value && detail::is_device_gp<ConstraintModel>::value) {
                     opt::BatchRequest* req = opt::current_batch();
                     if (req && _model.nb_samples() > 0 && detail::acts_like_first_elem(afun, (int)_model.dim_out())) {
@@ -397,6 +410,9 @@ namespace limbo_b200 {
         protected:
             // both models are device GPs whose means do not depend on the input: gradients from lb_eci_grad
             static constexpr bool has_grad = detail::has_candidate_grad<Model>::value && detail::has_candidate_grad<ConstraintModel>::value;
+            // both models are device GPs whose means do not depend on the input: the search from lb_eci_cmaes
+            static constexpr bool has_cmaes = detail::is_device_gp<Model>::value && detail::is_device_gp<ConstraintModel>::value
+                && detail::has_device_cmaes<Model>::value && detail::has_device_cmaes<ConstraintModel>::value;
 
             const Model& _model;
             const ConstraintModel& _constraint_model;

@@ -30,11 +30,12 @@ DECLARED_SYMBOLS = [
     "lb_create", "lb_destroy", "lb_clone", "lb_set_stream", "lb_sync", "lb_launch_count", "lb_set_data",
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
     "lb_acq_argmax", "lb_acq_argmax_dev", "lb_query_grad", "lb_query_grad_dev", "lb_acq_grad", "lb_acq_grad_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_eci_grad", "lb_eci_grad_dev", "lb_ehvi_argmax", "lb_ehvi_argmax_dev",
-    "lb_ehvi3d_argmax", "lb_ehvi3d_argmax_dev", "lb_acq_cmaes", "lb_ehvi_cmaes",
+    "lb_ehvi3d_argmax", "lb_ehvi3d_argmax_dev", "lb_acq_cmaes", "lb_ehvi_cmaes", "lb_eci_cmaes",
     "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_lml_grad_batch", "lb_lml_grad_batch_dev", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
     "lb_nb_samples", "lb_strerror", "lb_last_cuda_error", "lb_spgp_create", "lb_spgp_destroy", "lb_spgp_set_data", "lb_spgp_lik",
-    "lb_spgp_compute", "lb_spgp_query", "lb_spgp_acq_argmax", "lb_spgp_query_grad", "lb_spgp_acq_grad", "lb_spgp_launch_count",
+    "lb_spgp_compute", "lb_spgp_query", "lb_spgp_query_dev", "lb_spgp_acq_argmax", "lb_spgp_acq_argmax_dev", "lb_spgp_acq_cmaes",
+    "lb_spgp_query_grad", "lb_spgp_acq_grad", "lb_spgp_launch_count",
 ]
 
 _lib = None
@@ -106,6 +107,7 @@ def load() -> C.CDLL:
         "lb_ehvi3d_argmax_dev": ([p, p, p, dp, i64, dp, i64, dp, dp, dbl, dp, dbl, dp, dbl, dp, dp, dp], i32),
         "lb_acq_cmaes": ([p, i32, dp, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
         "lb_ehvi_cmaes": ([p, p, p, dp, i64, dp, dbl, dbl, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
+        "lb_eci_cmaes": ([p, p, dp, dbl, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
         "lb_debug_cmaes_capture": ([i32], i32),
         "lb_debug_cmaes_trace": ([dp, C.c_longlong], C.c_longlong),
         "lb_eci_grad": ([p, p, dp, i64, dp, dp, dbl, dp, dp, dbl, dp, dp, dp], i32),
@@ -135,6 +137,9 @@ def load() -> C.CDLL:
         "lb_spgp_compute": ([p, i64, i64, dp, dbl], i32),
         "lb_spgp_query": ([p, i64, dp, i32, dp, dp], i32),
         "lb_spgp_acq_argmax": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
+        "lb_spgp_query_dev": ([p, i64, dp, i32, dp, dp], i32),
+        "lb_spgp_acq_argmax_dev": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
+        "lb_spgp_acq_cmaes": ([p, i32, dp, i32, dbl, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp], i32),
         "lb_spgp_query_grad": ([p, i64, dp, i32, dp, dp, dp, dp], i32),
         "lb_spgp_acq_grad": ([p, i32, dp, i64, dp, i32, dp, dbl, dp, dp, dp], i32),
         "lb_spgp_launch_count": ([p], C.c_longlong),

@@ -42,7 +42,8 @@ class UCB:
         return self._model.acq_grad_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], Xq)
 
     def cmaes_batch(self, starts, **opts):
-        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (model.GP.acq_cmaes_batch)"""
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (the model's acq_cmaes_batch:
+        model.GP or model.SPGP)"""
         return self._model.acq_cmaes_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], starts, **opts)
 
 
@@ -119,8 +120,8 @@ class EI(_Improvement):
         return self._model.acq_grad_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], Xq)
 
     def cmaes_batch(self, starts, **opts):
-        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (model.GP.acq_cmaes_batch); before
-        the model has samples every value is 0 and the first start is returned"""
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts (the model's acq_cmaes_batch:
+        model.GP or model.SPGP); before the model has samples every value is 0 and the first start is returned"""
         starts = np.atleast_2d(starts)
         if len(self._model.samples()) < 1:
             return np.array(starts[0], dtype=np.float64), 0.0, 0
@@ -130,7 +131,8 @@ class EI(_Improvement):
 
 class ECI(_Improvement):
     """Expected constrained improvement (experimental/acqui/eci.hpp): EI on `model` weighted by the probability Pf that the first
-    output of `constraint_model` exceeds 1.  Pf = 1 when the constraint model has no samples or is None."""
+    output of `constraint_model` exceeds 1.  Pf = 1 when the constraint model has no samples or is None.  Both models are
+    model.GP; argmax_batch, grad_batch and cmaes_batch each run in one device call over both."""
 
     def __init__(self, model, constraint_model, iteration: int = 0, params=None):
         super().__init__(model, params)
@@ -178,6 +180,15 @@ class ECI(_Improvement):
         self._update_f_max(first_elem)
         return self._model.eci_grad_batch(self._constraint_model, self._f_max, self._jitter(), Xq)
 
+    def cmaes_batch(self, starts, **opts):
+        """(best_x, best_val, n_evals) of a batched CMA-ES on the device from each row of starts, over both models
+        (model.GP.eci_cmaes_batch); before the objective has samples every value is 0 and the first start is returned"""
+        starts = np.atleast_2d(starts)
+        if len(self._model.samples()) < 1:
+            return np.array(starts[0], dtype=np.float64), 0.0, 0
+        self._update_f_max(first_elem)
+        return self._model.eci_cmaes_batch(self._constraint_model, self._f_max, self._jitter(), starts, **opts)
+
 
 class EHVI:
     """Expected hypervolume improvement over two or three objectives (experimental/acqui/ehvi.hpp): `models` are the objectives'
@@ -185,7 +196,7 @@ class EHVI:
     the reference point (its first two (three) entries are used).  As in the reference, each model's sigma() (sigma^2 + noise) is
     passed where ehvi2d / ehvi3d_sliceupdate expect a standard deviation.  Every evaluation, the one-point __call__ included, runs
     on the device (lb_ehvi_argmax or lb_ehvi3d_argmax, and lb_ehvi_grad for two-objective gradients; three-objective gradients
-    raise NotImplementedError)."""
+    raise NotImplementedError).  cmaes_batch searches two or three objectives (lb_ehvi_cmaes); the models are model.GP."""
 
     def __init__(self, models, pop, ref_point, params=None):
         assert len(models) in (2, 3)  # ehvi.hpp:65 (two); three run ehvi3d_sliceupdate

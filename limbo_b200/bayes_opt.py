@@ -144,9 +144,11 @@ class BatchedCmaesSearch:
     """acquiopt<> policy: one random pass of `candidates` uniform points in [0,1]^D scored in one device pass, then one batched
     CMA-ES on the device (the acquisition's cmaes_batch, DESIGN.md §4.15) with one instance from each of the best `starts`
     distinct points: `lambda` offspring per instance (0: 4 + floor(3 ln D)), initial step `sigma`, at most `generations`
-    generations, an instance stopping when sigma sqrt(max diag C) < `tolx`.  Returns the better of the search's best point and the
-    random pass's (the random pass on ties); with an acquisition that has no cmaes_batch, or a model or mean the device search
-    does not take (model.MultiGP, a mean that depends on the input), the best point of the random pass."""
+    generations, an instance stopping when sigma sqrt(max diag C) < `tolx`.  The search takes UCB / GP_UCB / EI over model.GP and
+    model.SPGP, ECI over an objective and a constraint model.GP, and two- and three-objective EHVI over model.GP.  Returns the
+    better of the search's best point and the random pass's (the random pass on ties); with an acquisition that has no
+    cmaes_batch, or a model or mean the device search does not take (model.MultiGP, an SPGP before its first compute, a mean that
+    depends on the input), the best point of the random pass."""
 
     def __init__(self, params=None, rng: np.random.Generator | None = None):
         self._params = params

@@ -1545,7 +1545,7 @@ int lb_ehvi3d_argmax_dev(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, cons
         mean1_const, dMean2_at_q, mean2_const, dAcq_out, dBest_val, dBest_idx);
 }
 
-// ---- batched CMA-ES (lb_acq_cmaes, lb_ehvi_cmaes; cmaes.cu) -----------------------------------------------------------------------
+// ---- batched CMA-ES (lb_acq_cmaes, lb_eci_cmaes, lb_ehvi_cmaes; lb_spgp_acq_cmaes in spgp.cu; cmaes.cu) -----------------------------
 
 // Testing hook: with capture on, each search on the calling thread keeps the instances' states after every generation (R x
 // lb_cmaes_state_doubles(D) doubles each), then the last generation's R lambda x D candidates and R lambda values.
@@ -1566,19 +1566,17 @@ extern "C" long long lb_debug_cmaes_trace(double* dst, long long n)
 }
 
 extern "C++" {
-// The search loop on h's stream (h: the handle whose stream, pool and launch count the search uses; every handle the scoring reads
-// is locked by the caller).  prepare(M) runs once before the first generation; per generation the ask kernel writes the R lambda
-// candidates to the device, score(dCand, M, dVals, dBestVal, dBestIdx) enqueues the scorer of the _dev entry points on them, and
-// the tell kernel updates every live instance.  Each reduced-precision handle in `scored` clears and sets its timeout flag in
-// every fill, so after each generation the flags are ORed into one word of the search: a timeout in any generation makes the
-// search return LB_ERR_TIMEOUT.  After every 8th generation the host reads that word and the number of live instances, and stops
-// when none is left.  The best point over the instances (ties to the lower instance) and the candidates scored come back on the
-// host.
-template <typename Prepare, typename Score>
-static int cmaes_search(lb_gp_full* h, std::array<lb_gp_full*, 3> scored, const lb_cmaes_opts* opts, int64_t R, const double* starts,
-    Prepare&& prepare, Score&& score, double* best_x, double* best_val, int64_t* n_evals)
+// The search loop of every device CMA-ES (common.cuh).  prepare(M) runs once before the first generation; per generation the ask
+// kernel writes the R lambda candidates to the device, score(dCand, M, dVals, dBestVal, dBestIdx) enqueues the scorer of the _dev
+// entry points on them, and the tell kernel updates every live instance.  Each reduced-precision handle clears and sets its
+// timeout word in every fill, so after each generation the words in on.timeouts are ORed into one word of the search: a timeout
+// in any generation makes the search return LB_ERR_TIMEOUT.  After every 8th generation the host reads that word and the number
+// of live instances, and stops when none is left.  The best point over the instances (ties to the lower instance) and the
+// candidates scored come back on the host.
+int lb_cmaes_search(const LbCmaesHost& on, const lb_cmaes_opts* opts, int64_t R, const double* starts, const LbCmaesPrepare& prepare,
+    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals)
 {
-    const int D = h->D;
+    const int D = on.D;
     LbCmaes s{};
     std::vector<double> w;
     int rc = lb_cmaes_setup(*opts, D, (int)R, &s, &w);
@@ -1586,8 +1584,8 @@ static int cmaes_search(lb_gp_full* h, std::array<lb_gp_full*, 3> scored, const 
     const int64_t S = lb_cmaes_state_doubles(D), M = R * s.lam;
     std::vector<double> hs((size_t)(R * S));
     for (int64_t r = 0; r < R; ++r) lb_cmaes_init_state(s, opts->sigma0, starts + r * D, hs.data() + r * S);
-    cudaStream_t st = h->stream;
-    StreamTemps tmp(h->device, st);
+    cudaStream_t st = on.stream;
+    StreamTemps tmp(on.device, st);
     double *dW = nullptr, *dVals = nullptr, *dBV = nullptr;
     long long* dBI = nullptr;
     int* dLive = nullptr; // [0] live instances, [1] a reduced-precision timeout in some generation
@@ -1605,14 +1603,12 @@ static int cmaes_search(lb_gp_full* h, std::array<lb_gp_full*, 3> scored, const 
     if ((rc = prepare(M))) return rc;
     int g = 0;
     while (g < opts->generations) {
-        if ((rc = lb_launch_cmaes_ask(st, s, g, &h->launches)) || (rc = score(s.cand, M, dVals, dBV, dBI))) return rc;
-        for (lb_gp_full* q : scored) // the scoring of every handle is ordered before this point of h's stream
-            if (q && q->precision != LB_PREC_FP64 && q->N > 0 && q->ex.ws.dErr
-                && (rc = lb_launch_cmaes_flag(st, q->ex.ws.dErr.get(), dLive + 1, &h->launches)))
-                return rc;
+        if ((rc = lb_launch_cmaes_ask(st, s, g, on.launches)) || (rc = score(s.cand, M, dVals, dBV, dBI))) return rc;
+        for (const DevBuf<int>* e : on.timeouts) // the scoring of every handle is ordered before this point of the stream
+            if (e && *e && (rc = lb_launch_cmaes_flag(st, e->get(), dLive + 1, on.launches))) return rc;
         const bool count = (g + 1) % 8 == 0 && g + 1 < opts->generations;
         if (count) LB_CUDA(cudaMemsetAsync(dLive, 0, sizeof(int), st));
-        if ((rc = lb_launch_cmaes_tell(st, s, g, dVals, count ? dLive : nullptr, &h->launches))) return rc;
+        if ((rc = lb_launch_cmaes_tell(st, s, g, dVals, count ? dLive : nullptr, on.launches))) return rc;
         ++g;
         if (capture) {
             LB_CUDA(cudaMemcpyAsync(hs.data(), s.state, sizeof(double) * hs.size(), cudaMemcpyDeviceToHost, st));
@@ -1648,10 +1644,9 @@ static int cmaes_search(lb_gp_full* h, std::array<lb_gp_full*, 3> scored, const 
     LB_CUDA(cudaGetLastError());
     return LB_OK;
 }
-} // extern "C++"
 
-// the checks lb_acq_cmaes and lb_ehvi_cmaes share before any lock: pointers, R and finite starts (D columns)
-static int cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts, int D, const double* best_x, const double* best_val,
+// the checks every device CMA-ES entry point makes before any lock: pointers, R and finite starts (D columns)
+int lb_cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts, int D, const double* best_x, const double* best_val,
     const int64_t* n_evals)
 {
     if (!opts || !starts || !best_x || !best_val || !n_evals || R <= 0 || R > (int64_t)INT32_MAX) return LB_ERR_ARG;
@@ -1661,19 +1656,33 @@ static int cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts
     return LB_OK;
 }
 
+// the search runs on h's stream, pool and launch count and reads the timeout words of the reduced-precision handles it scores
+static LbCmaesHost cmaes_host(lb_gp_full* h, std::array<lb_gp_full*, 3> scored)
+{
+    LbCmaesHost on{h->device, h->stream, h->D, &h->launches, {nullptr, nullptr, nullptr}};
+    for (int i = 0; i < 3; ++i) {
+        lb_gp_full* q = scored[(size_t)i];
+        if (q && q->precision != LB_PREC_FP64 && q->N > 0) on.timeouts[(size_t)i] = &q->ex.ws.dErr; // N == 0: the prior, no word
+    }
+    return on;
+}
+
+static int cmaes_no_prepare(int64_t) { return LB_OK; }
+} // extern "C++"
+
 int lb_acq_cmaes(const lb_gp* hc, int acq_id, const double* acq_params, double mean_const, const lb_cmaes_opts* opts, int64_t R,
     const double* starts, double* best_x, double* best_val, int64_t* n_evals)
 {
     if (!hc || !acq_params) return LB_ERR_ARG;
     if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
     lb_gp_full* h = full(hc);
-    int rc = cmaes_args(opts, R, starts, h->D, best_x, best_val, n_evals);
+    int rc = lb_cmaes_args(opts, R, starts, h->D, best_x, best_val, n_evals);
     if (rc) return rc;
     if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
     LB_DEVICE(h);
     std::lock_guard<std::mutex> lock(h->ex.qmutex); // the model stays the same for the whole search
-    return cmaes_search(
-        h, {h, nullptr, nullptr}, opts, R, starts, [](int64_t) { return LB_OK; },
+    return lb_cmaes_search(
+        cmaes_host(h, {h, nullptr, nullptr}), opts, R, starts, cmaes_no_prepare,
         [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
             return query_common(h, M, dCand, true, nullptr, nullptr, true, acq_id, acq_params, nullptr, mean_const, dVals, dBV,
                 (int64_t*)dBI, true, true);
@@ -1681,12 +1690,44 @@ int lb_acq_cmaes(const lb_gp* hc, int acq_id, const double* acq_params, double m
         best_x, best_val, n_evals);
 }
 
+int lb_eci_cmaes(const lb_gp* obj, const lb_gp* con, const double* eci_params, double obj_mean_const, double con_mean_const,
+    const lb_cmaes_opts* opts, int64_t R, const double* starts, double* best_x, double* best_val, int64_t* n_evals)
+{
+    if (!obj || obj == con || !eci_params) return LB_ERR_ARG;
+    if (con && con->device != obj->device) return LB_ERR_ARG;
+    int rc = lb_cmaes_args(opts, R, starts, obj->D, best_x, best_val, n_evals);
+    if (rc) return rc;
+    lb_gp_full* o = full(obj);
+    lb_gp_full* c = con ? full(con) : nullptr;
+    LB_DEVICE(o);
+    return with_query_locks(o, c, [&] { // both models stay the same for the whole search
+        if (o->D <= 0) return LB_ERR_STATE;
+        if (o->N == 0) { // eci.hpp:86: every value is 0, so the first start wins and nothing is scored
+            std::memcpy(best_x, starts, sizeof(double) * o->D);
+            *best_val = 0.0;
+            *n_evals = 0;
+            return LB_OK;
+        }
+        if (!o->kernel_set) return LB_ERR_STATE;
+        const bool use_con = c && c->N > 0; // eci_locked's rules: Pf = 1 without constraint samples
+        if (use_con && c->D != o->D) return LB_ERR_ARG;
+        if (use_con && !c->kernel_set) return LB_ERR_STATE;
+        return lb_cmaes_search(
+            cmaes_host(o, {o, use_con ? c : nullptr, nullptr}), opts, R, starts, cmaes_no_prepare,
+            [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
+                return eci_locked(o, c, eci_params[0], eci_params[1], M, dCand, true, nullptr, obj_mean_const, nullptr, con_mean_const,
+                    dVals, dBV, (int64_t*)dBI);
+            },
+            best_x, best_val, n_evals);
+    });
+}
+
 int lb_ehvi_cmaes(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, const double* ref_point, int64_t k, const double* front,
     double mean0_const, double mean1_const, double mean2_const, const lb_cmaes_opts* opts, int64_t R, const double* starts,
     double* best_x, double* best_val, int64_t* n_evals)
 {
     if (!m0) return LB_ERR_ARG;
-    int rc = cmaes_args(opts, R, starts, m0->D, best_x, best_val, n_evals);
+    int rc = lb_cmaes_args(opts, R, starts, m0->D, best_x, best_val, n_evals);
     if (rc) return rc;
     std::vector<double> sorted;
     if ((rc = ehvi_front(m0, m1, m2, ref_point, k, front, 1, starts, &sorted))) return rc;
@@ -1706,7 +1747,7 @@ int lb_ehvi_cmaes(const lb_gp* m0, const lb_gp* m1, const lb_gp* m2, const doubl
                              : ehvi_score(a, b, ref_point, k, M, dMeans, mean0_const, mean1_const, dAcq, dB, dI);
                 });
         };
-        return cmaes_search(a, {a, b, c}, opts, R, starts, prepare, score, best_x, best_val, n_evals);
+        return lb_cmaes_search(cmaes_host(a, {a, b, c}), opts, R, starts, prepare, score, best_x, best_val, n_evals);
     };
     if (c) {
         std::scoped_lock lock(a->ex.qmutex, b->ex.qmutex, c->ex.qmutex); // deadlock-free whatever order other callers pass them in

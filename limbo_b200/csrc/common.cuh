@@ -14,9 +14,11 @@
 //     every triangular solve.
 #pragma once
 #include <cuda_runtime.h>
+#include <array>
 #include <cfloat>
 #include <cstdint>
 #include <cstdio>
+#include <functional>
 #include <vector>
 
 #define LB_TILE 128
@@ -743,7 +745,7 @@ size_t lb_ehvi3d_ws_doubles(int64_t k, int64_t M);
 int lb_launch_ehvi3d_front(cudaStream_t st, const double* r, int64_t k, const double* dFront, double* dWs, long long* launches);
 int lb_launch_ehvi3d_cells(cudaStream_t st, const double* r, int64_t k, const double* dFront, int64_t M, const LbEhvi3Model& m0,
     const LbEhvi3Model& m1, const LbEhvi3Model& m2, double* dWs, double* dAcq, long long* launches);
-// cmaes.cu: the batched CMA-ES of lb_acq_cmaes / lb_ehvi_cmaes (DESIGN.md §4.15).  Per instance, the device state is
+// cmaes.cu: the batched CMA-ES of lb_acq_cmaes / lb_eci_cmaes / lb_ehvi_cmaes / lb_spgp_acq_cmaes (DESIGN.md §4.15).  Per instance, the device state is
 // lb_cmaes_state_doubles(D) doubles: m, p_sigma, p_c, best_x (D each), C and A (D x D row-major each; A lower), then sigma,
 // best_val and the stop flag.
 #define LB_CMAES_MAX_D 64
@@ -771,6 +773,25 @@ int lb_launch_cmaes_ask(cudaStream_t st, const LbCmaes& s, int g, long long* lau
 int lb_launch_cmaes_flag(cudaStream_t st, const int* dErr, int* dFlag, long long* launches);
 // generation g's update from the R x lam values dVals; dLive (NULL: not counted) gains the instances still live after it
 int lb_launch_cmaes_tell(cudaStream_t st, const LbCmaes& s, int g, const double* dVals, int* dLive, long long* launches);
+// abi.cu: the search loop that every device CMA-ES entry point drives with its own scorer.  What it needs of the model: the
+// device and stream it runs on (its pool leases are returned when the search ends), D, the launch counter its kernels add to, and
+// the reduced-precision timeout word of each scored handle (NULL: none; fp64 scorers have none), read after every scoring since
+// the first fill may allocate it.  The caller holds every lock the scorer needs for the whole search.
+struct LbCmaesHost {
+    int device;
+    cudaStream_t stream;
+    int D;
+    long long* launches;
+    std::array<const DevBuf<int>*, 3> timeouts;
+};
+using LbCmaesPrepare = std::function<int(int64_t M)>; // once, before the first generation
+// enqueues the values of the M device candidates dCand into dVals and their argmax into dBestVal / dBestIdx, on the search's stream
+using LbCmaesScore = std::function<int(const double* dCand, int64_t M, double* dVals, double* dBestVal, long long* dBestIdx)>;
+int lb_cmaes_search(const LbCmaesHost& on, const lb_cmaes_opts* opts, int64_t R, const double* starts, const LbCmaesPrepare& prepare,
+    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals);
+// the checks every entry point makes before any lock: pointers, 0 < R <= INT32_MAX and finite starts (R x D)
+int lb_cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts, int D, const double* best_x, const double* best_val,
+    const int64_t* n_evals);
 // sparsify.cu
 int lb_run_sparsify(const lb_gp* h, cudaStream_t st, int64_t N, int D, const double* dX, int64_t max_points, long long* dKept,
     int64_t* n_kept, long long* dRemoved, double* dRemovedScore, long long* launches);

@@ -3,7 +3,8 @@
 //
 //   _likelihood / _likelihood_wp  spgp.hpp:446-580  -> lb_spgp_lik
 //   _compute(false)               spgp.hpp:389-407  -> lb_spgp_compute
-//   _predict                      spgp.hpp:582-610  -> lb_spgp_query / lb_spgp_acq_argmax
+//   _predict                      spgp.hpp:582-610  -> lb_spgp_query / lb_spgp_acq_argmax (and their _dev variants)
+//   a device CMA-ES over UCB / EI (not in the reference) -> lb_spgp_acq_cmaes
 //   its candidate gradient        (not in the reference) -> lb_spgp_query_grad / lb_spgp_acq_grad
 //
 // Every M x M factor and inverse reuses the GP path: Q = K(xb, xb) + del I and A = sig I + V~ V~^T are factorised by
@@ -553,7 +554,7 @@ struct lb_spgp {
     bool b1_ready = false; // Mv row 6 holds b1 = L^-T Lm^-T bet of the current factors (candidate gradients)
     double c = 0, sig = 0;
     // query workspace
-    DevBuf<double> dQx, dQxt, dMu, dS2;
+    DevBuf<double> dQx, dQxt, dMu, dS2; // dQx: the host entry points' candidates
     DevBuf<double> dGrad; // candidate gradients: the mean's input gradient, grad mu, grad sigma^2, the acquisition's, Mq x D each
     ArgmaxWs am; // acquisition values, means, argmax records
 };
@@ -807,10 +808,10 @@ int likelihood(lb_spgp* s, int M, const double* w, double jitter, double* f, dou
     return LB_OK;
 }
 
-// mu - mean and sigma^2 of Mq candidates (device row-major dQx) into s->dMu.get() / s->dS2.get(), in chunks of QCHUNK; with grad,
-// also the candidate gradients of each chunk (b1 in Mv row 6, ensure_b1), whose outputs start at candidate 0.  The gradient
-// products take one more Mp x Cp block behind the forward workspace, whose layout they leave as it is.
-int predict(lb_spgp* s, int64_t Mq, int optimized, const LbGradOut* grad = nullptr)
+// mu - mean and sigma^2 of Mq candidates (device row-major dXq) into dMu / dS2 (Mq each), in chunks of QCHUNK; with grad, also
+// the candidate gradients of each chunk (b1 in Mv row 6, ensure_b1), whose outputs start at candidate 0.  The gradient products
+// take one more Mp x Cp block behind the forward workspace, whose layout they leave as it is.
+int predict(lb_spgp* s, int64_t Mq, const double* dXq, int optimized, double* dMu, double* dS2, const LbGradOut* grad = nullptr)
 {
     const int D = s->D;
     const int64_t Mp = s->Mp;
@@ -826,14 +827,14 @@ int predict(lb_spgp* s, int64_t Mq, int optimized, const LbGradOut* grad = nullp
     double* tb = sq2 + Cp; // gradients: Lm^-T lmst, then lst - sig Lm^-T lmst
     for (int64_t q0 = 0; q0 < Mq; q0 += QCHUNK) {
         const int64_t nq = std::min<int64_t>(QCHUNK, Mq - q0), nqp = round_up(nq, LB_TILE);
-        spgp_stage_kernel<<<dim3(nblocks(nqp, 256), D), 256, 0, s->st>>>(s->dQx.get() + q0 * D, nq, D, s->dSb.get(), s->dQxt.get(), nqp);
+        spgp_stage_kernel<<<dim3(nblocks(nqp, 256), D), 256, 0, s->st>>>(dXq + q0 * D, nq, D, s->dSb.get(), s->dQxt.get(), nqp);
         spgp_kmat_kernel<<<nblocks(Mp * nqp, 256), 256, 0, s->st>>>(s->dXbt.get(), Mp, s->M, s->dQxt.get(), nqp, nq, D, s->c, ks, Mp, nqp, 0, 0.0, nullptr);
         s->launches += 2;
         if ((rc = gemm<false, true>(s, s->q->dLinv.get(), Mp, ks, Mp, lst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
         if ((rc = gemm<false, true>(s, s->a->dLinv.get(), Mp, lst, Mp, lmst, Mp, Mp, nqp, Mp, 1, 0.0))) return rc;
-        spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lmst, Mp, nq, s->dMv.get(), s->dMu.get() + q0, sq2);
+        spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lmst, Mp, nq, s->dMv.get(), dMu + q0, sq2);
         spgp_coldot_kernel<<<nblocks(nq, 8), 256, 0, s->st>>>(lst, Mp, nq, nullptr, nullptr, sq1);
-        spgp_pred_kernel<<<nblocks(nq, 256), 256, 0, s->st>>>(sq1, sq2, nq, s->c, s->sig, optimized ? s->sig : 0.0, s->dS2.get() + q0);
+        spgp_pred_kernel<<<nblocks(nq, 256), 256, 0, s->st>>>(sq1, sq2, nq, s->c, s->sig, optimized ? s->sig : 0.0, dS2 + q0);
         s->launches += 3;
         LB_CUDA(cudaGetLastError());
         if (!grad) continue;
@@ -850,22 +851,40 @@ int predict(lb_spgp* s, int64_t Mq, int optimized, const LbGradOut* grad = nullp
         o.acq = grad->acq ? grad->acq + q0 : nullptr;
         o.grad = grad->grad ? grad->grad + q0 * D : nullptr;
         spgp_query_grad_kernel<<<(unsigned)nq, GRAD_THREADS, 0, s->st>>>(ks, lmst, Mp, s->M, s->dMv.get() + 6 * Mp, s->dXbt.get(),
-            s->dQxt.get(), nqp, s->dSb.get(), D, s->dMu.get() + q0, s->dS2.get() + q0, o);
+            s->dQxt.get(), nqp, s->dSb.get(), D, dMu + q0, dS2 + q0, o);
         s->launches++;
         LB_CUDA(cudaGetLastError());
     }
     return LB_OK;
 }
 
-int ensure_query(lb_spgp* s, int64_t Mq, const double* Xq)
+// the outputs and argmax records of Mq candidates
+int ensure_query_ws(lb_spgp* s, int64_t Mq)
 {
     const size_t mq = sizeof(double) * Mq;
     int rc;
     for (DevBuf<double>* b : {&s->dMu, &s->dS2, &s->am.vals, &s->am.mean})
         if ((rc = b->reserve(s->device, s->st, mq))) return rc;
-    if ((rc = s->dQx.reserve(s->device, s->st, mq * s->D)) || (rc = s->am.reserve(s->device, s->st, Mq))) return rc;
+    return s->am.reserve(s->device, s->st, Mq);
+}
+
+// ensure_query_ws and the upload of Mq host candidates to dQx
+int ensure_query(lb_spgp* s, int64_t Mq, const double* Xq)
+{
+    const size_t mq = sizeof(double) * Mq;
+    int rc;
+    if ((rc = ensure_query_ws(s, Mq)) || (rc = s->dQx.reserve(s->device, s->st, mq * s->D))) return rc;
     LB_CUDA(cudaMemcpyAsync(s->dQx.get(), Xq, mq * s->D, cudaMemcpyHostToDevice, s->st));
     return LB_OK;
+}
+
+// the fused UCB / EI and argmax of lb_spgp_acq_argmax over the Mq predictions in s->dMu / s->dS2 (dMean: device, NULL for none),
+// values into dAcq (NULL: not kept)
+int acq_score(lb_spgp* s, int acq_id, const double* acq_params, int64_t Mq, const double* dMean, double mean_const, double* dAcq,
+    double* dBestVal, long long* dBestIdx)
+{
+    return lb_launch_acq_full(s->st, acq_id, acq_params[0], acq_params[1], Mq, s->dMu.get(), 1, dMean, mean_const, s->dS2.get(), dAcq,
+        s->am.blk_val.get(), s->am.blk_idx.get(), dBestVal, dBestIdx, &s->launches);
 }
 
 // b1 = L^-T (Lm^-T bet) into Mv row 6 (row 5: Lm^-T bet), once per set of factors; the likelihood's own b1 (row 2) is not touched
@@ -915,7 +934,7 @@ int grad_common(lb_spgp* s, int64_t Mq, const double* Xq, int optimized, int acq
     out.ds2 = ds2_out ? g + 2 * md : nullptr;
     out.acq = acq_out ? s->am.vals.get() : nullptr;
     out.grad = grad_out ? g + 3 * md : nullptr;
-    if ((rc = ensure_b1(s)) || (rc = predict(s, Mq, optimized, &out))) return rc;
+    if ((rc = ensure_b1(s)) || (rc = predict(s, Mq, s->dQx.get(), optimized, s->dMu.get(), s->dS2.get(), &out))) return rc;
     const auto back = [&](double* dst, const double* src, size_t n) -> int {
         if (dst) LB_CUDA(cudaMemcpyAsync(dst, src, sizeof(double) * n, cudaMemcpyDeviceToHost, s->st));
         return LB_OK;
@@ -1035,7 +1054,7 @@ int lb_spgp_query(const lb_spgp* sc, int64_t Mq, const double* Xq_rowmajor, int 
     LB_DEVICE(s);
     int rc;
     if ((rc = ensure_query(s, Mq, Xq_rowmajor))) return rc;
-    if ((rc = predict(s, Mq, optimized))) return rc;
+    if ((rc = predict(s, Mq, s->dQx.get(), optimized, s->dMu.get(), s->dS2.get()))) return rc;
     LB_CUDA(cudaMemcpyAsync(mu_minus_mean, s->dMu.get(), sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
     LB_CUDA(cudaMemcpyAsync(sigma2, s->dS2.get(), sizeof(double) * Mq, cudaMemcpyDeviceToHost, s->st));
     LB_CUDA(cudaStreamSynchronize(s->st));
@@ -1053,17 +1072,61 @@ int lb_spgp_acq_argmax(const lb_spgp* sc, int acq_id, const double* acq_params, 
     LB_DEVICE(s);
     int rc;
     if ((rc = ensure_query(s, Mq, Xq_rowmajor))) return rc;
-    if ((rc = predict(s, Mq, optimized))) return rc;
+    if ((rc = predict(s, Mq, s->dQx.get(), optimized, s->dMu.get(), s->dS2.get()))) return rc;
     ArgmaxWs& am = s->am;
     const double* dMean = nullptr;
     if (mean_at_q) {
         LB_CUDA(cudaMemcpyAsync(am.mean.get(), mean_at_q, sizeof(double) * Mq, cudaMemcpyHostToDevice, s->st));
         dMean = am.mean.get();
     }
-    if ((rc = lb_launch_acq_full(s->st, acq_id, acq_params[0], acq_params[1], Mq, s->dMu.get(), 1, dMean, mean_const, s->dS2.get(),
-             am.vals.get(), am.blk_val.get(), am.blk_idx.get(), am.best_val.get(), am.best_idx.get(), &s->launches)))
-        return rc;
+    if ((rc = acq_score(s, acq_id, acq_params, Mq, dMean, mean_const, am.vals.get(), am.best_val.get(), am.best_idx.get()))) return rc;
     return am.read_best(s->st, best_val, best_idx, acq_out, Mq);
+}
+
+int lb_spgp_query_dev(const lb_spgp* sc, int64_t Mq, const double* dXq_rowmajor, int optimized, double* dMu_minus_mean, double* dSigma2)
+{
+    lb_spgp* s = const_cast<lb_spgp*>(sc);
+    if (!s || Mq < 0 || (Mq > 0 && (!dXq_rowmajor || !dMu_minus_mean || !dSigma2))) return LB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (!s->computed) return LB_ERR_STATE;
+    if (Mq == 0) return LB_OK;
+    LB_DEVICE(s);
+    return predict(s, Mq, dXq_rowmajor, optimized, dMu_minus_mean, dSigma2);
+}
+
+int lb_spgp_acq_argmax_dev(const lb_spgp* sc, int acq_id, const double* acq_params, int64_t Mq, const double* dXq_rowmajor, int optimized,
+    const double* dMean_at_q, double mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx)
+{
+    lb_spgp* s = const_cast<lb_spgp*>(sc);
+    if (!s || !acq_params || Mq < 1 || !dXq_rowmajor || !dBest_val || !dBest_idx) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
+    std::lock_guard<std::mutex> lk(s->mu);
+    if (!s->computed) return LB_ERR_STATE;
+    LB_DEVICE(s);
+    int rc;
+    if ((rc = ensure_query_ws(s, Mq)) || (rc = predict(s, Mq, dXq_rowmajor, optimized, s->dMu.get(), s->dS2.get()))) return rc;
+    return acq_score(s, acq_id, acq_params, Mq, dMean_at_q, mean_const, dAcq_out, dBest_val, (long long*)dBest_idx);
+}
+
+int lb_spgp_acq_cmaes(const lb_spgp* sc, int acq_id, const double* acq_params, int optimized, double mean_const, const lb_cmaes_opts* opts,
+    int64_t R, const double* starts_rowmajor, double* best_x, double* best_val, int64_t* n_evals)
+{
+    lb_spgp* s = const_cast<lb_spgp*>(sc);
+    if (!s || !acq_params) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
+    int rc = lb_cmaes_args(opts, R, starts_rowmajor, s->D, best_x, best_val, n_evals);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(s->mu); // the model stays the same for the whole search
+    if (!s->computed) return LB_ERR_STATE;
+    LB_DEVICE(s);
+    const LbCmaesHost on{s->device, s->st, s->D, &s->launches, {nullptr, nullptr, nullptr}}; // fp64 only: no timeout word
+    return lb_cmaes_search(
+        on, opts, R, starts_rowmajor, [&](int64_t M) { return ensure_query_ws(s, M); },
+        [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
+            int e = predict(s, M, dCand, optimized, s->dMu.get(), s->dS2.get());
+            return e ? e : acq_score(s, acq_id, acq_params, M, nullptr, mean_const, dVals, dBV, dBI);
+        },
+        best_x, best_val, n_evals);
 }
 
 int lb_spgp_query_grad(const lb_spgp* sc, int64_t Mq, const double* Xq_rowmajor, int optimized, double* mu_minus_mean, double* sigma2,

@@ -279,6 +279,24 @@ class GP:
         return cmaes(self._lib, "lb_ehvi_cmaes", D, self._h, models[1]._h, models[2]._h if K == 3 else None, ptr(r), F.shape[0],
                      ptr(F) if F.size else None, *consts, S, **opts)
 
+    def eci_cmaes_batch(self, constraint_model, f_max: float, jitter: float, starts, **opts):
+        """Batched CMA-ES on the device (lb_eci_cmaes) over the expected constrained improvement of eci_argmax_batch: this GP is the
+        objective, `constraint_model` a GP on the same device or None (a constraint without samples gives Pf = 1, as None does);
+        starts and opts as acq_cmaes_batch.  Without objective samples every value is 0: (the first start, 0.0, 0).  Returns
+        (best_x, best_val, n_evals); NotImplementedError for a mean of either model that depends on the input."""
+        S = candidates(starts)
+        D = S.shape[1]
+        mconst = constant_mean(self, D)
+        con_h, cconst = None, 0.0
+        if constraint_model is not None:
+            con_h = constraint_model._h
+            cconst = constant_mean(constraint_model, D)
+            if constraint_model.nb_samples() == 0:
+                cconst = 0.0
+        self._push_prior_if_empty(D)  # the search needs the input dimension even when it scores nothing
+        return cmaes(self._lib, "lb_eci_cmaes", D, self._h, con_h, ptr(np.array([f_max, jitter], dtype=np.float64)), mconst, cconst, S,
+                     **opts)
+
     def query_grad_batch(self, Xq):
         """mu (M x P), sigma^2 (M) and their gradients with respect to the candidates, grad mu (M x D, of the first output) and
         grad sigma^2 (M x D), in one device pass (lb_query_grad); the mean's value and input gradient are added.  Raises

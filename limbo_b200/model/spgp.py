@@ -20,7 +20,7 @@ from .. import kernel as _kernel
 from .. import mean as _mean
 from .. import opt as _opt
 from .. import params as _params
-from ._calls import acq_param_pair, argmax, candidates, first_mean, first_mean_and_grad, ptr, values_and_grads
+from ._calls import acq_param_pair, argmax, candidates, cmaes, constant_mean, first_mean, first_mean_and_grad, ptr, values_and_grads
 
 
 class SPGP:
@@ -230,6 +230,17 @@ class SPGP:
         mean0, mconst, mgrad = first_mean_and_grad(self, Xq)
         return values_and_grads(self._lib, "lb_spgp_acq_grad", M, D, self._h, acq_id, ptr(ap), M, ptr(Xq), int(self._optimized), ptr(mean0),
                                 mconst, ptr(mgrad))
+
+    def acq_cmaes_batch(self, acq_id: int, acq_params, starts, **opts):
+        """Batched CMA-ES on the device (lb_spgp_acq_cmaes) over UCB / GP_UCB (acq_id 0) or EI (acq_id 1), parameters as
+        acq_argmax_batch; starts, opts and returns as model.GP.acq_cmaes_batch.  NotImplementedError before the model is computed
+        (there is no device prior to search) and for a mean that depends on the input."""
+        S = candidates(starts)
+        mconst = constant_mean(self, S.shape[1])
+        if self._w is None:
+            raise NotImplementedError("the device CMA-ES needs a computed SPGP")
+        return cmaes(self._lib, "lb_spgp_acq_cmaes", S.shape[1], self._h, acq_id, ptr(acq_param_pair(acq_params)), int(self._optimized),
+                     mconst, S, **opts)
 
     def launch_count(self) -> int:
         return int(self._lib.lb_spgp_launch_count(self._h))
