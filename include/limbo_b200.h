@@ -128,6 +128,20 @@ int lb_acq_argmax(const lb_gp* h, int acq_id, const double* acq_params, int64_t 
 /* same, device pointers; d_best = {value, (double) index bit-copied as int64} */
 int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int64_t M, const double* dXq_rowmajor,
     const double* dMean_at_q, double mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
+/* lb_acq_argmax over each of the handle's q = P output columns from one query of the M candidates: ParEGO's q scalarisations of
+ * the objectives (experimental/model/gp_parego.hpp:103-117) share the factor, the candidates' K* and sigma^2, and column r is scored
+ * with its own acquisition (acq_params[2 r], acq_params[2 r + 1]: UCB / GP_UCB alpha and an unused slot, or EI f_max and jitter) and
+ * its own mean (mean_at_q: M x q row-major, or NULL to add mean_const[r] to column r).  acq_out (optional) receives the M x q
+ * row-major values; best_val[r] / best_idx[r] the best candidate of column r, ties to the lowest index.  With q = 1 every output
+ * is bit-identical to lb_acq_argmax's.  The lock, stream and path rules of lb_acq_argmax.  LB_ERR_ARG for a NULL argument, M <= 0
+ * or q other than the handle's P (1 for a handle without observations); LB_ERR_UNSUPPORTED for an unknown acq_id, a
+ * reduced-precision handle or q > LB_ACQ_MAX_COLS (the launch has one grid row per column). */
+#define LB_ACQ_MAX_COLS 65535
+int lb_acq_argmax_cols(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, int64_t M, const double* Xq_rowmajor,
+    const double* mean_at_q, const double* mean_const, double* acq_out, double* best_val, int64_t* best_idx);
+/* same, device pointers except acq_params and mean_const (host, q x 2 and q); bit-identical to lb_acq_argmax_cols */
+int lb_acq_argmax_cols_dev(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, int64_t M, const double* dXq_rowmajor,
+    const double* dMean_at_q, const double* mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx);
 
 /* Candidate gradients for M candidates (row-major M x D), extending lb_query with what the reference's gradient optimisers
  * (opt/gradient_ascent.hpp, opt/adam.hpp, opt/rprop.hpp) ask of f(x, gradient), which acqui/ucb.hpp:83-90 and acqui/ei.hpp:85-116
@@ -266,6 +280,15 @@ typedef struct lb_cmaes_opts {
  * LB_ERR_UNSUPPORTED for D > 64 or lambda > 256; LB_ERR_STATE for a handle without a kernel.  Synchronises h's stream. */
 int lb_acq_cmaes(const lb_gp* h, int acq_id, const double* acq_params, double mean_const, const lb_cmaes_opts* opts, int64_t R,
     const double* starts_rowmajor, double* best_x, double* best_val, int64_t* n_evals);
+/* lb_acq_cmaes over lb_acq_argmax_cols's q = P columns: instance r searches column cols[r] (R host ints), so one generation is
+ * one query of R lambda candidates, each scored in its instance's column with that column's parameters (acq_params, q x 2) and
+ * input-free mean (mean_const, q); every value is lb_acq_argmax_cols's in that column.  best_x (q x D row-major) and best_val (q)
+ * hold each column's best point over the instances bound to it (ties to the lower instance); n_evals counts every column.  With
+ * q = 1 and every cols[r] = 0 the result is bit-identical to lb_acq_cmaes's for the same options.  fp64 handles only
+ * (LB_ERR_UNSUPPORTED otherwise); LB_ERR_ARG for q other than the handle's P, a cols entry outside [0, q), a column without an
+ * instance, and lb_acq_cmaes's cases.  h is locked for the whole search; synchronises h's stream. */
+int lb_acq_cmaes_cols(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, const double* mean_const, const lb_cmaes_opts* opts,
+    int64_t R, const double* starts_rowmajor, const int* cols, double* best_x, double* best_val, int64_t* n_evals);
 /* two-objective (m2 NULL, lb_ehvi_argmax, k x 2 front) or three-objective (lb_ehvi3d_argmax, k x 3 front) EHVI with input-free
  * means; the argument and lock rules of those calls (every handle is locked for the whole search), and lb_acq_cmaes's.  The
  * three-objective front pass runs once per search. */

@@ -171,6 +171,30 @@ namespace limbo_b200 {
                     "lb_acq_argmax");
                 return std::make_pair(best, (long)idx);
             }
+            // acq_argmax in each of the dim_out output columns from one device query (lb_acq_argmax_cols): params holds dim_out x 2
+            // values (row r: column r's alpha and 0, or f_max and jitter), column r adds the mean's output r, and best[r] / idx[r]
+            // are column r's best value and candidate (ties to the lowest index); values (optional) receives the M x dim_out values,
+            // row-major.  ParEGO's q scalarisations (DESIGN.md §4.16) are a model with q columns.
+            void acq_argmax_cols(int acq_id, const std::vector<double>& params, const std::vector<Eigen::VectorXd>& vs, std::vector<double>& best,
+                std::vector<long>& idx, std::vector<double>* values = nullptr) const
+            {
+                const long M = (long)vs.size();
+                const int P = _dim_out > 0 ? _dim_out : 1;
+                assert((long)params.size() == 2L * P);
+                if (_samples.empty()) _push_prior((int)vs[0].size());
+                std::vector<double> xq = detail::pack_rows(vs), mean((size_t)M * P), zero((size_t)P, 0.0);
+                for (long i = 0; i < M; ++i) {
+                    const Eigen::VectorXd mv = _mean_function(vs[(size_t)i], *this);
+                    for (int p = 0; p < P; ++p) mean[(size_t)(i * P + p)] = mv(p);
+                }
+                std::vector<int64_t> bi((size_t)P);
+                best.resize((size_t)P);
+                if (values) values->resize((size_t)(M * P));
+                lb_check(lb_acq_argmax_cols(_h, acq_id, P, params.data(), M, xq.data(), mean.data(), zero.data(), values ? values->data() : nullptr,
+                             best.data(), bi.data()),
+                    "lb_acq_argmax_cols");
+                idx.assign(bi.begin(), bi.end());
+            }
             // UCB / EI values (M) and gradients (M x D) with the FirstElem aggregator in one device pass (lb_acq_grad): what the
             // reference's gradient optimisers ask of acqui::UCB / EI (ucb.hpp:83-90, ei.hpp:85-116 assert(!gradient) there)
             void acq_grad(int acq_id, double p0, double p1, const std::vector<Eigen::VectorXd>& vs, Eigen::VectorXd& values,

@@ -29,7 +29,7 @@ class CmaesOpts(C.Structure):
 DECLARED_SYMBOLS = [
     "lb_create", "lb_destroy", "lb_clone", "lb_set_stream", "lb_sync", "lb_launch_count", "lb_set_data",
     "lb_set_data_dev", "lb_set_kernel", "lb_fit", "lb_load_factor", "lb_refit_alpha", "lb_append", "lb_query", "lb_query_dev",
-    "lb_acq_argmax", "lb_acq_argmax_dev", "lb_query_grad", "lb_query_grad_dev", "lb_acq_grad", "lb_acq_grad_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_eci_grad", "lb_eci_grad_dev", "lb_ehvi_argmax", "lb_ehvi_argmax_dev",
+    "lb_acq_argmax", "lb_acq_argmax_dev", "lb_acq_argmax_cols", "lb_acq_argmax_cols_dev", "lb_acq_cmaes_cols", "lb_query_grad", "lb_query_grad_dev", "lb_acq_grad", "lb_acq_grad_dev", "lb_eci_argmax", "lb_eci_argmax_dev", "lb_eci_grad", "lb_eci_grad_dev", "lb_ehvi_argmax", "lb_ehvi_argmax_dev",
     "lb_ehvi3d_argmax", "lb_ehvi3d_argmax_dev", "lb_acq_cmaes", "lb_ehvi_cmaes", "lb_eci_cmaes",
     "lb_ehvi_grad", "lb_ehvi_grad_dev", "lb_pareto_set", "lb_pareto_set_dev", "lb_log_lik", "lb_kernel_grad_log_lik", "lb_lml_grad_batch", "lb_lml_grad_batch_dev", "lb_compute_inv_kernel", "lb_log_loo_cv",
     "lb_kernel_grad_log_loo_cv", "lb_kinv_obs_mean", "lb_get", "lb_sparsify", "lb_sparsify_dev",
@@ -95,6 +95,9 @@ def load() -> C.CDLL:
         "lb_query_dev": ([p, i64, dp, dp, dp], i32),
         "lb_acq_argmax": ([p, i32, dp, i64, dp, dp, dbl, dp, dp, dp], i32),
         "lb_acq_argmax_dev": ([p, i32, dp, i64, dp, dp, dbl, dp, dp, dp], i32),
+        "lb_acq_argmax_cols": ([p, i32, i64, dp, i64, dp, dp, dp, dp, dp, dp], i32),
+        "lb_acq_argmax_cols_dev": ([p, i32, i64, dp, i64, dp, dp, dp, dp, dp, dp], i32),
+        "lb_acq_cmaes_cols": ([p, i32, i64, dp, dp, C.POINTER(CmaesOpts), i64, dp, dp, dp, dp, dp], i32),
         "lb_query_grad": ([p, i64, dp, dp, dp, dp, dp], i32),
         "lb_query_grad_dev": ([p, i64, dp, dp, dp, dp, dp], i32),
         "lb_acq_grad": ([p, i32, dp, i64, dp, dp, dbl, dp, dp, dp], i32),

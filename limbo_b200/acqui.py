@@ -46,6 +46,19 @@ class UCB:
         model.GP or model.SPGP)"""
         return self._model.acq_cmaes_batch(_lib.ACQ_UCB, [self._alpha(), 0.0], starts, **opts)
 
+    def _col_params(self):
+        return [[self._alpha(), 0.0]] * self._model.dim_out()
+
+    def argmax_cols(self, Xq, return_values: bool = False):
+        """argmax_batch in each output column of the model from one device query (model.GP.acq_argmax_cols, e.g. the q columns of
+        model.GPParego): (best_values (q), best_indices (q)[, values (M x q)])"""
+        return self._model.acq_argmax_cols(_lib.ACQ_UCB, self._col_params(), Xq, return_values)
+
+    def cmaes_cols(self, starts, cols, **opts):
+        """(best_x (q x D), best_val (q), n_evals) of a batched CMA-ES on the device in which the instance from starts[i] searches
+        column cols[i] (model.GP.acq_cmaes_cols)"""
+        return self._model.acq_cmaes_cols(_lib.ACQ_UCB, self._col_params(), starts, cols, **opts)
+
 
 def _one_point_grad(acqui, v, afun):
     assert afun is first_elem
@@ -127,6 +140,31 @@ class EI(_Improvement):
             return np.array(starts[0], dtype=np.float64), 0.0, 0
         self._update_f_max(first_elem)
         return self._model.acq_cmaes_batch(_lib.ACQ_EI, [self._f_max, float(get(self._params, "acqui_ei", "jitter"))], starts, **opts)
+
+    def _col_params(self):
+        """per column: f_max = max_i mu_r(x_i) over the samples (ei.hpp:100-108 with the column's element), from one N-point query of
+        every column, and the jitter"""
+        mu, _ = self._model.query_batch(np.stack(self._model.samples(), axis=0))
+        jitter = float(get(self._params, "acqui_ei", "jitter"))
+        return [[float(f), jitter] for f in mu.max(axis=0)]
+
+    def argmax_cols(self, Xq, return_values: bool = False):
+        """argmax_batch in each output column of the model from one device query (UCB.argmax_cols); 0 everywhere, index 0, before
+        the model has samples"""
+        q = self._model.dim_out()
+        if len(self._model.samples()) < 1:
+            vals = np.zeros((len(Xq), q))
+            return (np.zeros(q), np.zeros(q, dtype=np.int64), vals) if return_values else (np.zeros(q), np.zeros(q, dtype=np.int64))
+        return self._model.acq_argmax_cols(_lib.ACQ_EI, self._col_params(), Xq, return_values)
+
+    def cmaes_cols(self, starts, cols, **opts):
+        """UCB.cmaes_cols over EI; before the model has samples every value is 0 and each column returns its first start"""
+        starts = np.atleast_2d(starts)
+        if len(self._model.samples()) < 1:
+            cols = np.asarray(cols)
+            q = self._model.dim_out()
+            return np.stack([starts[int(np.argmax(cols == r))] for r in range(q)]).astype(np.float64), np.zeros(q), 0
+        return self._model.acq_cmaes_cols(_lib.ACQ_EI, self._col_params(), starts, cols, **opts)
 
 
 class ECI(_Improvement):

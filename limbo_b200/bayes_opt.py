@@ -75,6 +75,13 @@ class BatchedRandomSearch:
                 best, x = b2, cand[i2].copy()
         return x
 
+    def propose_batch(self, acqui, dim: int, bounded: bool = True) -> np.ndarray:
+        """one point per output column of the acquisition's model (q x D): the column's best of `candidates` uniform points, all
+        scored in one device query (the acquisition's argmax_cols); no refinement rounds"""
+        cand = self._rng.random((int(_get(self._params, "opt_batchedrandom", "candidates")), dim))
+        _, idx = acqui.argmax_cols(cand)
+        return cand[np.asarray(idx)].copy()
+
 
 def _best_distinct(cand, vals, n: int) -> np.ndarray:
     """the (at most) n best distinct rows of cand by vals, descending, NaN last"""
@@ -139,6 +146,9 @@ class BatchedGradientSearch:
             b2_t *= self.B2
         return x_best
 
+    def propose_batch(self, acqui, dim: int, bounded: bool = True) -> np.ndarray:
+        raise NotImplementedError("candidate gradients cover the first output column only")
+
 
 class BatchedCmaesSearch:
     """acquiopt<> policy: one random pass of `candidates` uniform points in [0,1]^D scored in one device pass, then one batched
@@ -172,6 +182,38 @@ class BatchedCmaesSearch:
         except (AttributeError, NotImplementedError):
             return x_best
         return np.asarray(x, dtype=np.float64) if v > best else x_best
+
+    def propose_batch(self, acqui, dim: int, bounded: bool = True) -> np.ndarray:
+        """one point per output column of the acquisition's model (q x D): one random pass scored in every column at once
+        (argmax_cols), then one device CMA-ES (cmaes_cols) with max(1, starts // q) instances per column, started from that column's
+        best distinct points; per column the better of the search's point and the random pass's (the random pass on ties)"""
+        cand = self._rng.random((int(self._p("candidates")), dim))
+        best, idx, vals = acqui.argmax_cols(cand, return_values=True)
+        x_best = cand[np.asarray(idx)].copy()
+        q = x_best.shape[0]
+        per = max(1, int(self._p("starts")) // q)
+        starts, cols = [], []
+        for r in range(q):
+            s = _best_distinct(cand, vals[:, r], per)
+            starts.append(s)
+            cols += [r] * s.shape[0]
+        x, v, _ = acqui.cmaes_cols(np.concatenate(starts), cols, lam=int(self._p("lambda")), sigma0=float(self._p("sigma")),
+                                   generations=int(self._p("generations")), tolx=float(self._p("tolx")),
+                                   seed=int(self._rng.integers(0, 2**63 - 1)), bounded=bounded)
+        better = np.asarray(v) > np.asarray(best)
+        x_best[better] = np.asarray(x, dtype=np.float64)[better]
+        return x_best
+
+
+def distinct_rows(X) -> np.ndarray:
+    """the rows of X without any row equal to an earlier one, in order"""
+    seen, keep = set(), []
+    for i, x in enumerate(np.asarray(X, dtype=np.float64)):
+        key = x.tobytes()
+        if key not in seen:
+            seen.add(key)
+            keep.append(i)
+    return np.asarray(X, dtype=np.float64)[keep]
 
 
 class BOptimizer:
@@ -399,3 +441,55 @@ class Ehvi(BoMulti):
             self.eval_and_add(sfun, x)
             self._current_iteration += 1
             self._total_iterations += 1
+
+
+class Parego(BOptimizer):
+    """ParEGO, mirroring experimental::bayes_opt::Parego (src/limbo/experimental/bayes_opt/parego.hpp:73-86): BOptimizer over a
+    model.GPParego that scalarises the K objectives with random weights (kernel and mean as given, Matern-5/2 and mean::Data by
+    default), with a single-output acquisition (UCB by default) and FirstElem.  best_observation() ranks the raw observations, as
+    the reference does.
+
+    With q = 1 it is BOptimizer over GPParego, and every acquisition optimiser works.  With q > 1 (qParEGO) the model holds q
+    scalarisations, each iteration proposes one point per column through the optimiser's propose_batch (BatchedRandomSearch: one
+    argmax_cols over its candidate set; BatchedCmaesSearch: cmaes_cols; BatchedGradientSearch raises NotImplementedError), a
+    proposal equal to an earlier column's is dropped, and each evaluated point is one iteration of stop_maxiterations, added with
+    its own add_sample (fresh weights each time).  DESIGN.md §4.16."""
+
+    def __init__(self, params=None, q: int = 1, kernel=None, mean=None, acqui=_acqui.UCB, acqui_opt=None,
+                 rng: np.random.Generator | None = None, device: int = 0, hp_opt=None):
+        from . import kernel as _kernel, mean as _mean
+        from .model import GPParego
+        rng = rng if rng is not None else np.random.default_rng()
+        model = GPParego(-1, int(q), params, kernel=kernel if kernel is not None else _kernel.MaternFiveHalves,
+                         mean=mean if mean is not None else _mean.Data, hp_opt=hp_opt, device=device, rng=rng)
+        super().__init__(model, params, acqui, acqui_opt, rng)
+        self._q = int(q)
+
+    def optimize(self, sfun, dim_in: int, afun=_acqui.first_elem, reset: bool = True) -> None:
+        if self._q == 1:
+            super().optimize(sfun, dim_in, afun, reset)
+            return
+        if reset:
+            self._samples, self._observations = [], []
+            self._current_iteration = 0
+        if self._total_iterations == 0 or reset:
+            for _ in range(int(_get(self._params, "init_randomsampling", "samples"))):
+                self.eval_and_add(sfun, self._rng.random(dim_in))
+        if self._observations:
+            self._model.compute(np.stack(self._samples), np.stack(self._observations))
+        hp_period = int(get(self._params, "bayes_opt_boptimizer", "hp_period"))
+        max_it = int(_get(self._params, "stop_maxiterations", "iterations"))
+        propose = getattr(self._acqui_opt, "propose_batch", None)
+        if propose is None:
+            raise NotImplementedError("the acquisition optimiser proposes one point per call; q > 1 needs propose_batch")
+        while self._current_iteration < max_it:
+            acqui = self._acqui_cls(self._model, self._current_iteration, params=self._params)
+            for x in distinct_rows(propose(acqui, dim_in, True)):
+                if self._current_iteration >= max_it:
+                    break
+                self.eval_and_add(sfun, x)
+                self._model.add_sample(self._samples[-1], self._observations[-1])
+                if hp_period > 0 and (self._current_iteration + 1) % hp_period == 0:
+                    self._model.optimize_hyperparams()
+                self._current_iteration += 1
+                self._total_iterations += 1

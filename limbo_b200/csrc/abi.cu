@@ -63,6 +63,7 @@ struct QueryWs { // per-handle query workspace (guarded by qmutex)
     DevBuf<double> dMu;    // M x P
     DevBuf<double> dS2;    // M
     ArgmaxWs am;           // acquisition values (M), host means uploaded (M), argmax records
+    DevBuf<double> dCols;  // lb_acq_argmax_cols: the q x 2 acquisition parameters, then the q mean constants
     DevBuf<double> dFront; // lb_ehvi_argmax: the front sorted by f[0] (k x 2); lb_ehvi3d_argmax: ehvi.cu's Front3 (9 k)
     DevBuf<double> dEhvi3; // lb_ehvi3d_argmax: the front pass's planes and the partial sums (lb_ehvi3d_ws_doubles; 271 MB at k = 256)
     DevBuf<double> dGrad;  // two-model gradients (lb_eci_grad, lb_ehvi_grad): grad mu (M x D), then grad sigma^2 (M x D)
@@ -993,9 +994,21 @@ static int query_timed_out(lb_gp_full* h)
     return herr ? LB_ERR_TIMEOUT : LB_OK;
 }
 
+// The per-column acquisition of lb_acq_argmax_cols / lb_acq_cmaes_cols (query.cu: acq_cols_kernel) over the handle's P columns:
+// acq_params holds P x 2 parameters, mean_at_q M x P means (or NULL), mean_const P constants, and best_val / best_idx P records.
+// dParams: the parameters then the constants on the device (3 P doubles), or NULL to upload acq_params and mean_const (host) into
+// the query workspace.  dInstCol (device, one column per CMA-ES instance of lam candidates): each candidate scored in its instance's
+// column only, M values and one record.
+struct AcqCols {
+    const double* mean_const;
+    const double* dParams;
+    const int* dInstCol;
+    int lam;
+};
+
 static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_dev, double* mu_out, double* s2_out,
     bool out_dev, int acq_id, const double* acq_params, const double* mean_at_q, double mean_const, double* acq_out,
-    double* best_val, int64_t* best_idx, bool with_acq, bool lock_held = false)
+    double* best_val, int64_t* best_idx, bool with_acq, bool lock_held = false, const AcqCols* cols = nullptr)
 {
     if (!hc || M < 0) return LB_ERR_ARG;
     if (M == 0) return LB_OK;
@@ -1030,25 +1043,39 @@ static int query_common(const lb_gp* hc, int64_t M, const double* Xq, bool xq_de
     if ((rc = query_fill(h, M, Xq, xq_dev))) return rc;
     if (!out_dev && (rc = query_timed_out(h))) return rc;
     if (with_acq) {
-        if ((rc = w.am.reserve(h->device, st, M))) return rc;
+        const int nrec = (cols && !cols->dInstCol) ? P : 1;
+        const int64_t nvals = M * nrec;
+        if ((rc = w.am.reserve(h->device, st, M, nrec))) return rc;
         const double* dMean = nullptr;
-        if ((rc = mean_on_device(h, st, mean_at_q, M, out_dev, &dMean))) return rc;
+        if ((rc = mean_on_device(h, st, mean_at_q, nvals, out_dev, &dMean))) return rc;
         double* dAcq = nullptr;
         if (acq_out) {
             if (out_dev) dAcq = acq_out;
             else {
-                if ((rc = ensure(h, w.am.vals, sizeof(double) * M))) return rc;
+                if ((rc = ensure(h, w.am.vals, sizeof(double) * nvals))) return rc;
                 dAcq = w.am.vals.get();
             }
         }
         double* dBV = out_dev ? best_val : w.am.best_val.get();
         long long* dBI = out_dev ? (long long*)best_idx : w.am.best_idx.get();
-        const double p0 = acq_params ? acq_params[0] : 0.0;
-        const double p1 = (acq_params && acq_id == LB_ACQ_EI) ? acq_params[1] : 0.0;
-        if ((rc = lb_launch_acq_full(st, acq_id, p0, p1, M, w.dMu.get(), P, dMean, mean_const, w.dS2.get(), dAcq, w.am.blk_val.get(),
-                 w.am.blk_idx.get(), dBV, dBI, &h->launches)))
-            return rc;
-        if (!out_dev && (rc = w.am.read_best(st, best_val, best_idx, acq_out, M))) return rc;
+        if (cols) {
+            const double* dParams = cols->dParams;
+            if (!dParams) {
+                if ((rc = ensure(h, w.dCols, sizeof(double) * 3 * P))) return rc;
+                LB_CUDA(cudaMemcpyAsync(w.dCols.get(), acq_params, sizeof(double) * 2 * P, cudaMemcpyHostToDevice, st));
+                LB_CUDA(cudaMemcpyAsync(w.dCols.get() + 2 * P, cols->mean_const, sizeof(double) * P, cudaMemcpyHostToDevice, st));
+                dParams = w.dCols.get();
+            }
+            rc = lb_launch_acq_cols(st, acq_id, dParams, M, w.dMu.get(), P, dMean, dParams + 2 * P, w.dS2.get(), cols->dInstCol, cols->lam,
+                dAcq, w.am.blk_val.get(), w.am.blk_idx.get(), dBV, dBI, &h->launches);
+        } else {
+            const double p0 = acq_params ? acq_params[0] : 0.0;
+            const double p1 = (acq_params && acq_id == LB_ACQ_EI) ? acq_params[1] : 0.0;
+            rc = lb_launch_acq_full(st, acq_id, p0, p1, M, w.dMu.get(), P, dMean, mean_const, w.dS2.get(), dAcq, w.am.blk_val.get(),
+                w.am.blk_idx.get(), dBV, dBI, &h->launches);
+        }
+        if (rc) return rc;
+        if (!out_dev && (rc = w.am.read_best(st, best_val, best_idx, acq_out, nvals, nrec))) return rc;
     }
     if (mu_out) {
         LB_CUDA(cudaMemcpyAsync(mu_out, w.dMu.get(), sizeof(double) * M * P, out_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
@@ -1085,6 +1112,30 @@ int lb_acq_argmax_dev(const lb_gp* h, int acq_id, const double* acq_params, int6
     if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_UNSUPPORTED;
     return query_common(h, M, dXq, true, nullptr, nullptr, true, acq_id, acq_params, dMean_at_q, mean_const, dAcq_out,
         dBest_val, dBest_idx, true);
+}
+
+// lb_acq_argmax_cols and _dev: one query of the M candidates, scored in each of the handle's q = P columns
+static int acq_cols_common(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, int64_t M, const double* Xq, bool dev,
+    const double* mean_at_q, const double* mean_const, double* acq_out, double* best_val, int64_t* best_idx)
+{
+    if (!h || !best_val || !best_idx || !acq_params || !mean_const || M <= 0) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_UNSUPPORTED;
+    if (h->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
+    if (q != n_outputs(h)) return LB_ERR_ARG;
+    if (q > LB_ACQ_MAX_COLS) return LB_ERR_UNSUPPORTED; // one grid row per column
+    const AcqCols cols{mean_const, nullptr, nullptr, 0};
+    return query_common(h, M, Xq, dev, nullptr, nullptr, dev, acq_id, acq_params, mean_at_q, 0.0, acq_out, best_val, best_idx, true, false,
+        &cols);
+}
+int lb_acq_argmax_cols(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, int64_t M, const double* Xq, const double* mean_at_q,
+    const double* mean_const, double* acq_out, double* best_val, int64_t* best_idx)
+{
+    return acq_cols_common(h, acq_id, q, acq_params, M, Xq, false, mean_at_q, mean_const, acq_out, best_val, best_idx);
+}
+int lb_acq_argmax_cols_dev(const lb_gp* h, int acq_id, int64_t q, const double* acq_params, int64_t M, const double* dXq,
+    const double* dMean_at_q, const double* mean_const, double* dAcq_out, double* dBest_val, int64_t* dBest_idx)
+{
+    return acq_cols_common(h, acq_id, q, acq_params, M, dXq, true, dMean_at_q, mean_const, dAcq_out, dBest_val, dBest_idx);
 }
 
 // One handle's gradient pass on h->stream: mu (w.dMu, M x P), sigma^2 (w.dS2, M) and the outputs of `out`, whose pointers start at
@@ -1574,7 +1625,7 @@ extern "C++" {
 // of live instances, and stops when none is left.  The best point over the instances (ties to the lower instance) and the
 // candidates scored come back on the host.
 int lb_cmaes_search(const LbCmaesHost& on, const lb_cmaes_opts* opts, int64_t R, const double* starts, const LbCmaesPrepare& prepare,
-    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals)
+    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals, const int* cols, int q)
 {
     const int D = on.D;
     LbCmaes s{};
@@ -1634,12 +1685,17 @@ int lb_cmaes_search(const LbCmaesHost& on, const lb_cmaes_opts* opts, int64_t R,
     LB_CUDA(cudaMemcpyAsync(&timeout, dLive + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
     LB_CUDA(cudaStreamSynchronize(st));
     if (timeout) return LB_ERR_TIMEOUT;
-    // per instance: best_x at 3 D, best_val at 4 D + 2 D^2 + 1 (cmaes.cu's layout)
-    int64_t best = 0;
-    for (int64_t r = 1; r < R; ++r)
-        if (hs[(size_t)(r * S + S - 2)] > hs[(size_t)(best * S + S - 2)]) best = r;
-    std::memcpy(best_x, hs.data() + best * S + 3 * D, sizeof(double) * D);
-    *best_val = hs[(size_t)(best * S + S - 2)];
+    // per instance: best_x at 3 D, best_val at 4 D + 2 D^2 + 1 (cmaes.cu's layout); per column, the first instance bound to it
+    // unless a later one is strictly better
+    std::vector<int64_t> best((size_t)q, -1);
+    for (int64_t r = 0; r < R; ++r) {
+        int64_t& b = best[(size_t)(cols ? cols[r] : 0)];
+        if (b < 0 || hs[(size_t)(r * S + S - 2)] > hs[(size_t)(b * S + S - 2)]) b = r;
+    }
+    for (int c = 0; c < q; ++c) {
+        std::memcpy(best_x + (int64_t)c * D, hs.data() + best[(size_t)c] * S + 3 * D, sizeof(double) * D);
+        best_val[c] = hs[(size_t)(best[(size_t)c] * S + S - 2)];
+    }
     *n_evals = (int64_t)g * M;
     LB_CUDA(cudaGetLastError());
     return LB_OK;
@@ -1688,6 +1744,46 @@ int lb_acq_cmaes(const lb_gp* hc, int acq_id, const double* acq_params, double m
                 (int64_t*)dBI, true, true);
         },
         best_x, best_val, n_evals);
+}
+
+int lb_acq_cmaes_cols(const lb_gp* hc, int acq_id, int64_t q, const double* acq_params, const double* mean_const, const lb_cmaes_opts* opts,
+    int64_t R, const double* starts, const int* cols, double* best_x, double* best_val, int64_t* n_evals)
+{
+    if (!hc || !acq_params || !mean_const || !cols) return LB_ERR_ARG;
+    if (acq_id != LB_ACQ_UCB && acq_id != LB_ACQ_EI) return LB_ERR_ARG;
+    lb_gp_full* h = full(hc);
+    int rc = lb_cmaes_args(opts, R, starts, h->D, best_x, best_val, n_evals);
+    if (rc) return rc;
+    if (h->precision != LB_PREC_FP64) return LB_ERR_UNSUPPORTED;
+    if (q != n_outputs(h)) return LB_ERR_ARG;
+    std::vector<char> covered((size_t)q, 0);
+    for (int64_t r = 0; r < R; ++r) {
+        if (cols[r] < 0 || cols[r] >= q) return LB_ERR_ARG;
+        covered[(size_t)cols[r]] = 1;
+    }
+    if (std::find(covered.begin(), covered.end(), 0) != covered.end()) return LB_ERR_ARG; // every column needs an instance
+    if (h->D <= 0 || !h->kernel_set) return LB_ERR_STATE;
+    LB_DEVICE(h);
+    std::lock_guard<std::mutex> lock(h->ex.qmutex); // the model stays the same for the whole search
+    StreamTemps tmp(h->device, h->stream);
+    double* dParams = nullptr;
+    int* dInstCol = nullptr;
+    auto prepare = [&](int64_t) {
+        int rc = tmp.alloc(sizeof(double) * 3 * q, &dParams);
+        if (rc || (rc = tmp.alloc(sizeof(int) * R, &dInstCol))) return rc;
+        LB_CUDA(cudaMemcpyAsync(dParams, acq_params, sizeof(double) * 2 * q, cudaMemcpyHostToDevice, h->stream));
+        LB_CUDA(cudaMemcpyAsync(dParams + 2 * q, mean_const, sizeof(double) * q, cudaMemcpyHostToDevice, h->stream));
+        LB_CUDA(cudaMemcpyAsync(dInstCol, cols, sizeof(int) * R, cudaMemcpyHostToDevice, h->stream));
+        return LB_OK;
+    };
+    return lb_cmaes_search(
+        cmaes_host(h, {h, nullptr, nullptr}), opts, R, starts, prepare,
+        [&](const double* dCand, int64_t M, double* dVals, double* dBV, long long* dBI) {
+            const AcqCols c{nullptr, dParams, dInstCol, (int)(M / R)};
+            return query_common(h, M, dCand, true, nullptr, nullptr, true, acq_id, acq_params, nullptr, 0.0, dVals, dBV, (int64_t*)dBI, true,
+                true, &c);
+        },
+        best_x, best_val, n_evals, cols, (int)q);
 }
 
 int lb_eci_cmaes(const lb_gp* obj, const lb_gp* con, const double* eci_params, double obj_mean_const, double con_mean_const,

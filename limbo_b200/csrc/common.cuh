@@ -501,24 +501,24 @@ private:
 struct ArgmaxWs {
     DevBuf<double> vals, mean, blk_val, best_val;
     DevBuf<long long> blk_idx, best_idx;
-    int reserve(int device, cudaStream_t stream, int64_t M)
+    // records of `cols` columns (lb_launch_acq_cols): cols x ceil(M / 256) block records and cols final records
+    int reserve(int device, cudaStream_t stream, int64_t M, int cols = 1)
     {
-        const size_t nblk = (size_t)((M + 255) / 256);
+        const size_t nblk = (size_t)((M + 255) / 256) * (size_t)cols;
         int rc;
         if ((rc = blk_val.reserve(device, stream, sizeof(double) * nblk)) || (rc = blk_idx.reserve(device, stream, sizeof(long long) * nblk))
-            || (rc = best_val.reserve(device, stream, sizeof(double))) || (rc = best_idx.reserve(device, stream, sizeof(long long))))
+            || (rc = best_val.reserve(device, stream, sizeof(double) * cols)) || (rc = best_idx.reserve(device, stream, sizeof(long long) * cols)))
             return rc;
         return LB_OK;
     }
-    // the final record, and the M values when vals_out, to the host; synchronises the stream
-    int read_best(cudaStream_t stream, double* best, int64_t* idx, double* vals_out, int64_t M) const
+    // the `cols` final records, and the nvals values when vals_out, to the host; synchronises the stream
+    int read_best(cudaStream_t stream, double* best, int64_t* idx, double* vals_out, int64_t nvals, int cols = 1) const
     {
-        long long bi = 0;
-        if (vals_out) LB_CUDA(cudaMemcpyAsync(vals_out, vals.get(), sizeof(double) * M, cudaMemcpyDeviceToHost, stream));
-        LB_CUDA(cudaMemcpyAsync(best, best_val.get(), sizeof(double), cudaMemcpyDeviceToHost, stream));
-        LB_CUDA(cudaMemcpyAsync(&bi, best_idx.get(), sizeof(long long), cudaMemcpyDeviceToHost, stream));
+        static_assert(sizeof(long long) == sizeof(int64_t), "best_idx is copied as int64_t");
+        if (vals_out) LB_CUDA(cudaMemcpyAsync(vals_out, vals.get(), sizeof(double) * nvals, cudaMemcpyDeviceToHost, stream));
+        LB_CUDA(cudaMemcpyAsync(best, best_val.get(), sizeof(double) * cols, cudaMemcpyDeviceToHost, stream));
+        LB_CUDA(cudaMemcpyAsync(idx, best_idx.get(), sizeof(long long) * cols, cudaMemcpyDeviceToHost, stream));
         LB_CUDA(cudaStreamSynchronize(stream));
-        *idx = (int64_t)bi;
         return LB_OK;
     }
 };
@@ -668,6 +668,12 @@ int lb_launch_query(const lb_gp* h, cudaStream_t st, int64_t M, const double* dX
 int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_t M, const double* dMu, int mu_stride,
     const double* dMeanAtQ, double mean_const, const double* dS2, double* dAcq, double* dBlkVal, long long* dBlkIdx,
     double* dBestVal, long long* dBestIdx, long long* launches);
+// acq_full over the P columns of mu (query.cu: acq_cols_kernel): dParams (P x 2), dMeanAtQ (M x P) or dMeanConst (P) per column.  Without
+// dInstCol: the M x P values (dAcq, may be NULL) and one record per column (dBlkVal / dBlkIdx: P x ceil(M / 256); dBestVal / dBestIdx: P).
+// With dInstCol: candidate m scored in column dInstCol[m / lam] only, M values and one record over all of them.
+int lb_launch_acq_cols(cudaStream_t st, int acq_id, const double* dParams, int64_t M, const double* dMu, int P, const double* dMeanAtQ,
+    const double* dMeanConst, const double* dS2, const int* dInstCol, int lam, double* dAcq, double* dBlkVal, long long* dBlkIdx,
+    double* dBestVal, long long* dBestIdx, long long* launches);
 int lb_launch_eci_full(cudaStream_t st, double f_max, double jitter, int64_t M, const double* dMuObj, int p_obj, const double* dMeanObj,
     double mean_obj_const, const double* dS2Obj, const double* dMuCon, int p_con, const double* dMeanCon, double mean_con_const,
     const double* dS2Con, double* dAcq, double* dBlkVal, long long* dBlkIdx, double* dBestVal, long long* dBestIdx, long long* launches);
@@ -787,8 +793,10 @@ struct LbCmaesHost {
 using LbCmaesPrepare = std::function<int(int64_t M)>; // once, before the first generation
 // enqueues the values of the M device candidates dCand into dVals and their argmax into dBestVal / dBestIdx, on the search's stream
 using LbCmaesScore = std::function<int(const double* dCand, int64_t M, double* dVals, double* dBestVal, long long* dBestIdx)>;
+// With cols (R host ints in [0, q)), instance r is bound to column cols[r], and best_x (q x D) / best_val (q) hold each column's best
+// over its instances (ties to the lower instance); without, one best over all of them.
 int lb_cmaes_search(const LbCmaesHost& on, const lb_cmaes_opts* opts, int64_t R, const double* starts, const LbCmaesPrepare& prepare,
-    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals);
+    const LbCmaesScore& score, double* best_x, double* best_val, int64_t* n_evals, const int* cols = nullptr, int q = 1);
 // the checks every entry point makes before any lock: pointers, 0 < R <= INT32_MAX and finite starts (R x D)
 int lb_cmaes_args(const lb_cmaes_opts* opts, int64_t R, const double* starts, int D, const double* best_x, const double* best_val,
     const int64_t* n_evals);

@@ -166,6 +166,30 @@ acq_kernel(int acq_id, double p0, double p1, int64_t M, const double* __restrict
     block_argmax(v, idx, blk_val, blk_idx);
 }
 
+// acq_kernel over the P columns of one query (ParEGO's q scalarisations, DESIGN.md §4.16): column r has its own parameters
+// (params[2r], params[2r + 1]) and mean (mean_at_q[m * P + r], or mean_const[r]); sigma^2 is shared.  Without inst_col, grid.y = P and
+// CTA (x, r) scores column r into acq[m * P + r] and the block record (x, r) of blk_val / blk_idx (gridDim.x records per column).
+// With inst_col (grid.y = 1), candidate m belongs to CMA-ES instance m / lam and is scored in that instance's column inst_col[m / lam],
+// into acq[m].  The value is acq_kernel's expression, so a column is bit-identical to acq_kernel over that column.
+__global__ void __launch_bounds__(256)
+acq_cols_kernel(int acq_id, const double* __restrict__ params, int64_t M, const double* __restrict__ mu0, int P,
+    const double* __restrict__ mean_at_q, const double* __restrict__ mean_const, const double* __restrict__ s2, const int* __restrict__ inst_col,
+    int lam, double* __restrict__ acq, double* __restrict__ blk_val, long long* __restrict__ blk_idx)
+{
+    const int64_t m = blockIdx.x * (int64_t)256 + threadIdx.x;
+    double v = -DBL_MAX;
+    long long idx = LLONG_MAX;
+    if (m < M) {
+        const int r = inst_col ? inst_col[m / lam] : (int)blockIdx.y;
+        const double mu = mu0[m * P + r] + (mean_at_q ? mean_at_q[m * P + r] : mean_const[r]);
+        v = lb_acq_value(acq_id, mu, s2[m], params[2 * r], params[2 * r + 1]);
+        if (acq) acq[inst_col ? m : m * P + r] = v;
+        idx = m;
+    }
+    const int64_t rec = (int64_t)blockIdx.y * gridDim.x;
+    block_argmax(v, idx, blk_val + rec, blk_idx + rec);
+}
+
 // experimental/acqui/eci.hpp:76-130 per candidate, FirstElem aggregator: the objective's EI factor times the probability
 // that the constraint model's first output exceeds 1,
 //   Pf = Phi((mu_c - 1) / sigma_c), or 1 when sigma_c < 1e-10 or there is no constraint model (mu_con == nullptr).
@@ -261,12 +285,16 @@ values_argmax_kernel(int64_t M, const double* __restrict__ vals, double* __restr
     block_argmax(m < M ? vals[m] : -DBL_MAX, m < M ? (long long)m : LLONG_MAX, blk_val, blk_idx);
 }
 
+// one CTA per column (blockIdx.y): column c reduces the nblk records from c * nblk into best_val / best_idx[c]
 __global__ void __launch_bounds__(256)
 argmax_final_kernel(int nblk, const double* __restrict__ blk_val, const long long* __restrict__ blk_idx,
     double* __restrict__ best_val, long long* __restrict__ best_idx)
 {
     __shared__ double sv[256];
     __shared__ long long si[256];
+    const int64_t c = blockIdx.y;
+    blk_val += c * nblk;
+    blk_idx += c * nblk;
     double v = -DBL_MAX;
     long long idx = LLONG_MAX;
     for (int b = threadIdx.x; b < nblk; b += 256) {
@@ -289,8 +317,8 @@ argmax_final_kernel(int nblk, const double* __restrict__ blk_val, const long lon
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        *best_val = sv[0];
-        *best_idx = si[0];
+        best_val[c] = sv[0];
+        best_idx[c] = si[0];
     }
 }
 
@@ -360,6 +388,19 @@ int lb_launch_acq_full(cudaStream_t st, int acq_id, double p0, double p1, int64_
     const int nblk = (int)((M + 255) / 256);
     acq_kernel<<<nblk, 256, 0, st>>>(acq_id, p0, p1, M, dMu, mu_stride, dMeanAtQ, mean_const, dS2, dAcq, dBlkVal, dBlkIdx);
     argmax_final_kernel<<<1, 256, 0, st>>>(nblk, dBlkVal, dBlkIdx, dBestVal, dBestIdx);
+    if (launches) *launches += 2;
+    LB_CUDA(cudaGetLastError());
+    return LB_OK;
+}
+
+int lb_launch_acq_cols(cudaStream_t st, int acq_id, const double* dParams, int64_t M, const double* dMu, int P, const double* dMeanAtQ,
+    const double* dMeanConst, const double* dS2, const int* dInstCol, int lam, double* dAcq, double* dBlkVal, long long* dBlkIdx,
+    double* dBestVal, long long* dBestIdx, long long* launches)
+{
+    const int nblk = (int)((M + 255) / 256), cols = dInstCol ? 1 : P;
+    acq_cols_kernel<<<dim3((unsigned)nblk, (unsigned)cols), 256, 0, st>>>(acq_id, dParams, M, dMu, P, dMeanAtQ, dMeanConst, dS2, dInstCol,
+        lam, dAcq, dBlkVal, dBlkIdx);
+    argmax_final_kernel<<<dim3(1, (unsigned)cols), 256, 0, st>>>(nblk, dBlkVal, dBlkIdx, dBestVal, dBestIdx);
     if (launches) *launches += 2;
     LB_CUDA(cudaGetLastError());
     return LB_OK;

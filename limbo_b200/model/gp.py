@@ -204,6 +204,47 @@ class GP:
         mean0, mconst = first_mean(self, Xq)
         return argmax(self._lib, "lb_acq_argmax", M, return_values, self._h, acq_id, ptr(ap), M, ptr(Xq), ptr(mean0), mconst)
 
+    def acq_argmax_cols(self, acq_id: int, acq_params, Xq, return_values: bool = False):
+        """acq_argmax_batch in each of the P output columns from one query (lb_acq_argmax_cols): acq_params is P x 2 (row r: column r's
+        alpha and 0, or f_max and jitter), and column r adds the mean's output r.  Returns (best_values (P), best_indices (P)[,
+        values (M x P)])."""
+        Xq = candidates(Xq)
+        M = Xq.shape[0]
+        P = max(self._dim_out, 1)
+        ap = np.ascontiguousarray(np.asarray(acq_params, dtype=np.float64).reshape(P, 2))
+        self._push_prior_if_empty(Xq.shape[1])
+        mf = self._mean_function
+        if mf.is_constant():
+            mean, mconst = None, np.ascontiguousarray(np.asarray(mf(Xq[0], self), dtype=np.float64).reshape(P))
+        else:
+            mean, mconst = np.ascontiguousarray(np.asarray(mf.batch(Xq, self), dtype=np.float64).reshape(M, P)), np.zeros(P)
+        vals = np.empty((M, P)) if return_values else None
+        best, idx = np.empty(P), np.empty(P, dtype=np.int64)
+        _lib.check(self._lib.lb_acq_argmax_cols(self._h, acq_id, P, ptr(ap), M, ptr(Xq), ptr(mean), ptr(mconst), ptr(vals), ptr(best),
+                                                ptr(idx)), "lb_acq_argmax_cols")
+        return (best, idx, vals) if return_values else (best, idx)
+
+    def acq_cmaes_cols(self, acq_id: int, acq_params, starts, cols, lam: int = 0, sigma0: float = 0.5, generations: int = 100,
+                       tolx: float = 1e-12, seed: int = 0, bounded: bool = True):
+        """acq_cmaes_batch over the P columns of acq_argmax_cols (lb_acq_cmaes_cols): the instance started from starts[i] searches
+        column cols[i], and every column needs one.  Returns (best_x (P x D), best_val (P), n_evals); NotImplementedError for a mean
+        that depends on the input."""
+        S = candidates(starts)
+        D = S.shape[1]
+        P = max(self._dim_out, 1)
+        mf = self._mean_function
+        if not mf.is_constant():
+            raise NotImplementedError("the device CMA-ES takes input-free means only")
+        self._push_prior_if_empty(D)
+        mconst = np.ascontiguousarray(np.asarray(mf(np.zeros(D), self), dtype=np.float64).reshape(P))
+        ap = np.ascontiguousarray(np.asarray(acq_params, dtype=np.float64).reshape(P, 2))
+        c = np.ascontiguousarray(np.asarray(cols, dtype=np.int32).reshape(S.shape[0]))
+        opts = _lib.CmaesOpts(int(lam), float(sigma0), int(generations), float(tolx), int(seed) & 0xFFFFFFFFFFFFFFFF, int(bool(bounded)))
+        bx, bv, n = np.empty((P, D)), np.empty(P), C.c_int64()
+        _lib.check(self._lib.lb_acq_cmaes_cols(self._h, acq_id, P, ptr(ap), ptr(mconst), C.byref(opts), S.shape[0], ptr(S), ptr(c), ptr(bx),
+                                               ptr(bv), C.addressof(n)), "lb_acq_cmaes_cols")
+        return bx, bv, n.value
+
     def eci_argmax_batch(self, constraint_model, f_max: float, jitter: float, Xq, return_values: bool = False):
         """Fused batched expected constrained improvement + argmax on the device (experimental/acqui/eci.hpp:76-130, FirstElem
         aggregator): this GP is the objective, `constraint_model` (a GP on the same device, or None for no constraints) gives

@@ -61,6 +61,9 @@ class defaults:
         pred_kernel_sigma_sq = 0.5
         pred_kernel_l = 0.5
 
+    class model_gp_parego:  # experimental/model/gp_parego.hpp:62-66
+        rho = 0.05
+
     class bayes_opt_boptimizer:  # bayes_opt/boptimizer.hpp:68-72
         hp_period = -1
 
